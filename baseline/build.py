@@ -12,7 +12,7 @@ def build(force=False):
     if not force and os.path.exists(OUT) and os.path.getmtime(OUT) >= os.path.getmtime(SRC):
         return OUT
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
            "-shared", "-cudart", "shared", "-o", OUT, SRC]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:

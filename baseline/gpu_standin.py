@@ -2,7 +2,7 @@
 
 The reference's own GPU build cannot run here: its kernels live in xformers 0.0.22 / diff-surfel-rasterization, which
 are neither vendored nor in the offline wheelhouse (BASELINE.md section 4).  north_star's target is stated against
-"the reference GPU build", so bench.py times, on the same B200 and the same shapes, what that build does
+"the reference GPU build", so bench.py times, on the same GPU and the same shapes, what that build does
 algorithmically with the libraries this image does have:
 
   TorchDiT -- the deployed DiT block stack restated as plain PyTorch modules run the way the reference runs them:

@@ -3,7 +3,7 @@
 //
 // The reference's GPU build drives github.com/hbb1/diff-surfel-rasterization, which is neither vendored nor
 // installable here (BASELINE.md section 4).  This file restates THAT package's flow as literally as its published
-// structure allows, so bench.py can time "what the reference GPU build does" on the same B200:
+// structure allows, so bench.py can time "what the reference GPU build does" on the same GPU:
 //   per VIEW (the reference loops views in Python, /root/reference/nsr/gs_surfel.py:65-114):
 //     preprocessCUDA (one thread per surfel) -> cub::DeviceScan::InclusiveSum of tiles_touched -> cudaMemcpy of
 //     num_rendered to the host (a device sync per view) -> duplicateWithKeys ((tile << 32) | depth keys) ->

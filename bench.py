@@ -9,8 +9,7 @@ one pass of the hot path over that batch.
   python bench.py --impl reference ...                     (CPU reference arm:
         the oracle port of the reference's rasteriser on all host cores)
 
-Prints ONE JSON line (rank 0).  See DESIGN.md "Measurement" for the definition
-of every field.
+Prints ONE JSON line (rank 0).
 """
 import argparse
 import ctypes as C
@@ -47,7 +46,7 @@ def measured_peaks():
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not a measured peak"
 
 
 def make_inputs(seed, P=P_SURFELS, views=VIEWS):
@@ -287,6 +286,8 @@ def run_gpu(args):
     dev_ms_max = float(t.item())
     value = world * V * args.steps / (dev_ms_max * 1e-3)
     stage_ms /= args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"color": color, "allmap": allmap, "radii": radii, "grad": grad})
 
     # ---- end-to-end through the public API with host buffers ("e2e")
     rnd = GaussianRenderer2DGS(RES, 3, {})
@@ -333,9 +334,9 @@ def run_gpu(args):
         ev_done.record()
         state["done"] = ev_done
 
-    # 50 warm-up steps, then >= 500 steps AND >= 2 s (round 1 timed 20 steps = 29 ms after 3 warm-up steps: one
-    # allocator / engine stall made BENCH and SCALE N=1 disagree 24x).  Per-step host times are kept: the mean gives
-    # the throughput, the median / p99 / max show whether a stall was inside the window.
+    # 50 warm-up steps, then exactly --steps timed steps (a short window is at the mercy of one allocator / engine
+    # stall: pass enough steps for >= 2 s).  Per-step host times are kept: the mean gives the throughput, the
+    # median / p99 / max show whether a stall was inside the window.
     E2E_WARMUP = 50
     for _ in range(E2E_WARMUP):
         step_e2e()
@@ -347,13 +348,11 @@ def run_gpu(args):
     barrier()
     e2e_steps, step_s = 0, []
     e0 = time.perf_counter()
-    while e2e_steps < max(args.steps, 500) or (time.perf_counter() - e0) < 2.0:
+    while e2e_steps < args.steps:
         t_a = time.perf_counter()
         step_e2e()
         step_s.append(time.perf_counter() - t_a)
         e2e_steps += 1
-        if e2e_steps >= 20000:
-            break
     state["done"].synchronize()
     e_local = time.perf_counter() - e0
     gc.enable()
@@ -383,7 +382,7 @@ def run_gpu(args):
     if rank == 0:
         hbm, peak_src = measured_peaks()
         HW = H * W
-        # algorithmic bytes per launch (DESIGN.md "Kernels"): one launch covers all NV views
+        # algorithmic bytes per launch: one launch covers all NV views
         bytes_k3 = 76.0 * D + 40.0 * HW * V
         bytes_k4 = 76.0 * D + 60.0 * HW * V + 72.0 * P * V
         names = ["preprocess", "binning", "render_fwd", "render_bwd", "preprocess_bwd"]
@@ -393,19 +392,14 @@ def run_gpu(args):
         else:
             dom, dom_bytes = "render_fwd", bytes_k3
         achieved = dom_bytes / (stages[dom] * 1e-3) / 1e9
-        traffic, traffic_src = None, None
-        tp = os.path.join(ROOT, "profiles", "traffic.json")        # DRAM bytes per launch from the committed ncu capture
-        if os.path.exists(tp):
-            tj = json.load(open(tp))
-            key = dom + "_kernel"
-            if key in tj:
-                traffic, traffic_src = tj[key]["dram_bytes"], tj.get("_source")
+        traffic, traffic_src = None, None                          # DRAM bytes per launch: not measured
         step_bytes = V * (52.0 * P + 40.0 * HW) + 76.0 * D + V * (60.0 * HW + 104.0 * P) + 76.0 * D
         # FP32-issue view of the forward composite (SURVEY 8d): dense-equivalent pair evaluations = sum over tiles of
-        # (instances in the tile x 256 pixels), ~50 flop each, against 148 SMs x 128 lanes x 2 x 1.965 GHz
+        # (instances in the tile x 256 pixels), ~50 flop each, against the H100 SXM data sheet's 67 TFLOP/s FP32
+        # (132 SMs x 128 lanes x 2 x 1.98 GHz)
         ts = ws[L.tile_start:L.tile_start + 4 * (V * ((H + 15) // 16) * ((W + 15) // 16) + 1)].view(torch.int32).cpu().numpy().astype(np.int64)
         evals = float((ts[1:] - ts[:-1]).sum() * 256)
-        fp32_peak = 148 * 128 * 2 * 1.965e9 / 1e12
+        fp32_peak = 132 * 128 * 2 * 1.98e9 / 1e12
         fp32 = {"kernel": "render_fwd", "dense_pair_evals": evals, "flop_per_eval": 50,
                 "achieved_tflops_dense_equivalent": evals * 50 / (stages["render_fwd"] * 1e-3) / 1e12, "peak_tflops": fp32_peak,
                 "frac_dense_equivalent": evals * 50 / (stages["render_fwd"] * 1e-3) / 1e12 / fp32_peak,
@@ -416,14 +410,13 @@ def run_gpu(args):
             try:
                 dit_leg = run_dit_leg(dev)
                 pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
-                tpk = float(pk.get("bf16_tflops", 1590.0))
+                tpk = float(pk.get("bf16_tflops", 989.0))          # H100 SXM data sheet, dense BF16
                 for kk in dit_leg["kernels"].values():
                     kk["frac_of_bf16_peak"] = kk["tflops"] / tpk
                 dit_leg["tensor_peak_tflops"] = tpk
-                dit_leg["frac_of_bf16_peak_sustained"] = dit_leg["tflops"] / float(pk.get("bf16_tflops_sustained", 1400.0))
                 dit_leg["deployed_L_N768"] = run_dit_deployed_leg(dev)
                 dit_leg["C4_L_N4096"] = run_dit_deployed_leg(dev, nfe=10, N=4096)
-                # samples/s is a throughput metric: 4 samples denoised together fill the 148 SMs far better than one
+                # samples/s is a throughput metric: 4 samples denoised together fill the 132 SMs far better than one
                 # (M = 6144 rows instead of 1536: the D->D GEMMs go from 96 to 384 tiles)
                 dit_leg["deployed_L_N768_4samples"] = run_dit_deployed_leg(dev, nfe=10, N=768, samples=4)
                 try:
@@ -454,9 +447,6 @@ def run_gpu(args):
                "roofline": {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": hbm, "unit": "GB/s",
                             "frac": achieved / hbm, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
                             "algorithmic_bytes_per_launch": dom_bytes,
-                            # what the hardware actually moved (ncu dram__bytes of the stage's kernels, profiles/traffic.json)
-                            # over the live stage time: round 2's backward trades bytes (per-pixel lists, record slices)
-                            # for instructions, so it moves ~4.6x the algorithmic bytes on purpose
                             "traffic_GBs": (traffic / (stages[dom] * 1e-3) / 1e9) if traffic else None,
                             "traffic_frac": (traffic / (stages[dom] * 1e-3) / 1e9 / hbm) if traffic else None,
                             "whole_step_algorithmic_GBs": step_bytes / (dev_ms_max / args.steps * 1e-3) / 1e9,
@@ -473,6 +463,22 @@ def run_gpu(args):
     if world > 1:
         dist.destroy_process_group()
 
+
+
+DUMP_MAX_ELEMS = 4 << 20          # per array: at most 16 MB of float32, so the four arrays stay under 64 MB
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes what the last timed step computed as <out_dir>/<name>.npy (float32).  An array with more than
+    DUMP_MAX_ELEMS elements is stored as a fixed sample of its flattened elements: the sorted indices
+    np.random.default_rng(0).choice(size, DUMP_MAX_ELEMS, replace=False), the same for every run."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy().reshape(-1)
+        if a.size > DUMP_MAX_ELEMS:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_MAX_ELEMS, replace=False))
+            a = a[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float32))
 
 
 # ---------------------------------------------------------------------------
@@ -814,7 +820,7 @@ def run_raster_standin(dev, steps=20):
 
 
 def run_gpu_standin(dev):
-    """GPU comparison baselines on the same B200 (baseline/gpu_standin.py; BASELINE.md section 4)."""
+    """GPU comparison baselines on the same GPU (baseline/gpu_standin.py; BASELINE.md section 4)."""
     from baseline import gpu_standin as gs
     out = {"what": "unfused PyTorch-CUDA restatement of the reference's DiT block stack: nn.Linear under bf16 autocast (cuBLAS) + "
                    "flash_attn_func + separate norm/modulate/GELU kernels, context K/V re-projected every block, 2B CFG forward"}
@@ -832,6 +838,8 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-dit", action="store_true", help="skip the secondary DiT sampling legs (DiT, cascade, stand-ins)")
     ap.add_argument("--no-c5", action="store_true", help="skip the C5 decode -> all-gather -> render leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's color / allmap / radii / grad as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

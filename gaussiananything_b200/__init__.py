@@ -1,4 +1,4 @@
-"""gaussiananything_b200 -- B200 (sm_100a) kernels for GaussianAnything's two hot paths
+"""gaussiananything_b200 -- H100 (sm_90a) kernels for GaussianAnything's two hot paths
 (surfel rasteriser; DiT denoiser + flow-matching sampler) behind the reference's own Python API.
 See INTEGRATION.md.  Nothing here falls back to CPU or to a library path."""
 import sys

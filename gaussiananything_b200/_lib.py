@@ -2,7 +2,7 @@
 
 There is NO CPU fallback: if the shared library is missing or does not load,
 importing anything that computes raises.  Build it with
-`python -m gaussiananything_b200.build` (nvcc, sm_100a).
+`python -m gaussiananything_b200.build` (nvcc, sm_90a).
 """
 import ctypes as C
 import os

@@ -1,4 +1,4 @@
-"""In-tree build of libga_b200.so (sm_100a only) with nvcc.
+"""In-tree build of libga_b200.so (sm_90a only) with nvcc.
 
 `python -m gaussiananything_b200.build` or `build()`; the .so is written next
 to this file so it travels to the GPU box with the repo snapshot.
@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libga_b200.so")
 OBJ = os.path.join(HERE, "csrc", "_obj")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 # per-file extra flags.  raster_preprocess.cu: no FMA contraction, so tile

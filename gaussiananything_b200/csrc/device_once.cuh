@@ -28,7 +28,7 @@ static inline int ga_sm_count()
     if (ga_first_use_on_device(f, &dev) || dev < 0 || dev >= 64) {
         int n = 0;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
         if (dev < 0 || dev >= 64) return n;
         f.value[dev] = n;
     }

@@ -1,4 +1,4 @@
-// tcgen05 flash attention (head_dim 64, no mask, no dropout) for the DiT
+// wgmma flash attention (head_dim 64, no mask, no dropout) for the DiT
 // self- and cross-attention: softmax(q k^T / 8) v.  Replaces
 // xformers.ops.memory_efficient_attention at
 // /root/reference/vit/vision_transformer.py:297 and
@@ -9,61 +9,30 @@
 // Output O [B, Nq, H*64] bf16 (token-major: the A operand of the out-projection GEMM).
 //
 // One CTA = 128 queries of one (batch, head); keys in blocks of 128:
-//   warp 0   : TMA producer (Q once, K/V double buffered)
-//   warp 1   : single-thread tcgen05.mma issuer: S = Q K^T (128x128x64) into TMEM,
-//              then O_blk = P V (128x64x128) with P staged in 128B-swizzled smem
-//   warps 2-5: softmax, one query row per thread: S from TMEM -> registers,
-//              online max/sum in the exp2 domain, P (bf16) -> smem, O_blk from
-//              TMEM accumulated in registers with the running rescale.
-// Two CTAs share an SM (97 KB smem, 256 TMEM columns each), so one CTA's MMAs / TMA loads overlap
-// the other's softmax; within a CTA the next block's QK^T is issued as soon as S has been read.
-//
-// Static-bound path: P never touches shared memory.  With P staged in smem a key block moves 144 KB through the
-// SM's 128 B/clk shared-memory port (QK^T reads Q+K 32 KB, P*V reads P+V 48 KB, st.shared of P 32 KB, TMA fills
-// 32 KB) = 1150 cycles per CTA and block -- more than the 1024 cycles the MUFU pipe needs for the block's 16k
-// exponentials, and exactly the 2300 cycles per block pair tools/trace_attn.py measured.  The softmax threads now
-// write bf16 P straight into TMEM (tcgen05.st, 64 columns) and P*V takes its A operand from there
-// (tcgen05.mma [d], [a_tmem], b_desc): 80 KB per block, the kernel is MUFU-bound again.
+//   warps 0-7 : two consumer warpgroups, 64 queries each.  S = Q K^T (wgmma m64n128k16, both operands from shared
+//               memory) lands in registers; the softmax runs on that fragment (a query row lives in the 4 lanes of a
+//               quad); P is re-packed to bf16 in registers and is the A operand of O += P V (wgmma m64n64k16 with A
+//               from registers), so P never touches shared memory.  The next block's Q K^T is issued right behind
+//               this block's P V and both run under one wait.
+//   warp 8    : TMA producer (Q once, K and V double buffered).
 #include "../../include/ga_b200.h"
 #include "device_once.cuh"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
-using namespace sm100;
+using namespace sm90;
 
 int ga_make_tmap_bf16(CUtensorMap *map, const void *ptr, uint64_t rows, uint64_t cols, uint64_t ld_elems,
                       uint32_t box_rows);
-
-#ifdef GA_B200_TRACE
-// Debug build only (tools/trace_attn.py): per-CTA timeline of softmax warp 2 / the MMA thread, 8 stamps per key block.
-__device__ unsigned long long g_attn_trace[1024 * 160];
-#define ATRACE(slot) do { if (lane == 0) g_attn_trace[(blockIdx.y * gridDim.x + blockIdx.x) * 160 + (slot)] = clock64(); } while (0)
-#define ATRACE_BLK(j, e) do { if ((j) < 19) ATRACE(8 + (j) * 8 + (e)); } while (0)
-#define ATRACE_START() do { if (threadIdx.x == 64) { unsigned smid_; asm volatile("mov.u32 %0, %%smid;" : "=r"(smid_)); \
-    g_attn_trace[(blockIdx.y * gridDim.x + blockIdx.x) * 160 + 0] = smid_; \
-    g_attn_trace[(blockIdx.y * gridDim.x + blockIdx.x) * 160 + 1] = clock64(); } } while (0)
-#define ATRACE_END() do { if (threadIdx.x == 64) g_attn_trace[(blockIdx.y * gridDim.x + blockIdx.x) * 160 + 2] = clock64(); } while (0)
-extern "C" int ga_debug_attn_trace(unsigned long long *host, int n)
-{
-    return (int)cudaMemcpyFromSymbol(host, g_attn_trace, sizeof(unsigned long long) * (size_t)n);
-}
-#else
-#define ATRACE(slot) do { } while (0)
-#define ATRACE_BLK(j, e) do { } while (0)
-#define ATRACE_START() do { } while (0)
-#define ATRACE_END() do { } while (0)
-#endif
 
 namespace {
 
 constexpr int AQ = 128, AK = 128, HD = 64;
 constexpr int kQBytes = AQ * HD * 2;            // 16 KB
 constexpr int kKBytes = AK * HD * 2;            // 16 KB per stage, 2 stages
-constexpr int kVBytes = HD * AK * 2;            // 16 KB (two 64-key sub-tiles of 8 KB), 1 stage
-constexpr int kPBytes = AQ * AK * 2;            // 32 KB (two 64-key sub-tiles of 16 KB), 1 buffer
-constexpr int kSmemAttn = kQBytes + 2 * kKBytes + kVBytes + kPBytes + 1024;     // 97 KB -> 2 CTAs / SM
-constexpr int kAttnThreads = 192;          // online softmax: TMA warp, MMA warp, 4 softmax warps (one row per thread)
-// static bound: NS threads per query row (each handles 128/NS keys): block = 64 + 128*NS threads
-constexpr uint32_t kTmemColsAttn = 256;         // S: 128 columns, O_blk: 64 columns; 2 CTAs share the SM's 512
+constexpr int kVBytes = HD * AK * 2;            // 16 KB per stage (two 64-key sub-tiles of 8 KB), 2 stages
+constexpr int kSmemAttn = kQBytes + 2 * kKBytes + 2 * kVBytes + 1024;
+constexpr int kConsumerWarps = 8;
+constexpr int kAttnThreads = 32 * kConsumerWarps + 32;
 
 __device__ __forceinline__ uint32_t pack2(float a, float b)
 {
@@ -77,345 +46,170 @@ __device__ __forceinline__ float ex2_fast(float x)
     return r;
 }
 
-// Two CTAs are co-resident per SM (97 KB smem, 256 TMEM columns, <=168 registers): while one CTA's softmax
-// warps keep the MUFU/FMA pipes busy, the other CTA's MMAs and TMA loads run -- the hardware interleaves the
-// two dependency chains, so the kernel needs no intra-CTA ping-pong.
-//
 // kStatic: the caller supplies an upper bound of |q.k| * scale (available for free when q and k are
 // RMS-normalised: |q.k| <= 64 max|w_q| max|w_k|).  exp2(s*scale - bound) then never overflows, so no running
-// maximum, no rescaling and no per-block read-out of O are needed: P*V accumulates in TMEM over all key blocks
-// and S is read from TMEM exactly once.  Mathematically identical to softmax (the constant cancels in O / l).
-template <bool kStatic, int kRowSplit>
-__global__ void __launch_bounds__(kStatic ? 64 + 128 * kRowSplit : kAttnThreads, 2)
+// maximum and no rescaling of O are needed.  Mathematically identical to softmax (the constant cancels in O / l).
+//
+// Fragment layout (wgmma accumulator, thread = warp wi of its warpgroup, lane l, r = l/4, c = l%4):
+//   s[4j + e]: query row 16 wi + r + 8 (e >> 1), key 8 j + 2 c + (e & 1)
+// The bf16 A fragment of m64k16 for keys [16 kk, 16 kk + 16) is {s[8kk..8kk+1], s[8kk+2..3], s[8kk+4..5], s[8kk+6..7]}
+// packed in pairs, i.e. the accumulator of Q K^T is already in the order P V needs.
+template <bool kStatic>
+__global__ void __launch_bounds__(kAttnThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant__ CUtensorMap tma_k,
                 const __grid_constant__ CUtensorMap tma_vt, __nv_bfloat16 *__restrict__ out,
                 const int Nq, const int Nk, const int pitch_q, const int pitch_k, const int heads,
                 const float scale_log2, const float bound_log2)
 {
     extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t q_full, k_full[2], k_empty[2], v_full, v_empty, s_full, s_empty, p_full, o_full, o_empty, p_empty;
-    __shared__ uint32_t tmem_slot;
-    __shared__ float s_lsum[kRowSplit][AQ];
+    __shared__ uint64_t q_full, k_full[2], k_empty[2], v_full[2], v_empty[2];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t *sQ = smem;
     uint8_t *sK = sQ + kQBytes;
     uint8_t *sV = sK + 2 * kKBytes;
-    uint8_t *sP = sV + kVBytes;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int bh = blockIdx.y;
     const int q0 = blockIdx.x * AQ;
     const int nb = (Nk + AK - 1) / AK;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         prefetch_tmap(&tma_q); prefetch_tmap(&tma_k); prefetch_tmap(&tma_vt);
-    }
-    if (warp == 1) {
-        if (lane == 0) {
-            mbar_init(&q_full, 1);
-            for (int s = 0; s < 2; s++) { mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 1); }
-            mbar_init(&v_full, 1); mbar_init(&v_empty, 1);
-            mbar_init(&s_full, 1); mbar_init(&o_full, 1);
-            mbar_init(&p_full, kStatic ? 128 * kRowSplit : 128); mbar_init(&o_empty, 128); mbar_init(&p_empty, 1);
-            mbar_init(&s_empty, 128 * kRowSplit);
-            fence_barrier_init();
+        mbar_init(&q_full, 1);
+        for (int s = 0; s < 2; s++) {
+            mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], kConsumerWarps);
+            mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], kConsumerWarps);
         }
-        __syncwarp();
-        tmem_alloc<kTmemColsAttn>(&tmem_slot);
+        fence_barrier_init();
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
-    // columns: S 0-127 (fp32 scores) | static path: P 128-191 (bf16 pairs), O 192-255 | online path: O 128-191
-    const uint32_t tS = tmem, tP = tmem + 128, tO = kStatic ? tmem + 192 : tmem + 128;
-#ifdef GA_B200_TRACE
-    if (threadIdx.x == 64) {
-        unsigned smid; asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-        g_attn_trace[(blockIdx.y * gridDim.x + blockIdx.x) * 160 + 0] = smid;
-        g_attn_trace[(blockIdx.y * gridDim.x + blockIdx.x) * 160 + 1] = clock64();
-    }
-#endif
     pdl_wait();
     pdl_launch_dependents();
 
-    if (warp == 0) {
+    if (warp == kConsumerWarps) {
         if (elect_one()) {
             mbar_expect_tx(&q_full, kQBytes);
             tma_load_2d(sQ, &tma_q, &q_full, 0, bh * pitch_q + q0);
-            // K runs one block ahead of V: its slot frees as soon as QK^T of block j-1 has retired, whereas the single
-            // V buffer frees only after P*V of block j-1 -- loading them in lock step delayed K_{j+1} (and with it
-            // S_{j+1}) past the end of block j's exponentials
-            auto load_k = [&](int j) {
+            for (int j = 0; j < nb; j++) {
                 const int s = j & 1;
-                mbar_wait(&k_empty[s], ((j >> 1) & 1) ^ 1);
+                const uint32_t ph = ((j >> 1) & 1) ^ 1;
+                mbar_wait(&k_empty[s], ph);
                 mbar_expect_tx(&k_full[s], kKBytes);
                 tma_load_2d(sK + s * kKBytes, &tma_k, &k_full[s], 0, bh * pitch_k + j * AK);
-            };
-            load_k(0);
-            for (int j = 0; j < nb; j++) {
-                if (j + 1 < nb) load_k(j + 1);
-                mbar_wait(&v_empty, (j & 1) ^ 1);
-                mbar_expect_tx(&v_full, kVBytes);
-                tma_load_2d(sV, &tma_vt, &v_full, j * AK, bh * HD);
-                tma_load_2d(sV + kVBytes / 2, &tma_vt, &v_full, j * AK + 64, bh * HD);
+                mbar_wait(&v_empty[s], ph);
+                mbar_expect_tx(&v_full[s], kVBytes);
+                tma_load_2d(sV + s * kVBytes, &tma_vt, &v_full[s], j * AK, bh * HD);
+                tma_load_2d(sV + s * kVBytes + kVBytes / 2, &tma_vt, &v_full[s], j * AK + 64, bh * HD);
             }
         }
-    } else if (warp == 1) {
-        if (elect_one()) {
-            constexpr uint32_t idesc_s = umma_idesc_bf16(AQ, AK);
-            constexpr uint32_t idesc_o = umma_idesc_bf16(AQ, HD);
-            const uint64_t qd = umma_desc_k_sw128(smem_u32(sQ));
-            const uint64_t pd = umma_desc_k_sw128(smem_u32(sP));
-            const uint64_t vd = umma_desc_k_sw128(smem_u32(sV));
-            mbar_wait(&q_full, 0);
-            auto issue_s = [&](int j) {
-                const int s = j & 1;
-                mbar_wait(&k_full[s], (j >> 1) & 1);
-                tc_fence_after();
-                const uint64_t kd = umma_desc_k_sw128(smem_u32(sK + s * kKBytes));
+        return;
+    }
+
+    const int cw = warp >> 2, wi = warp & 3;
+    const int r = lane >> 2, c = lane & 3;
+    const uint64_t qd = wgmma_desc_k_sw128(smem_u32(sQ + cw * 64 * 128));
+    float s_acc[AK / 2];
+    float o_acc[HD / 2];
 #pragma unroll
-                for (int k = 0; k < HD / 16; k++)
-                    umma_bf16_ss(tS, qd + (uint64_t)(2 * k), kd + (uint64_t)(2 * k), idesc_s, k != 0);
-                umma_commit(&k_empty[s]);
-                umma_commit(&s_full);
-            };
-            issue_s(0);
-            for (int j = 0; j < nb; j++) {
-                const uint32_t ph = j & 1;
-                if (kStatic) {
-                    // S_j is in the softmax threads' registers: the next QK^T runs under this block's exponentials
-                    if (j + 1 < nb) {
-                        mbar_wait(&s_empty, ph);
-                        tc_fence_after();
-                        if (j < 19) ATRACE(8 + j * 8 + 4);
-                        issue_s(j + 1);
-                        if (j < 19) ATRACE(8 + j * 8 + 5);
-                    }
-                    mbar_wait(&p_full, ph);                 // P_j staged
-                    if (j < 19) ATRACE(8 + j * 8 + 6);
-                } else {
-                    mbar_wait(&p_full, ph);                 // P_j staged; S_j has been consumed
-                    if (j + 1 < nb) issue_s(j + 1);         // next QK^T overlaps this block's P*V and the O read-out
-                }
-                mbar_wait(&v_full, ph);
-                if (!kStatic) mbar_wait(&o_empty, ph ^ 1);   // softmax warps have read O_{j-1}
-                tc_fence_after();
+    for (int i = 0; i < HD / 2; i++) o_acc[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+
+    auto issue_s = [&](int j) {
+        const int s = j & 1;
+        mbar_wait(&k_full[s], (j >> 1) & 1);
+        const uint64_t kd = wgmma_desc_k_sw128(smem_u32(sK + s * kKBytes));
+        fence_regs(s_acc);
+        wgmma_fence();
 #pragma unroll
-                for (int kk = 0; kk < AK / 16; kk++) {
-                    const uint64_t sub_v = (uint64_t)((kk >> 2) * ((kVBytes / 2) >> 4));
-                    if (kStatic) {
-                        // A = P from tensor memory: 16 keys = 8 columns per k-step
-                        umma_bf16_ts(tO, tP + (uint32_t)(kk * 8), vd + sub_v + (uint64_t)(2 * (kk & 3)), idesc_o,
-                                     (uint32_t)((j | kk) != 0));
-                    } else {
-                        const uint64_t sub_p = (uint64_t)((kk >> 2) * ((kPBytes / 2) >> 4));
-                        umma_bf16_ss(tO, pd + sub_p + (uint64_t)(2 * (kk & 3)), vd + sub_v + (uint64_t)(2 * (kk & 3)), idesc_o,
-                                     (uint32_t)(kk != 0));
-                    }
-                }
-                umma_commit(&v_empty);
-                if (kStatic && j < 19) ATRACE(8 + j * 8 + 7);
-                if (kStatic) {
-                    umma_commit(&p_empty);                  // P (and V) may be overwritten
-                    if (j == nb - 1) umma_commit(&o_full);  // O complete after the last key block
-                } else {
-                    umma_commit(&o_full);
-                }
-            }
+        for (int k = 0; k < HD / 16; k++) wgmma_ss<AK>(s_acc, qd + (uint64_t)(2 * k), kd + (uint64_t)(2 * k), (uint32_t)(k != 0));
+        wgmma_commit();
+    };
+
+    mbar_wait(&q_full, 0);
+    issue_s(0);
+    wgmma_wait<0>();
+    fence_regs(s_acc);
+    if (lane == 0) mbar_arrive(&k_empty[0]);
+
+    for (int j = 0; j < nb; j++) {
+        const int kbase = j * AK;
+        if (kbase + AK > Nk) {                                   // ragged last block only: mask the padding keys
+#pragma unroll
+            for (int i = 0; i < AK / 2; i++)
+                if (kbase + 8 * (i >> 2) + 2 * c + (i & 1) >= Nk) s_acc[i] = -INFINITY;
         }
-    } else {
-        const int qd4 = warp & 3;
-        const int row = qd4 * 32 + lane;
-        const uint32_t lane_off = (uint32_t)(qd4 * 32) << 16;
-        float m_run = -INFINITY, l_run = 0.f, corr = 0.f;
-        float o_acc[HD];
-#pragma unroll
-        for (int i = 0; i < HD; i++) o_acc[i] = 0.f;
-        uint8_t *prow = sP + (row >> 3) * 1024 + (row & 7) * 128;
-
-        auto accumulate_o = [&](int j, float c) {
-            mbar_wait(&o_full, j & 1);
-            tc_fence_after();
-#pragma unroll
-            for (int h2 = 0; h2 < 2; h2++) {
-                uint32_t r[32];
-                tmem_ld_32x32b_x32(tO + lane_off + h2 * 32, r);
-                tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < 32; i++) o_acc[h2 * 32 + i] = o_acc[h2 * 32 + i] * c + __uint_as_float(r[i]);
-            }
-            tc_fence_before();
-            mbar_arrive(&o_empty);
-        };
-
+        float m_use[2];
         if constexpr (kStatic) {
-            // kRowSplit threads per query row: this one handles keys [part*KP, part*KP+KP) of every block; with no
-            // running maximum the threads of a row never have to talk until the very end.
-            constexpr int KP = AK / kRowSplit;                 // 32 or 64 keys per thread
-            const int part = (warp - 2) >> 2;
-            float ls0 = 0.f, ls1 = 0.f, ls2 = 0.f, ls3 = 0.f;
-            // P sub-tile (64 keys each) and first 16-byte chunk inside it
-            const uint32_t tS_mine = tS + lane_off + part * KP;
-            const uint32_t tP_mine = tP + lane_off + part * (KP / 2);          // two bf16 per column
-            static_assert(KP == 64, "one tcgen05.st.x32 per thread and block");
-            for (int j = 0; j < nb; j++) {
-                mbar_wait(&s_full, j & 1);
-                tc_fence_after();
-                if (warp == 2 && j < 19) ATRACE(8 + j * 8 + 0);
-                const int kbase = j * AK + part * KP;
-                uint32_t r[KP / 32][32];
-#pragma unroll
-                for (int h2 = 0; h2 < KP / 32; h2++) tmem_ld_32x32b_x32(tS_mine + h2 * 32, r[h2]);   // all loads in flight
-                tmem_ld_wait();
-                tc_fence_before();
-                mbar_arrive(&s_empty);                       // S_j now lives in registers
-                if (warp == 2 && j < 19) ATRACE(8 + j * 8 + 1);
-                if (kbase + KP > Nk) {                       // ragged last block only (warp-uniform): mask the padding keys
-#pragma unroll
-                    for (int h2 = 0; h2 < KP / 32; h2++)
-#pragma unroll
-                        for (int i = 0; i < 32; i++)
-                            if (kbase + h2 * 32 + i >= Nk) r[h2][i] = 0xff800000u;      // -inf
-                }
-                uint32_t pk[32];                             // this thread's 64 probabilities as bf16 pairs
-#pragma unroll
-                for (int h2 = 0; h2 < KP / 32; h2++) {
-#pragma unroll
-                    for (int i = 0; i < 32; i++)
-                        r[h2][i] = __float_as_uint(ex2_fast(fmaf(__uint_as_float(r[h2][i]), scale_log2, -bound_log2)));
-#pragma unroll
-                    for (int i = 0; i < 32; i += 4) {
-                        ls0 += __uint_as_float(r[h2][i]); ls1 += __uint_as_float(r[h2][i + 1]);
-                        ls2 += __uint_as_float(r[h2][i + 2]); ls3 += __uint_as_float(r[h2][i + 3]);
-                    }
-#pragma unroll
-                    for (int i = 0; i < 16; i++)
-                        pk[h2 * 16 + i] = pack2(__uint_as_float(r[h2][2 * i]), __uint_as_float(r[h2][2 * i + 1]));
-                }
-                if (warp == 2 && j < 19) ATRACE(8 + j * 8 + 2);
-                if (j > 0) mbar_wait(&p_empty, (j - 1) & 1); // P*V of the previous block has retired
-                tc_fence_after();
-                tmem_st_32x32b_x32(tP_mine, pk);
-                tmem_st_wait();
-                tc_fence_before();
-                mbar_arrive(&p_full);
-                if (warp == 2 && j < 19) ATRACE(8 + j * 8 + 3);
-            }
-            s_lsum[part][row] = (ls0 + ls1) + (ls2 + ls3);
-            asm volatile("bar.sync 1, %0;\n" ::"n"(128 * kRowSplit) : "memory");      // the softmax warps only
-            float lt = 0.f;
-#pragma unroll
-            for (int k = 0; k < kRowSplit; k++) lt += s_lsum[k][row];
-            const float inv = 1.0f / lt;
-            mbar_wait(&o_full, 0);
-            tc_fence_after();
-            constexpr int OC = HD / kRowSplit;                 // head dims this thread writes out
-            const int q = q0 + row;
-            const int ob = bh / heads, oh = bh % heads;
-            uint4 *dst = reinterpret_cast<uint4 *>(out + ((size_t)ob * Nq + q) * (size_t)(heads * HD) + oh * HD + part * OC);
-            auto write_out = [&](const auto &ro) {
-                if (q < Nq) {
-#pragma unroll
-                    for (int i = 0; i < OC / 8; i++)
-                        dst[i] = make_uint4(pack2(__uint_as_float(ro[8 * i]) * inv, __uint_as_float(ro[8 * i + 1]) * inv),
-                                            pack2(__uint_as_float(ro[8 * i + 2]) * inv, __uint_as_float(ro[8 * i + 3]) * inv),
-                                            pack2(__uint_as_float(ro[8 * i + 4]) * inv, __uint_as_float(ro[8 * i + 5]) * inv),
-                                            pack2(__uint_as_float(ro[8 * i + 6]) * inv, __uint_as_float(ro[8 * i + 7]) * inv));
-                }
-            };
-            if constexpr (OC == 32) {
-                uint32_t ro[32];
-                tmem_ld_32x32b_x32(tO + lane_off + part * OC, ro);
-                tmem_ld_wait();
-                write_out(ro);
-            } else {
-                uint32_t ro[16];
-                tmem_ld_32x32b_x16(tO + lane_off + part * OC, ro);
-                tmem_ld_wait();
-                write_out(ro);
-            }
-            tc_fence_before();
+            m_use[0] = m_use[1] = bound_log2;
         } else {
-        for (int j = 0; j < nb; j++) {
-            mbar_wait(&s_full, j & 1);
-            tc_fence_after();
-            const int kbase = j * AK;
-            const bool ragged = kbase + AK > Nk;
-            // pass 1: row maximum (S stays in TMEM; re-reading it is cheaper than 128 live registers)
-            float mx = -INFINITY;
-#pragma unroll 1
-            for (int c = 0; c < AK; c += 32) {
-                uint32_t r[32];
-                tmem_ld_32x32b_x32(tS + lane_off + c, r);
-                tmem_ld_wait();
+            float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-                for (int i = 0; i < 32; i++) {
-                    const float v = (ragged && kbase + c + i >= Nk) ? -INFINITY : __uint_as_float(r[i]);
-                    mx = fmaxf(mx, v);
+            for (int i = 0; i < AK / 2; i++) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s_acc[i]);
+#pragma unroll
+            for (int hf = 0; hf < 2; hf++) {
+                mx[hf] = fmaxf(mx[hf], __shfl_xor_sync(0xffffffffu, mx[hf], 1));
+                mx[hf] = fmaxf(mx[hf], __shfl_xor_sync(0xffffffffu, mx[hf], 2));
+                const float m_new = fmaxf(m_run[hf], mx[hf] * scale_log2);
+                const float corr = ex2_fast(m_run[hf] - m_new);
+                m_run[hf] = m_new;
+                m_use[hf] = m_new;
+                l_run[hf] *= corr;
+#pragma unroll
+                for (int jj = 0; jj < HD / 8; jj++) {
+                    o_acc[4 * jj + 2 * hf] *= corr;
+                    o_acc[4 * jj + 2 * hf + 1] *= corr;
                 }
             }
-            const float corr_prev = corr;
-            const float m_new = fmaxf(m_run, mx * scale_log2);
-            corr = ex2_fast(m_run - m_new);
-            m_run = m_new;
-            // the previous block's P*V must have retired before P is overwritten; fold its result in now
-            if (j > 0) accumulate_o(j - 1, corr_prev);
-            // pass 2: p = 2^(s*scale - m), row sum, bf16 P into 128B-swizzled smem
-            float lsum = 0.f;
-#pragma unroll 1
-            for (int c = 0; c < AK; c += 32) {
-                uint32_t r[32];
-                tmem_ld_32x32b_x32(tS + lane_off + c, r);
-                tmem_ld_wait();
-                float p[32];
-#pragma unroll
-                for (int i = 0; i < 32; i++) {
-                    const float v = (ragged && kbase + c + i >= Nk) ? -INFINITY : __uint_as_float(r[i]);
-                    const float xx = fmaf(v, scale_log2, -m_new);
-                    p[i] = ex2_fast(xx);
-                    lsum += p[i];
-                }
-#pragma unroll
-                for (int g = 0; g < 4; g++) {
-                    const int c8 = (c >> 3) + g;                 // 16-byte chunk index along the 128 keys
-                    const int sub = c8 >> 3, q16 = c8 & 7;
-                    uint4 *dst = reinterpret_cast<uint4 *>(prow + sub * (kPBytes / 2) + ((q16 ^ (row & 7)) << 4));
-                    *dst = make_uint4(pack2(p[8 * g], p[8 * g + 1]), pack2(p[8 * g + 2], p[8 * g + 3]),
-                                      pack2(p[8 * g + 4], p[8 * g + 5]), pack2(p[8 * g + 6], p[8 * g + 7]));
-                }
-            }
-            l_run = l_run * corr + lsum;
-            fence_proxy_async_smem();
-            tc_fence_before();
-            mbar_arrive(&p_full);
         }
-        accumulate_o(nb - 1, corr);
-        const int q = q0 + row;
-        if (q < Nq) {
-            const float inv = 1.0f / l_run;
-            const int b = bh / heads, h = bh % heads;
-            uint4 *dst = reinterpret_cast<uint4 *>(out + ((size_t)b * Nq + q) * (size_t)(heads * HD) + h * HD);
+        uint32_t pa[AK / 16][4];
 #pragma unroll
-            for (int i = 0; i < 8; i++)
-                dst[i] = make_uint4(pack2(o_acc[8 * i] * inv, o_acc[8 * i + 1] * inv),
-                                    pack2(o_acc[8 * i + 2] * inv, o_acc[8 * i + 3] * inv),
-                                    pack2(o_acc[8 * i + 4] * inv, o_acc[8 * i + 5] * inv),
-                                    pack2(o_acc[8 * i + 6] * inv, o_acc[8 * i + 7] * inv));
+        for (int i = 0; i < AK / 2; i += 2) {
+            const int hf = (i >> 1) & 1;
+            const float p0 = ex2_fast(fmaf(s_acc[i], scale_log2, -m_use[hf]));
+            const float p1 = ex2_fast(fmaf(s_acc[i + 1], scale_log2, -m_use[hf]));
+            l_run[hf] += p0 + p1;
+            pa[i >> 3][(i >> 1) & 3] = pack2(p0, p1);
         }
-        tc_fence_before();
+        // O += P V_j, then (under the same wait) S = Q K_{j+1}^T
+        const int sv = j & 1;
+        mbar_wait(&v_full[sv], (j >> 1) & 1);
+        const uint64_t vd = wgmma_desc_k_sw128(smem_u32(sV + sv * kVBytes));
+        fence_regs(o_acc);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < AK / 16; kk++)
+            wgmma_m64n64k16_rs(o_acc, pa[kk], vd + (uint64_t)((kk >> 2) * ((kVBytes / 2) >> 4) + 2 * (kk & 3)), 1u);
+        wgmma_commit();
+        if (j + 1 < nb) issue_s(j + 1);
+        wgmma_wait<0>();
+        fence_regs(o_acc);
+        fence_regs(s_acc);
+#pragma unroll
+        for (int kk = 0; kk < AK / 16; kk++)
+#pragma unroll
+            for (int e = 0; e < 4; e++) asm volatile("" : "+r"(pa[kk][e])::"memory");    // live until P V retired
+        if (lane == 0) {
+            mbar_arrive(&v_empty[sv]);
+            if (j + 1 < nb) mbar_arrive(&k_empty[(j + 1) & 1]);
         }
     }
-    __syncthreads();
-#ifdef GA_B200_TRACE
-    if (threadIdx.x == 64) g_attn_trace[(blockIdx.y * gridDim.x + blockIdx.x) * 160 + 2] = clock64();
-#endif
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc<kTmemColsAttn>(tmem);
+
+    const int b = bh / heads, h = bh % heads;
+#pragma unroll
+    for (int hf = 0; hf < 2; hf++) {
+        float l = l_run[hf];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        const float inv = 1.0f / l;
+        const int q = q0 + cw * 64 + wi * 16 + r + 8 * hf;
+        if (q < Nq) {
+            __nv_bfloat16 *dst = out + ((size_t)b * Nq + q) * (size_t)(heads * HD) + h * HD + 2 * c;
+#pragma unroll
+            for (int jj = 0; jj < HD / 8; jj++)
+                *reinterpret_cast<uint32_t *>(dst + 8 * jj) = pack2(o_acc[4 * jj + 2 * hf] * inv, o_acc[4 * jj + 2 * hf + 1] * inv);
+        }
     }
 }
-
 
 }  // namespace
 
@@ -428,9 +222,9 @@ extern "C" int ga_attention_bf16(const void *Q, const void *K, const void *Vt, v
     const uint64_t BH = (uint64_t)batch * heads;
     static GaPerDevice attr_set;
     if (ga_first_use_on_device(attr_set)) {
-        cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemAttn);
+        cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemAttn);
         if (e != cudaSuccess) return (int)e;
-        e = cudaFuncSetAttribute(attn_fwd_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemAttn);
+        e = cudaFuncSetAttribute(attn_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemAttn);
         if (e != cudaSuccess) return (int)e;
     }
     // static-bound softmax only while exp(-2*bound) stays far from the fp32/bf16 underflow range
@@ -448,8 +242,8 @@ extern "C" int ga_attention_bf16(const void *Q, const void *K, const void *Vt, v
     __nv_bfloat16 *o = reinterpret_cast<__nv_bfloat16 *>(out);
     cudaStream_t st = (cudaStream_t)stream;
     if (use_static)
-        return (int)ga_launch_pdl(attn_fwd_kernel<true, 2>, grid, dim3(64 + 128 * 2), (size_t)kSmemAttn, st, tq, tk, tv, o, Nq,
+        return (int)ga_launch_pdl(attn_fwd_kernel<true>, grid, dim3(kAttnThreads), (size_t)kSmemAttn, st, tq, tk, tv, o, Nq,
                                   Nk, pitch_q, pitch_k, heads, scale_log2, score_bound * log2e);
-    return (int)ga_launch_pdl(attn_fwd_kernel<false, 1>, grid, dim3(kAttnThreads), (size_t)kSmemAttn, st, tq, tk, tv, o, Nq, Nk,
+    return (int)ga_launch_pdl(attn_fwd_kernel<false>, grid, dim3(kAttnThreads), (size_t)kSmemAttn, st, tq, tk, tv, o, Nq, Nk,
                               pitch_q, pitch_k, heads, scale_log2, 0.0f);
 }

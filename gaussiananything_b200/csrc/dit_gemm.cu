@@ -1,35 +1,34 @@
-// tcgen05 GEMM for the DiT denoiser: C[M,N] = A[M,K] * W[N,K]^T, bf16 operands,
-// fp32 accumulation in TMEM, fused epilogues.  Replaces the cuBLAS nn.Linear +
+// wgmma GEMM for the DiT denoiser: C[M,N] = A[M,K] * W[N,K]^T, bf16 operands,
+// fp32 accumulation in registers, fused epilogues.  Replaces the cuBLAS nn.Linear +
 // separate bias / GELU / gate / residual / qk-RMSNorm / permute kernels of
 // /root/reference/dit/dit_models_xformers.py:765-787,
 // /root/reference/vit/vision_transformer.py:215-303 and
 // /root/reference/ldm/modules/attention.py:484-561.
 //
-// Persistent kernel, one CTA per SM looping over 128 x BN output tiles:
-//   warp 0   : TMA producer  (cp.async.bulk.tensor, 128B-swizzled K-major tiles)
-//   warp 1   : TMEM allocator + single-thread tcgen05.mma issuer
-//   warps 2-9: epilogue, one accumulator row per thread (tcgen05.ld 32x32b), half the columns per warp
-// smem ring of kStages {A 128x64, W BNx64} bf16 tiles with full/empty mbarriers; the TMEM accumulator is
-// double buffered (acc_full/acc_empty) so the epilogue of one tile overlaps the main loop of the next.
+// Persistent kernel, one CTA per SM looping over 128 x BN output tiles, three warpgroups:
+//   warpgroup 0   : TMA producer (one elected thread; cp.async.bulk.tensor, 128B-swizzled K-major tiles)
+//   warpgroups 1-2: consumers, 64 rows each: wgmma m64nBNk16 from shared memory into registers, then the
+//                   epilogue straight from the accumulator registers
+// smem ring of kStages {A 128x64, W BNx64} bf16 tiles with full/empty mbarriers.  The producer keeps filling the
+// ring for the next tile while the consumers run the epilogue of this one.
 #include "../../include/ga_b200.h"
 #include "device_once.cuh"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
-using namespace sm100;
+using namespace sm90;
 
 namespace {
 
 constexpr int BM = 128, BK = 64;
-constexpr int kEpiWarps = 8;
-constexpr int kThreads = 64 + 32 * kEpiWarps;          // TMA warp + MMA warp + 8 epilogue warps
+constexpr int kConsumerWarps = 8;
+constexpr int kThreads = 128 + 32 * kConsumerWarps;      // producer warpgroup + 2 consumer warpgroups
 
 template <int BN> struct GemmCfg {
-    static constexpr int kStages = (BN >= 256) ? 3 : (BN >= 192 ? 4 : (BN >= 128 ? 5 : 7));    // + 36 KB of epilogue staging
     static constexpr int kABytes = BM * BK * 2;
     static constexpr int kBBytes = BN * BK * 2;
+    static constexpr int kStages = (200 * 1024) / (kABytes + kBBytes) > 8 ? 8 : (200 * 1024) / (kABytes + kBBytes);
     static constexpr int kRing = kStages * (kABytes + kBBytes);
-    static constexpr int kSmem = kRing + 1024 + 36 * 1024;
-    static constexpr int kTmemCols = (2 * BN <= 128) ? 128 : (2 * BN <= 256 ? 256 : 512);     // double-buffered accumulator (power of two)
+    static constexpr int kSmem = kRing + 1024 + kConsumerWarps * 2048;       // + epilogue staging
 };
 
 // exact-erf GELU to ~3e-7 (Abramowitz-Stegun 7.1.28: erf x = 1 - (1 + a1 x + .. + a6 x^6)^-16), 1 MUFU + ~16 FP32
@@ -58,27 +57,34 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b)
 }
 
 // ---- epilogue ---------------------------------------------------------------
-// tcgen05.ld hands every thread ONE accumulator row, so storing straight from that layout makes each warp store
-// touch 32 different rows (32 sectors per instruction) -- measured, the store queue then bounds the whole GEMM
-// (epilogue warps busy ~90 % of the time, tensor pipe ~30 %).  Each epilogue warp therefore owns a 4 KB staging
-// buffer (32 rows x 128 B, 16-byte chunks XOR-swizzled by row&7 so both phases are bank-conflict free):
-//   phase A (thread = row)          : TMEM -> registers -> staging
-//   phase B (8 lanes = one 128 B row): staging -> bias / GELU / gate / residual -> coalesced global stores
-// The epilogue mode is a template parameter: with a run-time switch inside the unrolled loops the kernel grew to
-// 5k instructions and a fifth of the epilogue's stall samples were instruction-cache misses.
-constexpr int kStageBytes = 4096;          // per epilogue warp
-constexpr int kHeadParams = 128;           // floats per epilogue warp: 64 bias + 64 norm weights (HEADS mode)
+// A warp's accumulator fragment covers 16 rows; a lane holds pairs of adjacent columns of two rows, so storing
+// straight from registers would write 8-byte pieces of 8 rows per instruction.  Each consumer warp therefore owns a
+// 2 KB staging buffer (16 rows x 128 B, 16-byte chunks XOR-swizzled by row&7 so both phases are bank-conflict free):
+//   phase A (fragment layout)          : registers -> staging, 32 fp32 columns at a time
+//   phase B (8 lanes = one 128 B row)  : staging -> bias / GELU / gate / residual -> coalesced global stores
+// The epilogue mode is a template parameter, so the unrolled loops carry no run-time switch.
+constexpr int kStageBytes = 2048;          // per consumer warp
+constexpr int kWarpRows = 16;              // accumulator rows per warp
 
-__device__ __forceinline__ void stage_rows(uint32_t stg, int lane, const uint32_t (&r)[32])
+// columns [32 ch, 32 ch + 32) of the warp's 16 rows -> staging (fp32, row-major, 128 B per row)
+template <int R>
+__device__ __forceinline__ void stage_chunk(uint32_t stg, int lane, const float (&acc)[R], int ch)
 {
-    const uint32_t row = stg + lane * 128;
+    const int r = lane >> 2, c = lane & 3;
 #pragma unroll
-    for (int ch = 0; ch < 8; ch++)
-        sts128(row + ((ch ^ (lane & 7)) << 4), r[4 * ch], r[4 * ch + 1], r[4 * ch + 2], r[4 * ch + 3]);
+    for (int jj = 0; jj < 4; jj++) {
+        const int j = 4 * ch + jj;
+        const int col = 8 * jj + 2 * c;                        // column inside the chunk
+#pragma unroll
+        for (int hf = 0; hf < 2; hf++) {
+            const int row = r + 8 * hf;
+            sts64(stg + row * 128 + (((col >> 2) ^ (row & 7)) << 4) + (col & 3) * 4, acc[4 * j + 2 * hf],
+                  acc[4 * j + 2 * hf + 1]);
+        }
+    }
 }
 
-// per-lane column parameters of phase B (this lane's 4 columns nn .. nn+3), fetched BEFORE the TMEM load so
-// their latency hides under it
+// per-lane column parameters of phase B (this lane's 4 columns nn .. nn+3)
 struct ColParams { float bias[4]; float gate[4]; };
 
 template <int MODE>
@@ -91,35 +97,36 @@ __device__ __forceinline__ void load_col_params(const GaGemmEpilogue &ep, int la
         cp.gate[j] = 1.f;
     }
     if (MODE == GA_EPI_RESID_GATE_F32 && ep.gate) {
-        const int b = m0w / ep.rows_per_batch;           // used when the warp's 32 rows sit in one batch element
+        const int b = m0w / ep.rows_per_batch;           // used when the warp's rows sit in one batch element
 #pragma unroll
         for (int j = 0; j < 4; j++) if (nn + j < N) cp.gate[j] = __ldg(ep.gate + (size_t)b * ep.gate_ld + nn + j);
     }
 }
 
-// 32 fp32 accumulator columns [n, n+32) of the warp's 32 rows [m0w, m0w+32), already staged by stage_rows()
+// 32 fp32 accumulator columns [n, n+32) of the warp's 16 rows [m0w, m0w+16), already staged by stage_chunk()
 template <int MODE>
-__device__ __forceinline__ void epilogue32(const GaGemmEpilogue &ep, uint32_t stg, int lane, int m0w, int n, int M, int N,
-                                           const ColParams &cp)
+__device__ __forceinline__ void epilogue_chunk(const GaGemmEpilogue &ep, uint32_t stg, int lane, int m0w, int n, int M,
+                                               int N, const ColParams &cp)
 {
+    constexpr int kIt = kWarpRows / 4;
     const int ch = lane & 7, rsub = lane >> 3;
     const int nn = n + ch * 4;                                 // this lane's 4 columns
     const bool vec = (nn + 4 <= N) && (ep.ld_out % 4) == 0;
     bool one_batch = true;
     if (MODE == GA_EPI_RESID_GATE_F32 && ep.gate)
-        one_batch = (m0w + 31) / ep.rows_per_batch == m0w / ep.rows_per_batch;
-    uint4 acc[8];
+        one_batch = (m0w + kWarpRows - 1) / ep.rows_per_batch == m0w / ep.rows_per_batch;
+    uint4 acc[kIt];
 #pragma unroll
-    for (int it = 0; it < 8; it++) {
+    for (int it = 0; it < kIt; it++) {
         const int rr = it * 4 + rsub;
         acc[it] = lds128(stg + rr * 128 + ((ch ^ (rr & 7)) << 4));
     }
-    // residual rows are read up front, all eight in flight at once: interleaved with the stores below the compiler
-    // must assume they alias and the loop degenerates into eight serial L2 round trips per chunk
-    float4 res[8];
+    // residual rows are read up front, all in flight at once: interleaved with the stores below the compiler
+    // must assume they alias and the loop degenerates into serial L2 round trips per chunk
+    float4 res[kIt];
     if (MODE == GA_EPI_RESID_GATE_F32 && vec) {
 #pragma unroll
-        for (int it = 0; it < 8; it++) {
+        for (int it = 0; it < kIt; it++) {
             const int m = m0w + it * 4 + rsub;
             res[it] = (m < M) ? *reinterpret_cast<const float4 *>(reinterpret_cast<const float *>(ep.out) +
                                                                    (size_t)m * ep.ld_out + nn)
@@ -128,7 +135,7 @@ __device__ __forceinline__ void epilogue32(const GaGemmEpilogue &ep, uint32_t st
     }
     if (nn >= N) return;
 #pragma unroll
-    for (int it = 0; it < 8; it++) {
+    for (int it = 0; it < kIt; it++) {
         const int m = m0w + it * 4 + rsub;
         if (m >= M) continue;
         float v[4] = {__uint_as_float(acc[it].x) + cp.bias[0], __uint_as_float(acc[it].y) + cp.bias[1],
@@ -174,399 +181,218 @@ __device__ __forceinline__ void epilogue32(const GaGemmEpilogue &ep, uint32_t st
     }
 }
 
-// HEADS epilogue for one head (64 columns [n, n+64)) of the warp's 32 rows: two TMEM passes keep the live set at
-// 32 values.  which = n / inner (+ first_part): 0 q, 1 k, 2 v ; head = (n % inner) / 64   ("(K H D)" column
-// layout, vit/vision_transformer.py:191,255).  q/k: per-head RMSNorm (dit/norm.py:27-40), fp32, then * weight;
-// a token's 64 bf16 are one 128 B line of the [B, H, tok_pitch, 64] layout.  v is stored transposed per head,
-// [B, H, 64, tok_pitch], so that P*V is a K-major x K-major contraction: staged as [d][32 tokens].
-__device__ __forceinline__ void epilogue_head(const GaGemmEpilogue &ep, uint32_t stg, float *hp, uint32_t taddr, int lane,
-                                              int m0w, int n, int M)
+// HEADS epilogue for one head (64 columns [n, n+64), accumulator groups 8h .. 8h+7) of the warp's 16 rows.
+// which = n / inner (+ first_part): 0 q, 1 k, 2 v ; head = (n % inner) / 64   ("(K H D)" column layout,
+// vit/vision_transformer.py:191,255).  q/k: per-head RMSNorm (dit/norm.py:27-40), fp32, then * weight; a row's 64
+// columns sit in the 4 lanes of a quad, so its sum of squares is two shuffles.  A token's 64 bf16 are one 128 B line
+// of the [B, H, tok_pitch, 64] layout.  v is stored transposed per head, [B, H, 64, tok_pitch], so that P*V is a
+// K-major x K-major contraction: staged as [d][16 tokens].
+template <int R>
+__device__ __forceinline__ void epilogue_head(const GaGemmEpilogue &ep, uint32_t stg, const float (&acc)[R], int h,
+                                              int lane, int m0w, int n, int M)
 {
     const int inner = ep.heads * 64;
     const int which = n / inner + ep.first_part;
     const int head = (n % inner) / 64;
     const float *w = which == 0 ? ep.qn_w : (which == 1 ? ep.kn_w : nullptr);
-    hp[lane] = ep.bias ? __ldg(ep.bias + n + lane) : 0.f;
-    hp[32 + lane] = ep.bias ? __ldg(ep.bias + n + 32 + lane) : 0.f;
-    hp[64 + lane] = w ? __ldg(w + lane) : 1.f;
-    hp[96 + lane] = w ? __ldg(w + 32 + lane) : 1.f;
-    __syncwarp();
+    const int r = lane >> 2, c = lane & 3;
+    float x[2][16];
+#pragma unroll
+    for (int jj = 0; jj < 8; jj++) {
+        const int j = 8 * h + jj, col = 8 * jj + 2 * c;
+        const float b0 = ep.bias ? __ldg(ep.bias + n + col) : 0.f;
+        const float b1 = ep.bias ? __ldg(ep.bias + n + col + 1) : 0.f;
+        x[0][2 * jj] = acc[4 * j] + b0;     x[0][2 * jj + 1] = acc[4 * j + 1] + b1;
+        x[1][2 * jj] = acc[4 * j + 2] + b0; x[1][2 * jj + 1] = acc[4 * j + 3] + b1;
+    }
     const int rpb = ep.rows_per_batch;
     const int b_first = m0w / rpb;
-    const bool one_batch = (m0w + 31) / rpb == b_first;
-    uint32_t r[32];
-    float rs = 1.0f;
-    if (w) {
-        float ss = 0.f;
+    const bool one_batch = (m0w + kWarpRows - 1) / rpb == b_first;
+    if (which <= 1) {
+        float rs[2] = {1.f, 1.f};
+        if (w) {
 #pragma unroll
-        for (int h2 = 0; h2 < 2; h2++) {
-            tmem_ld_32x32b_x32(taddr + h2 * 32, r);
-            tmem_ld_wait();
+            for (int hf = 0; hf < 2; hf++) {
+                float ss = 0.f;
 #pragma unroll
-            for (int i = 0; i < 32; i++) {
-                const float x = __uint_as_float(r[i]) + hp[h2 * 32 + i];
-                ss += x * x;
+                for (int i = 0; i < 16; i++) ss += x[hf][i] * x[hf][i];
+                ss += __shfl_xor_sync(0xffffffffu, ss, 1);
+                ss += __shfl_xor_sync(0xffffffffu, ss, 2);
+                rs[hf] = rsqrtf(ss * (1.0f / 64.0f) + ep.eps);
             }
         }
-        rs = rsqrtf(ss * (1.0f / 64.0f) + ep.eps);
-    }
-    if (which <= 1) {
 #pragma unroll
-        for (int h2 = 0; h2 < 2; h2++) {
-            tmem_ld_32x32b_x32(taddr + h2 * 32, r);
-            tmem_ld_wait();
+        for (int jj = 0; jj < 8; jj++) {
+            const int col = 8 * jj + 2 * c;
+            const float w0 = w ? __ldg(w + col) : 1.f, w1 = w ? __ldg(w + col + 1) : 1.f;
 #pragma unroll
-            for (int c4 = 0; c4 < 4; c4++) {
-                uint32_t pk[4];
-#pragma unroll
-                for (int j = 0; j < 4; j++) {
-                    const int i = c4 * 8 + j * 2;
-                    const float x0 = (__uint_as_float(r[i]) + hp[h2 * 32 + i]) * rs * hp[64 + h2 * 32 + i];
-                    const float x1 = (__uint_as_float(r[i + 1]) + hp[h2 * 32 + i + 1]) * rs * hp[64 + h2 * 32 + i + 1];
-                    pk[j] = pack_bf16(x0, x1);
-                }
-                sts128(stg + lane * 128 + (((h2 * 4 + c4) ^ (lane & 7)) << 4), pk[0], pk[1], pk[2], pk[3]);
+            for (int hf = 0; hf < 2; hf++) {
+                const int row = r + 8 * hf;
+                sts32(stg + row * 128 + ((jj ^ (row & 7)) << 4) + 4 * c,
+                      pack_bf16(x[hf][2 * jj] * rs[hf] * w0, x[hf][2 * jj + 1] * rs[hf] * w1));
             }
         }
         warp_sync_smem();
         __nv_bfloat16 *base = reinterpret_cast<__nv_bfloat16 *>(which == 0 ? ep.q : ep.k);
         const int ch = lane & 7, rsub = lane >> 3;
-        uint4 x[8];
+        uint4 v[kWarpRows / 4];
 #pragma unroll
-        for (int it = 0; it < 8; it++) {
+        for (int it = 0; it < kWarpRows / 4; it++) {
             const int rr = it * 4 + rsub;
-            x[it] = lds128(stg + rr * 128 + ((ch ^ (rr & 7)) << 4));
+            v[it] = lds128(stg + rr * 128 + ((ch ^ (rr & 7)) << 4));
         }
 #pragma unroll
-        for (int it = 0; it < 8; it++) {
+        for (int it = 0; it < kWarpRows / 4; it++) {
             const int m = m0w + it * 4 + rsub;
             if (m >= M) continue;
             const int b = one_batch ? b_first : m / rpb;
             const int t = m - b * rpb;
-            *reinterpret_cast<uint4 *>(base + (((size_t)b * ep.heads + head) * ep.tok_pitch + t) * 64 + ch * 8) = x[it];
+            *reinterpret_cast<uint4 *>(base + (((size_t)b * ep.heads + head) * ep.tok_pitch + t) * 64 + ch * 8) = v[it];
         }
     } else {
         const int t0 = m0w - b_first * rpb;
-        const bool fast = one_batch && (m0w + 32 <= M) && (ep.tok_pitch % 8) == 0 && (t0 % 8) == 0;
+        const bool fast = one_batch && (m0w + kWarpRows <= M) && (ep.tok_pitch % 8) == 0 && (t0 % 8) == 0;
         __nv_bfloat16 *vt = reinterpret_cast<__nv_bfloat16 *>(ep.vt);
-#pragma unroll
-        for (int h2 = 0; h2 < 2; h2++) {
-            tmem_ld_32x32b_x32(taddr + h2 * 32, r);
-            tmem_ld_wait();
-            if (fast) {
-#pragma unroll
-                for (int i = 0; i < 32; i++) {
-                    const __nv_bfloat16 hv = __float2bfloat16(__uint_as_float(r[i]) + hp[h2 * 32 + i]);
-                    asm volatile("st.shared.b16 [%0], %1;\n" ::"r"(stg + (uint32_t)((h2 * 32 + i) * 64 + lane * 2)),
-                                 "h"(*reinterpret_cast<const unsigned short *>(&hv)));
-                }
-            } else {
-                const int m = m0w + lane;
-                if (m < M) {
-                    const int b = m / rpb, t = m - b * rpb;
-                    __nv_bfloat16 *dst = vt + (((size_t)b * ep.heads + head) * 64 + h2 * 32) * ep.tok_pitch + t;
-#pragma unroll
-                    for (int i = 0; i < 32; i++)
-                        dst[(size_t)i * ep.tok_pitch] = __float2bfloat16(__uint_as_float(r[i]) + hp[h2 * 32 + i]);
-                }
-            }
-        }
         if (fast) {
+            // staging [d][16 tokens]: 32 B per head dimension
+#pragma unroll
+            for (int jj = 0; jj < 8; jj++)
+#pragma unroll
+                for (int hf = 0; hf < 2; hf++)
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const __nv_bfloat16 hv = __float2bfloat16(x[hf][2 * jj + e]);
+                        asm volatile("st.shared.b16 [%0], %1;\n" ::"r"(stg + (uint32_t)((8 * jj + 2 * c + e) * 32 + (r + 8 * hf) * 2)),
+                                     "h"(*reinterpret_cast<const unsigned short *>(&hv)));
+                    }
             warp_sync_smem();
-            const int ch = lane & 3, dsub = lane >> 2;
-            uint4 x[8];
+            uint4 v[4];
 #pragma unroll
-            for (int it = 0; it < 8; it++) x[it] = lds128(stg + (it * 8 + dsub) * 64 + ch * 16);
+            for (int it = 0; it < 4; it++) {
+                const int idx = it * 32 + lane;
+                v[it] = lds128(stg + (idx >> 1) * 32 + (idx & 1) * 16);
+            }
 #pragma unroll
-            for (int it = 0; it < 8; it++) {
-                const int dd = it * 8 + dsub;
-                *reinterpret_cast<uint4 *>(vt + (((size_t)b_first * ep.heads + head) * 64 + dd) * ep.tok_pitch + t0 + ch * 8) =
-                    x[it];
+            for (int it = 0; it < 4; it++) {
+                const int idx = it * 32 + lane, dd = idx >> 1;
+                *reinterpret_cast<uint4 *>(vt + (((size_t)b_first * ep.heads + head) * 64 + dd) * ep.tok_pitch + t0 +
+                                           (idx & 1) * 8) = v[it];
+            }
+        } else {
+#pragma unroll
+            for (int hf = 0; hf < 2; hf++) {
+                const int m = m0w + r + 8 * hf;
+                if (m >= M) continue;
+                const int b = m / rpb, t = m - b * rpb;
+                __nv_bfloat16 *dst = vt + ((size_t)b * ep.heads + head) * 64 * ep.tok_pitch + t;
+#pragma unroll
+                for (int jj = 0; jj < 8; jj++)
+#pragma unroll
+                    for (int e = 0; e < 2; e++)
+                        dst[(size_t)(8 * jj + 2 * c + e) * ep.tok_pitch] = __float2bfloat16(x[hf][2 * jj + e]);
             }
         }
     }
-    warp_sync_smem();       // staging buffer and hp[] are rewritten by the next call
+    warp_sync_smem();       // the staging buffer is rewritten by the next call
 }
 
-// One epilogue warp drains its half of the BN accumulator columns for its 32 rows.
+// One consumer warp drains its 16 rows x BN columns of the accumulator.
 template <int BN, int MODE>
-__device__ __forceinline__ void epilogue_tile(const GaGemmEpilogue &ep, uint32_t stg, float *hp, uint32_t trow, int lane,
-                                              int chalf, int m0w, int n0, int M, int N)
+__device__ __forceinline__ void epilogue_tile(const GaGemmEpilogue &ep, uint32_t stg, const float (&acc)[BN / 2], int lane,
+                                              int m0w, int n0, int M, int N)
 {
-    if (m0w >= M) return;                                          // warp-uniform: these 32 rows are padding
-    if (MODE == GA_EPI_HEADS) {
-#pragma unroll 1
-        for (int c = chalf * (BN / 2); c < (chalf + 1) * (BN / 2); c += 64)
-            if (n0 + c < N) epilogue_head(ep, stg, hp, trow + c, lane, m0w, n0 + c, M);
+    if (m0w >= M) return;                                          // warp-uniform: these rows are padding
+    if constexpr (MODE == GA_EPI_HEADS) {
+#pragma unroll
+        for (int h = 0; h < BN / 64; h++)
+            if (n0 + 64 * h < N) epilogue_head(ep, stg, acc, h, lane, m0w, n0 + 64 * h, M);
     } else {
-        const int c0 = chalf * (BN / 2), c1 = (chalf + 1) * (BN / 2);
-        if (n0 + c0 >= N) return;                                  // warp-uniform
-        // software pipeline over the 32-column chunks: the TMEM load of chunk c+1 is in flight while chunk c is
-        // staged and stored
-        uint32_t r[32];
-        ColParams cp;
-        load_col_params<MODE>(ep, lane, m0w, n0 + c0, N, cp);
-        tmem_ld_32x32b_x32(trow + c0, r);
-#pragma unroll 1
-        for (int c = c0; c < c1; c += 32) {
-            if (n0 + c >= N) break;                                // warp-uniform
-            tmem_ld_wait();
-            stage_rows(stg, lane, r);
-            const bool more = (c + 32 < c1) && (n0 + c + 32 < N);
-            ColParams cpn;
-            if (more) {
-                tmem_ld_32x32b_x32(trow + c + 32, r);
-                load_col_params<MODE>(ep, lane, m0w, n0 + c + 32, N, cpn);
-            }
+#pragma unroll
+        for (int ch = 0; ch < BN / 32; ch++) {
+            if (n0 + 32 * ch >= N) break;                          // warp-uniform
+            ColParams cp;
+            load_col_params<MODE>(ep, lane, m0w, n0 + 32 * ch, N, cp);
+            stage_chunk(stg, lane, acc, ch);
             warp_sync_smem();
-            epilogue32<MODE>(ep, stg, lane, m0w, n0 + c, M, N, cp);
+            epilogue_chunk<MODE>(ep, stg, lane, m0w, n0 + 32 * ch, M, N, cp);
             warp_sync_smem();
-            if (more) cp = cpn;
         }
     }
 }
 
-// Persistent: grid = min(#tiles, #SMs); every role loops over the CTA's tiles.  The TMEM accumulator is double
-// buffered (2*BN columns), so the epilogue of tile i overlaps the TMA/MMA main loop of tile i+1.
-// CS > 1: a cluster of CS CTAs works on CS vertically adjacent tiles (same n-block).  Each CTA loads its own A
-// tile and 1/CS of the shared W tile, multicast to every CTA of the cluster, so the L2 -> SM operand traffic per
-// CTA drops from (128 + BN) to (128 + BN/CS) rows per k-block -- the main loop is L2-bandwidth bound otherwise.
-template <int BN, int CS, int MODE>
+// Persistent: grid = min(#tiles, #SMs); producer and consumers walk the same tile sequence.
+template <int BN, int MODE>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                     const GaGemmEpilogue ep, const int M, const int N, const int K)
 {
     using Cfg = GemmCfg<BN>;
     extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t full_bar[Cfg::kStages], empty_bar[Cfg::kStages], acc_full[2], acc_empty[2];
-    __shared__ uint32_t tmem_slot;
+    __shared__ uint64_t full_bar[Cfg::kStages], empty_bar[Cfg::kStages];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t *smem_a = smem, *smem_b = smem + Cfg::kStages * Cfg::kABytes;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;
     const int nk = (K + BK - 1) / BK;
     const int num_m = (M + BM - 1) / BM, num_n = (N + BN - 1) / BN;
-    const int num_mg = (num_m + CS - 1) / CS;          // groups of CS m-blocks
-    const int tiles = num_mg * num_n;                  // work items per CLUSTER
-    const int crank = CS > 1 ? (int)cluster_ctarank() : 0;
-    const int cid = blockIdx.x / CS, ncl = gridDim.x / CS;
-    constexpr uint16_t kMask = (uint16_t)((1u << CS) - 1);
+    const int tiles = num_m * num_n;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         prefetch_tmap(&tma_a);
         prefetch_tmap(&tma_b);
+        for (int s = 0; s < Cfg::kStages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps); }
+        fence_barrier_init();
     }
-    if (warp == 1) {
-        if (lane == 0) {
-            for (int s = 0; s < Cfg::kStages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CS); }
-            for (int a = 0; a < 2; a++) { mbar_init(&acc_full[a], 1); mbar_init(&acc_empty[a], kEpiWarps); }
-            fence_barrier_init();
-        }
-        __syncwarp();
-        tmem_alloc<Cfg::kTmemCols>(&tmem_slot);
-    }
-    tc_fence_before();
     __syncthreads();
-    if (CS > 1) cluster_sync_all();                    // peers' barriers exist before anyone multicasts into them
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
     pdl_wait();                     // inputs (A, the residual stream, the gate table) come from earlier kernels
     pdl_launch_dependents();        // let the next kernel run its own prologue under our main loop
 
-    if (warp == 0) {
-        if (elect_one()) {
+    if (wg == 0) {
+        setmaxnreg_dec<40>();
+        if (warp == 0 && elect_one()) {
             int it = 0;
-            for (int tile = cid; tile < tiles; tile += ncl) {
-                const int m0 = ((tile % num_mg) * CS + crank) * BM, n0 = (tile / num_mg) * BN;
+            for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+                const int m0 = (tile % num_m) * BM, n0 = (tile / num_m) * BN;
                 for (int kb = 0; kb < nk; kb++, it++) {
                     const int s = it % Cfg::kStages;
-                    const uint32_t ph = (it / Cfg::kStages) & 1;
-                    mbar_wait(&empty_bar[s], ph ^ 1);       // all CS consumers released this stage
+                    mbar_wait(&empty_bar[s], ((it / Cfg::kStages) & 1) ^ 1);     // every consumer warp released it
                     mbar_expect_tx(&full_bar[s], Cfg::kABytes + Cfg::kBBytes);
                     tma_load_2d(smem_a + s * Cfg::kABytes, &tma_a, &full_bar[s], kb * BK, m0);
-                    if (CS == 1) {
-                        tma_load_2d(smem_b + s * Cfg::kBBytes, &tma_b, &full_bar[s], kb * BK, n0);
-                    } else {
-                        constexpr int kPart = Cfg::kBBytes / CS;        // this CTA's slice of the W tile
-                        tma_load_2d_mcast(smem_b + s * Cfg::kBBytes + crank * kPart, &tma_b, &full_bar[s], kb * BK,
-                                          n0 + crank * (BN / CS), kMask);
-                    }
+                    tma_load_2d(smem_b + s * Cfg::kBBytes, &tma_b, &full_bar[s], kb * BK, n0);
                 }
-            }
-        }
-    } else if (warp == 1) {
-        if (elect_one()) {
-            constexpr uint32_t idesc = umma_idesc_bf16(BM, BN);
-            int it = 0, lt = 0;
-            for (int tile = cid; tile < tiles; tile += ncl, lt++) {
-                const int a = lt & 1;
-                mbar_wait(&acc_empty[a], ((lt >> 1) & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t tacc = tmem + (uint32_t)(a * BN);
-                for (int kb = 0; kb < nk; kb++, it++) {
-                    const int s = it % Cfg::kStages;
-                    mbar_wait(&full_bar[s], (it / Cfg::kStages) & 1);
-                    tc_fence_after();
-                    const uint64_t ad = umma_desc_k_sw128(smem_u32(smem_a + s * Cfg::kABytes));
-                    const uint64_t bd = umma_desc_k_sw128(smem_u32(smem_b + s * Cfg::kBBytes));
-#pragma unroll
-                    for (int k = 0; k < BK / 16; k++)
-                        umma_bf16_ss(tacc, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), idesc, (kb | k) != 0);
-                    if (CS == 1) umma_commit(&empty_bar[s]);            // frees the smem stage when these MMAs retire
-                    else umma_commit_mcast(&empty_bar[s], kMask);       // ... in every CTA that multicasts into it
-                }
-                umma_commit(&acc_full[a]);          // accumulator of this tile complete
             }
         }
     } else {
-        const int ew = warp - 2;
-        const int q = warp & 3;                     // TMEM lane quarter this warp may access
-        const int chalf = ew >> 2;                  // which half of the BN columns this warp drains
-        const uint32_t stg = smem_u32(smem + Cfg::kRing + ew * kStageBytes);
-        float *hp = reinterpret_cast<float *>(smem + Cfg::kRing + kEpiWarps * kStageBytes) + ew * kHeadParams;
-        int lt = 0;
-        for (int tile = cid; tile < tiles; tile += ncl, lt++) {
-            const int m0 = ((tile % num_mg) * CS + crank) * BM, n0 = (tile / num_mg) * BN;
-            const int a = lt & 1;
-            mbar_wait(&acc_full[a], (lt >> 1) & 1);
-            tc_fence_after();
-            const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * BN);
-            epilogue_tile<BN, MODE>(ep, stg, hp, trow, lane, chalf, m0 + q * 32, n0, M, N);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[a]);
-        }
-    }
-    __syncthreads();
-    if (CS > 1) cluster_sync_all();                    // nobody exits while a peer can still write into its smem
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc<Cfg::kTmemCols>(tmem);
-    }
-}
-
-// ---------------------------------------------------------------------------
-// CTA-pair variant (tcgen05 cta_group::2): a cluster of two CTAs computes a 256 x BN tile.  Each CTA stages its own
-// 128 rows of A and HALF of the W tile (BN/2 rows), so the operand bytes an SM has to ingest per MMA cycle halve
-// for W -- the 1-CTA kernel's main loop is bound by exactly that ingest.  The leader issues one M=256 MMA per
-// k-step; commits are multicast to both CTAs' barriers; both CTAs run their own TMA producer and epilogue.
-// ---------------------------------------------------------------------------
-template <int BN> struct PairCfg {
-    static constexpr int kABytes = BM * BK * 2;                 // 16 KB
-    static constexpr int kBBytes = (BN / 2) * BK * 2;           // this CTA's half of the W tile
-    static constexpr int kStages = (BN >= 256) ? 5 : 7;
-    static constexpr int kRing = kStages * (kABytes + kBBytes);
-    static constexpr int kSmem = kRing + 1024 + 36 * 1024;
-    static constexpr int kTmemCols = 2 * BN;
-};
-
-template <int BN, int MODE>
-__global__ void __launch_bounds__(kThreads, 1)
-gemm_bf16_tn_pair_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
-                         const GaGemmEpilogue ep, const int M, const int N, const int K)
-{
-    using Cfg = PairCfg<BN>;
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t full_bar[Cfg::kStages], empty_bar[Cfg::kStages], acc_full[2], acc_empty[2];
-    __shared__ uint32_t tmem_slot;
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t *smem_a = smem, *smem_b = smem + Cfg::kStages * Cfg::kABytes;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int nk = (K + BK - 1) / BK;
-    const int num_m = (M + BM - 1) / BM, num_n = (N + BN - 1) / BN;
-    const int num_mg = (num_m + 1) / 2;
-    const int tiles = num_mg * num_n;                   // work items per pair
-    const int crank = (int)cluster_ctarank();
-    const bool leader = crank == 0;
-    const int cid = blockIdx.x >> 1, ncl = gridDim.x >> 1;
-
-    if (warp == 0 && lane == 0) {
-        prefetch_tmap(&tma_a);
-        prefetch_tmap(&tma_b);
-    }
-    if (warp == 1) {
-        if (lane == 0) {
-            for (int s = 0; s < Cfg::kStages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-            for (int a = 0; a < 2; a++) { mbar_init(&acc_full[a], 1); mbar_init(&acc_empty[a], 2 * kEpiWarps); }
-            fence_barrier_init();
-        }
-        __syncwarp();
-        tmem_alloc_2cta<Cfg::kTmemCols>(&tmem_slot);
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
-    pdl_wait();                     // inputs come from earlier kernels; everything above overlapped their tail
-    pdl_launch_dependents();
-
-    if (warp == 0) {
-        if (elect_one()) {
-            int it = 0;
-            for (int tile = cid; tile < tiles; tile += ncl) {
-                const int m0 = ((tile % num_mg) * 2 + crank) * BM, n0 = (tile / num_mg) * BN + crank * (BN / 2);
-                for (int kb = 0; kb < nk; kb++, it++) {
-                    const int s = it % Cfg::kStages;
-                    const uint32_t ph = (it / Cfg::kStages) & 1;
-                    mbar_wait(&empty_bar[s], ph ^ 1);
-                    if (leader) mbar_expect_tx(&full_bar[s], 2 * (Cfg::kABytes + Cfg::kBBytes));   // both CTAs' bytes
-                    tma_load_2d_2cta(smem_a + s * Cfg::kABytes, &tma_a, &full_bar[s], kb * BK, m0);
-                    tma_load_2d_2cta(smem_b + s * Cfg::kBBytes, &tma_b, &full_bar[s], kb * BK, n0);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (leader && elect_one()) {
-            constexpr uint32_t idesc = umma_idesc_bf16(2 * BM, BN);
-            int it = 0, lt = 0;
-            for (int tile = cid; tile < tiles; tile += ncl, lt++) {
-                const int a = lt & 1;
-                mbar_wait(&acc_empty[a], ((lt >> 1) & 1) ^ 1);      // both CTAs' epilogues drained this accumulator
-                tc_fence_after();
-                const uint32_t tacc = tmem + (uint32_t)(a * BN);
-                for (int kb = 0; kb < nk; kb++, it++) {
-                    const int s = it % Cfg::kStages;
-                    mbar_wait(&full_bar[s], (it / Cfg::kStages) & 1);
-                    tc_fence_after();
-                    const uint64_t ad = umma_desc_k_sw128(smem_u32(smem_a + s * Cfg::kABytes));
-                    const uint64_t bd = umma_desc_k_sw128(smem_u32(smem_b + s * Cfg::kBBytes));
+        setmaxnreg_inc<232>();
+        const int cw = wg - 1;                      // which 64-row half of the tile
+        const int wi = warp & 3;                    // 16-row slice of that half
+        const uint32_t stg = smem_u32(smem + Cfg::kRing + (cw * 4 + wi) * kStageBytes);
+        float acc[BN / 2];
+        int it = 0;
+        for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+            const int m0 = (tile % num_m) * BM, n0 = (tile / num_m) * BN;
+            for (int kb = 0; kb < nk; kb++, it++) {
+                const int s = it % Cfg::kStages;
+                mbar_wait(&full_bar[s], (it / Cfg::kStages) & 1);
+                const uint64_t ad = wgmma_desc_k_sw128(smem_u32(smem_a + s * Cfg::kABytes + cw * 64 * 128));
+                const uint64_t bd = wgmma_desc_k_sw128(smem_u32(smem_b + s * Cfg::kBBytes));
+                fence_regs(acc);
+                wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < BK / 16; k++)
-                        umma_bf16_ss_2cta(tacc, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), idesc, (kb | k) != 0);
-                    umma_commit_2cta(&empty_bar[s]);
-                }
-                umma_commit_2cta(&acc_full[a]);
+                for (int k = 0; k < BK / 16; k++)
+                    wgmma_ss<BN>(acc, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), (uint32_t)((kb | k) != 0));
+                wgmma_commit();
+                fence_regs(acc);
+                wgmma_wait<1>();                    // the previous stage's MMAs have retired: release its slot
+                fence_regs(acc);
+                if (kb > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % Cfg::kStages]);
             }
+            wgmma_wait<0>();
+            fence_regs(acc);
+            if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % Cfg::kStages]);
+            epilogue_tile<BN, MODE>(ep, stg, acc, lane, m0 + cw * 64 + wi * kWarpRows, n0, M, N);
         }
-    } else {
-        const int ew = warp - 2;
-        const int q = warp & 3;
-        const int chalf = ew >> 2;
-        const uint32_t stg = smem_u32(smem + Cfg::kRing + ew * kStageBytes);
-        float *hp = reinterpret_cast<float *>(smem + Cfg::kRing + kEpiWarps * kStageBytes) + ew * kHeadParams;
-        int lt = 0;
-        for (int tile = cid; tile < tiles; tile += ncl, lt++) {
-            const int m0 = ((tile % num_mg) * 2 + crank) * BM, n0 = (tile / num_mg) * BN;
-            const int a = lt & 1;
-            mbar_wait(&acc_full[a], (lt >> 1) & 1);
-            tc_fence_after();
-            const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * BN);
-            epilogue_tile<BN, MODE>(ep, stg, hp, trow, lane, chalf, m0 + q * 32, n0, M, N);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if (leader) mbar_arrive(&acc_empty[a]);
-                else mbar_arrive_remote(&acc_empty[a], 0);
-            }
-        }
-    }
-    __syncthreads();
-    cluster_sync_all();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc_2cta<Cfg::kTmemCols>(tmem);
     }
 }
 
@@ -609,85 +435,41 @@ int ga_make_tmap_bf16(CUtensorMap *map, const void *ptr, uint64_t rows, uint64_t
 
 static int sm_count() { return ga_sm_count(); }
 
-template <int BN, int CS, int MODE>
+template <int BN, int MODE>
 static int launch_gemm_mode(const CUtensorMap &ta, const CUtensorMap &tb, const GaGemmEpilogue &ep, int M, int N, int K,
                             cudaStream_t s)
 {
     using Cfg = GemmCfg<BN>;
     static GaPerDevice attr_set;
     if (ga_first_use_on_device(attr_set)) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_bf16_tn_kernel<BN, CS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        cudaError_t e = cudaFuncSetAttribute(gemm_bf16_tn_kernel<BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                              Cfg::kSmem);
         if (e != cudaSuccess) return (int)e;
     }
-    const int num_m = (M + BM - 1) / BM, num_n = (N + BN - 1) / BN;
-    const int items = ((num_m + CS - 1) / CS) * num_n;              // work items per cluster
-    int clusters = sm_count() / CS;
-    if (items < clusters) clusters = items;
-    dim3 grid(clusters * CS);
-    if (CS == 1)
-        return (int)ga_launch_pdl(gemm_bf16_tn_kernel<BN, CS, MODE>, grid, dim3(kThreads), (size_t)Cfg::kSmem, s, ta, tb, ep,
-                                  M, N, K);
-    return (int)ga_launch_cluster(gemm_bf16_tn_kernel<BN, CS, MODE>, grid, dim3(kThreads), (size_t)Cfg::kSmem, s,
-                                  (unsigned)CS, ta, tb, ep, M, N, K);
+    const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
+    const int grid = tiles < sm_count() ? tiles : sm_count();
+    return (int)ga_launch_pdl(gemm_bf16_tn_kernel<BN, MODE>, dim3(grid), dim3(kThreads), (size_t)Cfg::kSmem, s, ta, tb, ep,
+                              M, N, K);
 }
 
-template <int BN, int CS>
+template <int BN>
 static int launch_gemm(const void *A, int lda, const void *W, int ldw, const GaGemmEpilogue &ep, int M, int N, int K,
                        cudaStream_t s)
 {
     CUtensorMap ta, tb;
     int rc = ga_make_tmap_bf16(&ta, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, BM);
     if (rc) return rc;
-    rc = ga_make_tmap_bf16(&tb, W, (uint64_t)N, (uint64_t)K, (uint64_t)ldw, (uint32_t)(BN / CS));
+    rc = ga_make_tmap_bf16(&tb, W, (uint64_t)N, (uint64_t)K, (uint64_t)ldw, (uint32_t)BN);
     if (rc) return rc;
     switch (ep.mode) {
-    case GA_EPI_BF16: return launch_gemm_mode<BN, CS, GA_EPI_BF16>(ta, tb, ep, M, N, K, s);
-    case GA_EPI_GELU_BF16: return launch_gemm_mode<BN, CS, GA_EPI_GELU_BF16>(ta, tb, ep, M, N, K, s);
-    case GA_EPI_F32: return launch_gemm_mode<BN, CS, GA_EPI_F32>(ta, tb, ep, M, N, K, s);
-    case GA_EPI_RESID_GATE_F32: return launch_gemm_mode<BN, CS, GA_EPI_RESID_GATE_F32>(ta, tb, ep, M, N, K, s);
+    case GA_EPI_BF16: return launch_gemm_mode<BN, GA_EPI_BF16>(ta, tb, ep, M, N, K, s);
+    case GA_EPI_GELU_BF16: return launch_gemm_mode<BN, GA_EPI_GELU_BF16>(ta, tb, ep, M, N, K, s);
+    case GA_EPI_F32: return launch_gemm_mode<BN, GA_EPI_F32>(ta, tb, ep, M, N, K, s);
+    case GA_EPI_RESID_GATE_F32: return launch_gemm_mode<BN, GA_EPI_RESID_GATE_F32>(ta, tb, ep, M, N, K, s);
     case GA_EPI_HEADS:
         if (BN == 128 || BN == 256)
-            return launch_gemm_mode<((BN == 128 || BN == 256) ? BN : 128), CS, GA_EPI_HEADS>(ta, tb, ep, M, N, K, s);
+            return launch_gemm_mode<((BN == 128 || BN == 256) ? BN : 128), GA_EPI_HEADS>(ta, tb, ep, M, N, K, s);
         return GA_ERR_BADARG;
-    default: return GA_ERR_BADARG;
-    }
-}
-
-template <int BN, int MODE>
-static int launch_gemm_pair_mode(const CUtensorMap &ta, const CUtensorMap &tb, const GaGemmEpilogue &ep, int M, int N, int K,
-                                 cudaStream_t s)
-{
-    using Cfg = PairCfg<BN>;
-    static GaPerDevice attr_set;
-    if (ga_first_use_on_device(attr_set)) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_bf16_tn_pair_kernel<BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             Cfg::kSmem);
-        if (e != cudaSuccess) return (int)e;
-    }
-    const int num_m = (M + BM - 1) / BM, num_n = (N + BN - 1) / BN;
-    const int items = ((num_m + 1) / 2) * num_n;
-    int pairs = sm_count() / 2;
-    if (items < pairs) pairs = items;
-    return (int)ga_launch_cluster(gemm_bf16_tn_pair_kernel<BN, MODE>, dim3(pairs * 2), dim3(kThreads), (size_t)Cfg::kSmem, s,
-                                  2u, ta, tb, ep, M, N, K);
-}
-
-template <int BN>
-static int launch_gemm_pair(const void *A, int lda, const void *W, int ldw, const GaGemmEpilogue &ep, int M, int N, int K,
-                            cudaStream_t s)
-{
-    CUtensorMap ta, tb;
-    int rc = ga_make_tmap_bf16(&ta, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, BM);
-    if (rc) return rc;
-    rc = ga_make_tmap_bf16(&tb, W, (uint64_t)N, (uint64_t)K, (uint64_t)ldw, (uint32_t)(BN / 2));
-    if (rc) return rc;
-    switch (ep.mode) {
-    case GA_EPI_BF16: return launch_gemm_pair_mode<BN, GA_EPI_BF16>(ta, tb, ep, M, N, K, s);
-    case GA_EPI_GELU_BF16: return launch_gemm_pair_mode<BN, GA_EPI_GELU_BF16>(ta, tb, ep, M, N, K, s);
-    case GA_EPI_F32: return launch_gemm_pair_mode<BN, GA_EPI_F32>(ta, tb, ep, M, N, K, s);
-    case GA_EPI_RESID_GATE_F32: return launch_gemm_pair_mode<BN, GA_EPI_RESID_GATE_F32>(ta, tb, ep, M, N, K, s);
-    case GA_EPI_HEADS: return launch_gemm_pair_mode<BN, GA_EPI_HEADS>(ta, tb, ep, M, N, K, s);
     default: return GA_ERR_BADARG;
     }
 }
@@ -696,26 +478,14 @@ extern "C" int ga_gemm_bf16_tn(const void *A, int lda, const void *W, int ldw, i
                                const GaGemmEpilogue *epi, int block_n, void *stream)
 {
     if (!A || !W || !epi || M <= 0 || N <= 0 || K <= 0) return GA_ERR_BADARG;
-    // block_n = tile width {64,128,256} + 1000 * cluster size {1 (default), 2}; 9000 + width = CTA pair
-    const int cs = block_n >= 1000 ? block_n / 1000 : 1;
-    const int bn = block_n % 1000;
+    // block_n = tile width {64, 128, 192, 256}
+    const int bn = block_n;
     if (epi->mode == GA_EPI_HEADS && (N % 64 != 0 || epi->heads <= 0 || bn < 128)) return GA_ERR_BADARG;
     if (bn != 64 && bn != 128 && bn != 192 && bn != 256) return GA_ERR_BADARG;
-    if (bn == 192 && (cs != 1 || epi->mode == GA_EPI_HEADS)) return GA_ERR_BADARG;        // 96 columns per epilogue warp: no whole heads
+    if (bn == 192 && epi->mode == GA_EPI_HEADS) return GA_ERR_BADARG;        // 192 is not a whole number of heads per half
     cudaStream_t s = (cudaStream_t)stream;
-    if (cs == 1) {
-        if (bn == 64) return launch_gemm<64, 1>(A, lda, W, ldw, *epi, M, N, K, s);
-        if (bn == 128) return launch_gemm<128, 1>(A, lda, W, ldw, *epi, M, N, K, s);
-        if (bn == 192) return launch_gemm<192, 1>(A, lda, W, ldw, *epi, M, N, K, s);
-        return launch_gemm<256, 1>(A, lda, W, ldw, *epi, M, N, K, s);
-    }
-    if (cs == 2) {
-        if (bn == 128) return launch_gemm<128, 2>(A, lda, W, ldw, *epi, M, N, K, s);
-        if (bn == 256) return launch_gemm<256, 2>(A, lda, W, ldw, *epi, M, N, K, s);
-    }
-    if (cs == 9) {          // 9xxx: CTA pair (cta_group::2), 256 x bn tile per pair
-        if (bn == 128) return launch_gemm_pair<128>(A, lda, W, ldw, *epi, M, N, K, s);
-        if (bn == 256) return launch_gemm_pair<256>(A, lda, W, ldw, *epi, M, N, K, s);
-    }
-    return GA_ERR_BADARG;
+    if (bn == 64) return launch_gemm<64>(A, lda, W, ldw, *epi, M, N, K, s);
+    if (bn == 128) return launch_gemm<128>(A, lda, W, ldw, *epi, M, N, K, s);
+    if (bn == 192) return launch_gemm<192>(A, lda, W, ldw, *epi, M, N, K, s);
+    return launch_gemm<256>(A, lda, W, ldw, *epi, M, N, K, s);
 }

@@ -1,5 +1,5 @@
 // Row-wise / small kernels of the DiT denoiser (everything that is not a
-// tcgen05 contraction): fused RMSNorm + adaLN modulate, the timestep /
+// wgmma contraction): fused RMSNorm + adaLN modulate, the timestep /
 // pooled-vector / adaLN prologue, the token embedder, the final layer with the
 // classifier-free-guidance combine, and the ODE state update.
 // Math follows /root/reference/dit/dit_i23d.py:511-567,707-750,
@@ -244,7 +244,7 @@ embed_fc1_kernel(const float *__restrict__ xin, int Cx, const float *__restrict_
 }
 
 // NeRF positional encoding of xyz (utils/nerf_utils.py:50-65, multires 10): [x, sin(2^k x), cos(2^k x)]_k,
-// 63 features padded to 64 (bf16) so the projection is one tcgen05 GEMM with K = 64.
+// 63 features padded to 64 (bf16) so the projection is one wgmma GEMM with K = 64.
 __global__ void xyz_pe_kernel(const float *__restrict__ xyz, __nv_bfloat16 *__restrict__ out, int R)
 {
     const int r = blockIdx.x * blockDim.x + threadIdx.x;

@@ -320,4 +320,4 @@ extern "C" int ga_raster_backward_ex(const float *gauss13, int batch, int P, int
     return 0;
 }
 
-extern "C" const char *ga_b200_version(void) { return "ga_b200 0.1 (sm_100a)"; }
+extern "C" const char *ga_b200_version(void) { return "ga_b200 0.1 (sm_90a)"; }

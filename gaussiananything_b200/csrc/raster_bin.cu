@@ -11,6 +11,7 @@
 // sort, without a host read-back and with ~3 passes over 8-byte keys instead
 // of ~10 over 12-byte pairs.
 #include "raster_common.cuh"
+#include "device_once.cuh"
 
 #define SCAN_THREADS 1024
 #define SORT_WARP_MAX 512          // tiles up to this many instances are sorted by a single warp in registers
@@ -284,7 +285,7 @@ cudaError_t ga_launch_binning(const RasterDims &d, const RasterWs &w, cudaStream
     }
     dim3 grid((d.P + 255) / 256, d.NV);
     scatter_kernel<<<grid, 256, 0, s>>>(d, w);
-    const int big_grid = d.NV * d.T < 148 * 7 ? d.NV * d.T : 148 * 7;      // 32 KB of keys per block: 7 blocks per SM
+    const int big_grid = d.NV * d.T < ga_sm_count() * 7 ? d.NV * d.T : ga_sm_count() * 7;      // 32 KB of keys per block: 7 blocks per SM
     // the few tiles above the warp-sort limit are sorted by whole blocks (a long tail of a handful of CTAs): on the
     // side stream, beside the warp-per-tile kernel that fills the GPU, instead of after it
     GaSide *g = ga_side();

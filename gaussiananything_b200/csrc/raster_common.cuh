@@ -1,4 +1,4 @@
-// Shared definitions of the surfel rasteriser kernels (sm_100a).
+// Shared definitions of the surfel rasteriser kernels (sm_90a).
 // Algorithm: github.com/hbb1/diff-surfel-rasterization as called by
 // /root/reference/nsr/gs_surfel.py:85-114; constants per SURVEY.md App. A.
 #pragma once
@@ -26,7 +26,7 @@ struct RasterDims {
     int H, W, gx, gy, T;       // T = gx*gy tiles per image
     float scale_modifier;
     int64_t max_instances;
-    // the two unpinned judgement calls of the restatement (DESIGN.md 1), switchable so that pinning against
+    // the two unpinned judgement calls of the restatement (oracle/surfel_oracle.c), switchable so that pinning against
     // upstream is a flip of the defaults below; ga_raster_set_variant() overrides them at run time (tests)
     int list_k;                // > 0: the forward records every pixel's contributions (<= list_k per pixel), see RasterWs.lists
     int radius_formula;        // 0: ceil(max(ex, ey, 3*FilterSize))   1: ceil(3*max(ex, ey, FilterSize))

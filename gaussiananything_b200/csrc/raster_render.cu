@@ -13,7 +13,7 @@
 //    gradient over the warp with shuffles, over the CTA in shared memory, and
 //    issues one global atomic per (tile, surfel, component).
 #include "raster_common.cuh"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 #include "device_once.cuh"
 #include <cstdlib>
 
@@ -772,8 +772,8 @@ struct BwdASmem {
 __device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gsrc, uint32_t bytes, uint64_t *bar)
 {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(
-                     sm100::smem_u32(smem_dst)),
-                 "l"(gsrc), "r"(bytes), "r"(sm100::smem_u32(bar))
+                     sm90::smem_u32(smem_dst)),
+                 "l"(gsrc), "r"(bytes), "r"(sm90::smem_u32(bar))
                  : "memory");
 }
 
@@ -857,8 +857,8 @@ render_bwd_a_kernel(RasterDims d, RasterWs ws, BwdLists L, const float *__restri
         sm.maxn = 0;
         if (LISTS) {
 #pragma unroll
-            for (int i = 0; i < BWD_A_RING; i++) { sm100::mbar_init(&s_full[i], 1); sm100::mbar_init(&s_empty[i], 8); }
-            sm100::fence_barrier_init();
+            for (int i = 0; i < BWD_A_RING; i++) { sm90::mbar_init(&s_full[i], 1); sm90::mbar_init(&s_empty[i], 8); }
+            sm90::fence_barrier_init();
         }
     }
     __syncthreads();
@@ -878,8 +878,8 @@ render_bwd_a_kernel(RasterDims d, RasterWs ws, BwdLists L, const float *__restri
     const int maxn = sm.maxn;
     auto issue_row = [&](const int j) {                                   // thread 0 only: j-th row in processing order
         const int slot = j % BWD_A_RING, use = j / BWD_A_RING;
-        if (use > 0) sm100::mbar_wait(&s_empty[slot], (uint32_t)((use - 1) & 1));      // all 8 warps are done with its last row
-        sm100::mbar_expect_tx(&s_full[slot], 4096u);
+        if (use > 0) sm90::mbar_wait(&s_empty[slot], (uint32_t)((use - 1) & 1));      // all 8 warps are done with its last row
+        sm90::mbar_expect_tx(&s_full[slot], 4096u);
         bulk_g2s(&s_rows[slot][0], tile_rows + (size_t)(maxn - 1 - j) * 4096, 4096u, &s_full[slot]);
     };
     if (LISTS) {
@@ -967,13 +967,13 @@ render_bwd_a_kernel(RasterDims d, RasterWs ws, BwdLists L, const float *__restri
             for (int j = 0; j < maxn; j++) {
                 const int k = maxn - 1 - j, slot = j % BWD_A_RING;
                 if (threadIdx.x == 0 && j + BWD_A_RING - 2 < maxn) issue_row(j + BWD_A_RING - 2);
-                sm100::mbar_wait(&s_full[slot], (uint32_t)((j / BWD_A_RING) & 1));
+                sm90::mbar_wait(&s_full[slot], (uint32_t)((j / BWD_A_RING) & 1));
                 if (nl > k) {
                     const uint4 cur = s_rows[slot][pix_local];
                     contribute(hi - 1 - (int)cur.x, (int)cur.x, __uint_as_float(cur.y), __uint_as_float(cur.z));
                 }
                 __syncwarp();
-                if (lane == 0) sm100::mbar_arrive(&s_empty[slot]);          // this warp has read row k out of the slot
+                if (lane == 0) sm90::mbar_arrive(&s_empty[slot]);          // this warp has read row k out of the slot
             }
         } else if (LISTS) {
             while (true) {

@@ -1,5 +1,5 @@
-// Row-wise kernels of the VAE decode path latent tokens -> surfels (SURVEY.md 8f row N1; DESIGN.md 6b): everything
-// around the tcgen05 GEMMs / attention that the DiT kernels do not already cover.
+// Row-wise kernels of the VAE decode path latent tokens -> surfels (SURVEY.md 8f row N1): everything
+// around the wgmma GEMMs / attention that the DiT kernels do not already cover.
 //   layernorm_modulate : LayerNorm [* w + b] [* (1 + scale[row]) + shift[row]] -> bf16      (DiTBlock2, PreNorm)
 //   thin_linear        : [LayerNorm affine] [SiLU] x . W^T + b with <= 16 outputs              (conv_sr, residual heads)
 //   micro_attention    : qk-normed attention over sequences of <= 16 tokens, one warp per (sequence, head)

@@ -9,7 +9,7 @@ Same constructor arguments, attribute names and state_dict key layout (a
 reference checkpoint loads with strict=True), same `forward(x, timesteps,
 context)` / `forward_with_cfg(x, t, context, cfg_scale)` contracts.  The
 forward pass does no arithmetic in torch: every op is a kernel of
-libga_b200.so (tcgen05 GEMMs with fused epilogues, tcgen05 flash attention,
+libga_b200.so (wgmma GEMMs with fused epilogues, wgmma flash attention,
 fused RMSNorm+modulate, ...) enqueued on the current CUDA stream, optionally
 replayed from a CUDA graph.  There is no CPU / eager fallback.
 
@@ -74,19 +74,20 @@ def _ck(rc, what):
 
 
 _GEMM_CFG_ENV = None
+_SMS = 132                # H100 SXM: one persistent GEMM CTA per SM
 
 
 def _gemm_config(M, N, mode=None):
-    """Tile width (+ 1000 * cluster size, ga_b200.h) from a two-term cost model fitted to the round-2 sweep
-    (tools/sweep_gemm.py, profiles/r02_gemm_sweep.txt, cuBLAS column as yardstick):
+    """Tile width (ga_b200.h) from a two-term cost model checked against the H100 sweep
+    (tools/sweep_gemm.py, profiles/gemm_sweep_h100.txt):
 
-        cost(BN) = ceil(tiles(BN) / 148) * (BN + 64)
+        cost(BN) = ceil(tiles(BN) / 132) * (BN + 64)
 
     -- waves of the persistent grid times the per-tile work (the main loop scales with BN, the +64 is the fixed
-    TMA-fill / epilogue-drain share that makes wide tiles more efficient per byte).  It reproduces the measured winner on
-    all nine DiT shapes: 192 for 4096x768 (K = 768: 8.1 vs 9.5 us; K = 3072: 16.6 vs 21.8), 4096x3072 and 1536x4096,
-    256 for 4096x2304 and 1536x3072, 128 for the under-filled 1536x1024 GEMMs of the deployed size.
-    The HEADS epilogue (whole 64-wide heads per half tile: 128 or 256 only) stays at 128.  GA_B200_GEMM_CFG="big,small" overrides."""
+    TMA-fill / epilogue-drain share that makes wide tiles more efficient per byte).  It picks the measured winner on
+    all nine DiT shapes: 192 for 4096x768 (11.3 vs 13.1 us at 256), 4096x2304, 1536x3072 and 1536x4096, 256 for
+    4096x3072 and 2738x1536, 128 for the under-filled 1536x1024 GEMMs of the deployed size.
+    The HEADS epilogue (whole 64-wide heads per warpgroup: 128 or 256 only) stays at 128.  GA_B200_GEMM_CFG="big,small" overrides."""
     global _GEMM_CFG_ENV
     if _GEMM_CFG_ENV is None:
         import os
@@ -102,7 +103,7 @@ def _gemm_config(M, N, mode=None):
         if bn > 128 and N < bn:
             continue
         tiles = rows * -(-N // bn)
-        cost = -(-tiles // 148) * (bn + 64)
+        cost = -(-tiles // _SMS) * (bn + 64)
         if best_cost is None or cost < best_cost:
             best, best_cost = bn, cost
     return best
@@ -217,7 +218,7 @@ class DiT_I23D_PCD_PixelArt_noclip(nn.Module):
         if has_caption:
             raise NotImplementedError("caption conditioning is not on the deployed i23d path")
         if hidden_size % num_heads or hidden_size // num_heads != 64:
-            raise ValueError("the B200 attention kernel is specialised for head_dim 64 (all reference archs)")
+            raise ValueError("the attention kernel is specialised for head_dim 64 (all reference archs)")
         assert roll_out
         self.depth, self.mlp_ratio, self.learn_sigma = depth, mlp_ratio, learn_sigma
         self.in_channels = in_channels
@@ -635,7 +636,7 @@ def DiT_L_Pixelart_clay_pcd_stage2(**kw):
 def DiT_B_Pixelart_clay_pcd_stage2(**kw):
     # As in the reference (dit_i23d.py:1554-1559) this entry leaves num_heads at its default of 16, i.e.
     # head_dim 48, and conditions by concatenation (use_pe_cond=False).  head_dim 48 is not supported by the
-    # B200 attention kernel, so constructing it raises ValueError; the deployed stage-2 model is the -L entry.
+    # attention kernel, so constructing it raises ValueError; the deployed stage-2 model is the -L entry.
     return DiT_I23D_PCD_PixelArt_noclip_clay_stage2(depth=12, use_clay_ca=True, hidden_size=768, **kw)
 
 

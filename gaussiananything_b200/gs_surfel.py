@@ -2,7 +2,7 @@
 
 Same constructor, attributes and `render(...)` signature / return dict, but the
 B x V Python loop (reference lines 65-176: >= 6 launches + one device-to-host
-read per view) is a single batched launch set of the B200 kernels; the
+read per view) is a single batched launch set of the CUDA kernels; the
 per-view post-processing (reference lines 121-163) is applied to the whole
 [B,V,...] batch at once.
 """

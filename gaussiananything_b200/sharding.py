@@ -3,7 +3,7 @@ samples decoded where they were sampled, ONE all-gather of the decoded surfels, 
 an interleaved share of all (sample, view) pairs.  No collective inside any kernel.
 
 The reference has no multi-GPU inference at all (scripts/gradio_app_cascaded.py:96-100 pins world size 1);
-this is the B200-native addition BASELINE.json's north_star asks for.  Works with NCCL (GPU) and gloo
+this is the GPU-native addition BASELINE.json's north_star asks for.  Works with NCCL (GPU) and gloo
 (CPU, used by the tests for the host logic)."""
 from typing import List, Tuple
 

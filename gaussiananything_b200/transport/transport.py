@@ -1,7 +1,7 @@
 """`Transport` and `Sampler` with the public surface of
 /root/reference/transport/transport.py:46-489 (SiT-style flow matching).
 
-Host-side logic only: the model evaluations it drives are the B200 DiT kernels
+Host-side logic only: the model evaluations it drives are the CUDA DiT kernels
 when `model` is a gaussiananything_b200.dit module (any callable works).
 """
 import enum

@@ -8,7 +8,7 @@ Mirrors what the reference's deployed decoder class does between DiT sampling an
 `SurfelDecoder(state_dict, ...)` takes the reference module's state_dict (keys vit_decoder.*, superresolution.*);
 `decode(latent_normalized, query_pcd_xyz)` returns the same entries the reference's ret_dict carries
 (gaussians_base, gaussians_upsampled{,_2,_3}, gaussians).  No torch arithmetic: every op is a kernel of libga_b200.so
-(tcgen05 GEMMs with fused epilogues, tcgen05 attention for the DiT2 blocks, one-warp-per-sequence attention for the
+(wgmma GEMMs with fused epilogues, wgmma attention for the DiT2 blocks, one-warp-per-sequence attention for the
 up-samplers' micro-sequences, row kernels).  bf16 tensor-core operands, fp32 residual streams.  No CPU fallback.
 """
 import ctypes as C

@@ -1,5 +1,5 @@
 /*
- * ga_b200.h -- C ABI of libga_b200.so: B200 (sm_100a) kernels for the two hot
+ * ga_b200.h -- C ABI of libga_b200.so: H100 (sm_90a) kernels for the two hot
  * paths of GaussianAnything.  Plain pointers and sizes only; no torch types.
  *
  * All pointers are DEVICE pointers unless stated otherwise.  No entry point
@@ -198,7 +198,7 @@ int ga_raster_backward(const float *gauss13, int batch, int P, int views,
  * ---------------------------------------------------------------------------
  */
 
-/* Epilogues fused into the tcgen05 GEMM  C[M,N] = A[M,K] * W[N,K]^T (+ bias). */
+/* Epilogues fused into the wgmma GEMM  C[M,N] = A[M,K] * W[N,K]^T (+ bias). */
 #define GA_EPI_BF16            0   /* out bf16 [M, ld_out]                                   */
 #define GA_EPI_GELU_BF16       1   /* out bf16 = gelu_erf(acc + bias)   (FusedMLP first half) */
 #define GA_EPI_F32             2   /* out fp32 [M, ld_out]                                   */
@@ -223,9 +223,7 @@ typedef struct GaGemmEpilogue {
 } GaGemmEpilogue;
 
 /* A [M, lda] bf16 row-major, W [N, ldw] bf16 row-major (nn.Linear weight), K contiguous in both.
- * block_n = tile width {64, 128, 192, 256} (the 128 x width output tile; 192: not for GA_EPI_HEADS) + 1000 * cluster size {1, 2}: a cluster of
- * CTAs on vertically adjacent tiles shares the W tile through TMA multicast (e.g. 4256 = width 256, cluster 4);
- * 9000 + width {128, 256} = CTA pair (tcgen05 cta_group::2) computing a 256 x width tile.
+ * block_n = tile width {64, 128, 192, 256} of the 128 x width output tile (192: not for GA_EPI_HEADS).
  * lda, ldw multiples of 8. */
 int ga_gemm_bf16_tn(const void *A, int lda, const void *W, int ldw, int M, int N, int K,
                     const GaGemmEpilogue *epi, int block_n, void *stream);
@@ -265,7 +263,7 @@ int ga_cfg_combine(const float *eps, float *out, int64_t half_elems, float cfg_s
 int ga_axpy(float *x, const float *v, float a, int64_t n, void *stream);          /* x += a v */
 int ga_f32_to_bf16(const float *x, void *y, int64_t n, void *stream);
 
-/* ---- VAE decode path latent tokens -> surfels (SURVEY 8f row N1; building blocks, see DESIGN.md 6b) -------------
+/* ---- VAE decode path latent tokens -> surfels (SURVEY 8f row N1; building blocks) -------------
  * Replaces the elementwise / small-matrix torch ops of /root/reference/vit/vit_triplane.py:287-345,991-1064,1289-1313,
  * 1388-1440, /root/reference/dit/dit_decoder.py:15-42 and /root/reference/nsr/srt/layers.py:82-90,146-186. */
 /* out_bf16[r] = LayerNorm(x[r]) [* w + bias] [* (1 + scale[b]) + shift[b]], b = r / rows_per_batch (1 = per token);

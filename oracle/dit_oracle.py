@@ -148,11 +148,11 @@ def forward_with_cfg(sd, x, t, context, cfg_scale, num_heads, depth, emulate_bf1
 
 def load_golden(path):
     """Reads a tests/golden/dit_*.npz written by make_dit_golden.py."""
-    import numpy as np
-    z = np.load(path)
-    sd = {k[4:]: torch.from_numpy(z[k].copy()).view(torch.bfloat16).float() for k in z.files if k.startswith("sd__")}
-    ctx = {k[5:]: torch.from_numpy(z[k]) for k in z.files if k.startswith("ctx__")}
-    acts = {k[5:]: torch.from_numpy(z[k]) for k in z.files if k.startswith("act__")}
+    from oracle.golden_io import load_parts
+    z = load_parts(path)
+    sd = {k[4:]: torch.from_numpy(z[k].copy()).view(torch.bfloat16).float() for k in z if k.startswith("sd__")}
+    ctx = {k[5:]: torch.from_numpy(z[k]) for k in z if k.startswith("ctx__")}
+    acts = {k[5:]: torch.from_numpy(z[k]) for k in z if k.startswith("act__")}
     meta = [int(v) for v in z["meta"]]
     cfg = dict(depth=meta[0], hidden=meta[1], heads=meta[2], cin=meta[3], ctx_dim=meta[4], stage2=bool(meta[5]),
                use_pe=bool(meta[6]))

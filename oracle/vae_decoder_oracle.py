@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE ONLY.  Pinned: tests/test_oracle_vae.py checks this file against golden vectors that
 tests/golden/make_vae_golden.py produced by running the reference's own code on CPU (third-party xformers / timm ops
-stubbed by their published semantics, tests/golden/_ref_stubs.py).  No CUDA path exists for this row yet (DESIGN.md 6b);
+stubbed by their published semantics, tests/golden/_ref_stubs.py).  No CUDA path exists for this row yet;
 the oracle and the goldens are the first step of building it.
 
 Follows:
@@ -120,17 +120,17 @@ def decode(sd, latent, query_xyz, num_heads, depth, scene_max=0.45, skip_weight=
 
 
 def load_golden(path):
-    import numpy as np
-    z = np.load(path)
+    from oracle.golden_io import load_parts
+    z = load_parts(path)
     sd = {}
-    for k in z.files:
+    for k in z:
         if k.startswith("w:"):
             bits = torch.from_numpy(z[k].astype("int32")).to(torch.int32) << 16
             sd[k[2:]] = bits.view(torch.float32)
         elif k.startswith("f:"):
             sd[k[2:]] = torch.from_numpy(z[k])
     D, depth, heads, zc, B, N = [int(v) for v in z["meta"]]
-    out = {k[4:]: torch.from_numpy(z[k]) for k in z.files if k.startswith("out_")}
+    out = {k[4:]: torch.from_numpy(z[k]) for k in z if k.startswith("out_")}
     return dict(sd=sd, D=D, depth=depth, heads=heads, latent=torch.from_numpy(z["in_latent"]),
                 xyz=torch.from_numpy(z["in_xyz"]), out=out, scene_max=float(z["scene_range_max"]),
                 skip_weight=float(z["skip_weight"]))

@@ -19,6 +19,8 @@ from _ref_stubs import *  # noqa: F401,F403  (installs the stubs, exposes torch 
 import torch, torch.nn as nn, torch.nn.functional as F
 import io, contextlib, os
 import numpy as np
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+from oracle.golden_io import save_parts  # noqa: E402
 from dit import dit_i23d, dit_models_xformers as dmx
 import transport as ref_transport
 
@@ -78,7 +80,8 @@ def run(name, cls, seed, B, N, M, Cin, ctx_dim, stage2, **kw):
                 **{"act__" + k: v.numpy() for k, v in acts.items()})
     save["meta"] = np.array([kw["depth"], kw["hidden_size"], kw["num_heads"], Cin, ctx_dim, int(stage2),
                              int(kw.get("use_pe_cond", False))])
-    np.savez_compressed(os.path.join(OUT, name + ".npz"), **save)
+    # the second block's weights go to <name>.part2.npz: every committed file stays under 1 MB
+    save_parts(os.path.join(OUT, name + ".npz"), save, {k for k in save if k.startswith("sd__blocks.1.")})
     print(name, "params", sum(v.numel() for v in sd.values()), "|y|", float(y.abs().mean()))
 
 

@@ -15,6 +15,8 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from _ref_stubs import *  # noqa: F401,F403  (installs the stubs, puts /root/reference on sys.path)
 import numpy as np
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+from oracle.golden_io import save_parts  # noqa: E402
 import torch
 
 from guided_diffusion import dist_util
@@ -74,7 +76,7 @@ def main():
         else:
             save["f:" + k] = v.float().numpy()
     path = os.path.join(OUT, "vae_decoder_small.npz")
-    np.savez_compressed(path, **save)
+    save_parts(path, save, {"out_gaussians_upsampled_2", "out_gaussians_upsampled_3"})     # every file under 1 MB
     print(path, "params", sum(p.numel() for p in m.parameters()), "kB", os.path.getsize(path) // 1024,
           {k: save[k].shape for k in save if k.startswith("out_")})
 

@@ -1,10 +1,10 @@
-"""GPU parity tests of the DiT path: tcgen05 GEMM epilogues, tcgen05 attention, row kernels (each against a
+"""GPU parity tests of the DiT path: wgmma GEMM epilogues, wgmma attention, row kernels (each against a
 plain torch fp32 reference of the same op on bf16-rounded inputs), then the whole denoiser and the sampler
 against the oracle on the golden vectors generated from the reference's own code.
 
 Tolerances: operands are bf16 (as under the reference's autocast), accumulation fp32.  Against the
 bf16-emulating oracle (same operands rounded) the bar is 6e-3 rel-L2 (1.5 bf16 eps); against the fp32 golden 2e-2.
-BASELINE.json's 1e-4 is only reachable with fp32 operands -- see DESIGN.md "DiT precision"."""
+BASELINE.json's 1e-4 is only reachable with fp32 operands."""
 import ctypes as C
 import math
 import os

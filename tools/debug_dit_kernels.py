@@ -1,4 +1,4 @@
-"""GPU diagnostics for the tcgen05 kernels (prints errors instead of asserting)."""
+"""GPU diagnostics for the wgmma kernels (prints errors instead of asserting)."""
 import ctypes as C
 import math
 import sys

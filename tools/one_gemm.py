@@ -1,4 +1,4 @@
-"""Run one tcgen05 GEMM configuration a few times (for ncu): python tools/one_gemm.py M N K cfg [gelu]."""
+"""Run one wgmma GEMM configuration a few times (for ncu): python tools/one_gemm.py M N K cfg [gelu]."""
 import ctypes as C
 import math
 import sys

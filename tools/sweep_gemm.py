@@ -1,4 +1,4 @@
-"""GPU sweep of the tcgen05 GEMM tile / cluster configurations on the DiT shapes (prints a table)."""
+"""GPU sweep of the wgmma GEMM tile widths on the DiT shapes (prints a table)."""
 import ctypes as C
 import math
 import sys
@@ -13,7 +13,7 @@ dev = torch.device("cuda:0")
 st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 shapes = [(4096, 768, 768), (4096, 2304, 768), (4096, 3072, 768), (4096, 768, 3072),
           (1536, 1024, 1024), (1536, 3072, 1024), (1536, 4096, 1024), (1536, 1024, 4096), (2738, 1536, 1024)]
-cfgs = [64, 128, 192, 256, 9128]
+cfgs = [64, 128, 192, 256]
 MODE = dit.EPI_GELU_BF16 if "gelu" in sys.argv else (dit.EPI_RESID_GATE_F32 if "resid" in sys.argv else dit.EPI_BF16)
 for (M, N, K) in shapes:
     torch.manual_seed(0)

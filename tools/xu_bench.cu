@@ -1,5 +1,5 @@
 // Micro-benchmark: sustained MUFU.EX2 rate per SM for the softmax instruction mix (build + run on the GPU box:
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o /tmp/xu_bench tools/xu_bench.cu && /tmp/xu_bench)
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o /tmp/xu_bench tools/xu_bench.cu && /tmp/xu_bench)
 #include <cstdio>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
