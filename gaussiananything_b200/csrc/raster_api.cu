@@ -110,11 +110,11 @@ extern "C" int ga_raster_layout_ex(int batch, int P, int views, int H, int W,
     L->ids = off;        off = align_up(off + mi * sizeof(uint32_t), 256);
     L->final_T = off;    off = align_up(off + (size_t)d.NV * 3 * HW * sizeof(float), 256);
     L->n_contrib = off;  off = align_up(off + (size_t)d.NV * 2 * HW * sizeof(int32_t), 256);
-    L->inst_off = off;   off = align_up(off + mi * sizeof(uint32_t), 256);
+    L->inst_off = off;                                                       // unused, 0 bytes
     L->inst_cnt = off;   off = align_up(off + mi * sizeof(uint32_t), 256);
     L->n_list = off;     off = align_up(off + (list_k ? (size_t)d.NV * HW * sizeof(int32_t) : 0), 256);
     L->tile_flag = off;  off = align_up(off + (list_k ? NVT * sizeof(uint32_t) : 0), 256);
-    L->tile_rec_start = off; off = align_up(off + (list_k ? (NVT + 1) * sizeof(uint32_t) : 0), 256);
+    L->tile_rec_start = off;                                                 // unused, 0 bytes
     L->lists = off;      off = align_up(off + (size_t)list_k * NVT * 256 * 16, 256);
     L->total_bytes = off;
     return 0;
@@ -133,11 +133,9 @@ static void carve(const GaRasterLayout &L, void *base, RasterWs *w)
     w->ids = (uint32_t *)(p + L.ids);
     w->final_T = (float *)(p + L.final_T);
     w->n_contrib = (int32_t *)(p + L.n_contrib);
-    w->inst_off = (uint32_t *)(p + L.inst_off);
     w->inst_cnt = (uint32_t *)(p + L.inst_cnt);
     w->n_list = (int32_t *)(p + L.n_list);
     w->tile_flag = (uint32_t *)(p + L.tile_flag);
-    w->tile_rec_start = (uint32_t *)(p + L.tile_rec_start);
     w->lists = (uint4 *)(p + L.lists);
 }
 
@@ -171,9 +169,7 @@ static int raster_forward_impl(int stage, const float *gauss13, int batch, int P
     }
     if (stage == 0 || stage == 2) {
         if (list_k && (e = cudaMemsetAsync(w.tile_flag, 0, (size_t)d.NV * d.T * sizeof(uint32_t), s)) != cudaSuccess) return (int)e;
-        if (list_k) e = ga_launch_render_fwd_with_slices(d, w, bg, out_color, out_allmap, s);
-        else e = ga_launch_render_fwd(d, w, bg, out_color, out_allmap, s);
-        if (e != cudaSuccess) return (int)e;
+        if ((e = ga_launch_render_fwd(d, w, bg, out_color, out_allmap, s)) != cudaSuccess) return (int)e;
         prof(3, s);
     }
     return 0;
@@ -238,21 +234,13 @@ extern "C" int ga_raster_forward_render(const float *gauss13, int batch, int P, 
                                out_allmap, out_radii, workspace, workspace_bytes, max_instances, stream);
 }
 
-// Backward scratch = gradient accumulators [NV*P][18] | tile slice starts (room for the largest tile grid, 255 x 255
-// per image) | flag | record lists of the split backward: GA_BWD_RECORDS_PER_SURFEL 16-byte records per (surfel,
-// view).  The lists need sum over instances of the cull-box area inside the tile (~26 per instance on C2, i.e. ~45 per
-// surfel-view); scenes that need more fall back to the fused kernel on the device (no error, no host sync).
-#ifndef GA_BWD_RECORDS_PER_SURFEL
-#define GA_BWD_RECORDS_PER_SURFEL 64
-#endif
+// Backward scratch = gradient accumulators [NV*P][18]; the per-(pixel, surfel) records stay in shared memory
 static size_t bwd_acc_bytes(int batch, int P, int views) { return align_up((size_t)batch * views * P * GA_GRAD_F * sizeof(float), 256); }
-static size_t bwd_tiles_bytes(int batch, int views) { return align_up(((size_t)batch * views * 255 * 255 + 1) * sizeof(uint32_t), 256); }
 
 extern "C" size_t ga_raster_backward_scratch_bytes(int batch, int P, int views)
 {
     if (batch <= 0 || P <= 0 || views <= 0) return 0;
-    return bwd_acc_bytes(batch, P, views) + bwd_tiles_bytes(batch, views) + 256 +
-           align_up((size_t)batch * views * P * GA_BWD_RECORDS_PER_SURFEL * 16, 256);
+    return bwd_acc_bytes(batch, P, views);
 }
 
 extern "C" int ga_raster_backward(const float *gauss13, int batch, int P, int views,
@@ -287,7 +275,7 @@ extern "C" int ga_raster_backward_ex(const float *gauss13, int batch, int P, int
     GaRasterLayout L;
     ga_raster_layout_ex(batch, P, views, H, W, max_instances, list_k, &L);
     if (workspace_bytes < L.total_bytes) return GA_ERR_WORKSPACE;
-    const size_t need = bwd_acc_bytes(batch, P, views);                 // the accumulators are mandatory, the lists optional
+    const size_t need = bwd_acc_bytes(batch, P, views);                 // a larger buffer is accepted; the rest is unused
     if (scratch_bytes < need) return GA_ERR_WORKSPACE;
     RasterWs w;
     carve(L, const_cast<void *>(workspace), &w);
@@ -296,23 +284,7 @@ extern "C" int ga_raster_backward_ex(const float *gauss13, int batch, int P, int
     float *grad_acc = (float *)scratch;
     prof(4, s);
     if ((e = cudaMemsetAsync(grad_acc, 0, need, s)) != cudaSuccess) return (int)e;
-    BwdLists lists = {};
-    {
-        // a caller that passes only the accumulators (the round-1 scratch size) gets the fused kernel
-        const size_t fixed = need + bwd_tiles_bytes(batch, views) + 256;
-        if (scratch_bytes > fixed + 4096) {
-            char *p = (char *)scratch + need;
-            lists.tile_rec_start = (uint32_t *)p;
-            lists.records = (uint4 *)(p + bwd_tiles_bytes(batch, views) + 256);
-            const size_t cap = (scratch_bytes - fixed) / 16;
-            lists.capacity = (uint32_t)(cap > 0xfffffff0ull ? 0xfffffff0ull : cap);
-            lists.inst_off = w.inst_off;
-            lists.inst_cnt = w.inst_cnt;
-            const size_t mi = (size_t)(max_instances > 0 ? max_instances : 1);
-            if ((e = cudaMemsetAsync(w.inst_cnt, 0, mi * sizeof(uint32_t), s)) != cudaSuccess) return (int)e;
-        }
-    }
-    if ((e = ga_launch_render_bwd(d, w, bg, dL_dcolor, dL_dallmap, grad_acc, lists, s)) != cudaSuccess) return (int)e;
+    if ((e = ga_launch_render_bwd(d, w, bg, dL_dcolor, dL_dallmap, grad_acc, s)) != cudaSuccess) return (int)e;
     prof(5, s);
     if ((e = ga_launch_preprocess_bwd(d, w, gauss13, viewmats, projmats, radii, grad_acc, grad_gauss13, s)) != cudaSuccess)
         return (int)e;

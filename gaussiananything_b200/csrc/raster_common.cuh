@@ -57,18 +57,7 @@ struct RasterWs {
     uint4 *lists;
     int32_t *n_list;
     uint32_t *tile_flag;
-    uint32_t *tile_rec_start;  // (list_k > 0) [NV*T + 1] slice layout of the backward's record buffer, computed by the forward
-    uint32_t *inst_off;        // backward (split path): start of every instance's record slice
-    uint32_t *inst_cnt;        // ... and the number of records in it
-};
-
-// global-memory record lists of the split backward (carved from the backward scratch buffer)
-struct BwdLists {
-    uint32_t *tile_rec_start;  // [NV*T + 1] exclusive scan of the per-tile slice totals; [NV*T] = records needed
-                               // (> capacity: the split kernels exit and the fused kernel runs)
-    uint4 *records;
-    uint32_t capacity;         // records the buffer holds
-    uint32_t *inst_off, *inst_cnt;
+    uint32_t *inst_cnt;        // (list_k > 0) contributions of every instance, counted by the forward
 };
 
 // a side stream + fork/join events per device for kernels that are independent of the main stream's next kernel
@@ -95,14 +84,12 @@ cudaError_t ga_launch_binning(const RasterDims &d, const RasterWs &w, cudaStream
                               cudaEvent_t status_event = nullptr);
 cudaError_t ga_launch_render_fwd(const RasterDims &d, const RasterWs &w, const float *bg,
                                  float *out_color, float *out_allmap, cudaStream_t s);
-cudaError_t ga_launch_render_fwd_with_slices(const RasterDims &d, const RasterWs &w, const float *bg, float *out_color,
-                                             float *out_allmap, cudaStream_t s);
 #ifndef GA_LIST_K
 #define GA_LIST_K 32               /* default per-pixel list capacity callers pass as list_k */
 #endif
 cudaError_t ga_launch_render_bwd(const RasterDims &d, const RasterWs &w, const float *bg,
                                  const float *dL_dcolor, const float *dL_dallmap,
-                                 float *grad_acc, const BwdLists &lists, cudaStream_t s);
+                                 float *grad_acc, cudaStream_t s);
 cudaError_t ga_launch_preprocess_bwd(const RasterDims &d, const RasterWs &w, const float *gauss13,
                                      const float *viewmats, const float *projmats,
                                      const int32_t *radii, const float *grad_acc,

@@ -9,11 +9,10 @@
 //    against the warp's block and the warp only evaluates the hits.  The cull
 //    box contains every pixel that can reach alpha >= 1/255, so results are
 //    identical to evaluating every (pixel, surfel) pair.
-//  * the backward recomputes the forward per tile, reduces each surfel's
-//    gradient over the warp with shuffles, over the CTA in shared memory, and
-//    issues one global atomic per (tile, surfel, component).
+//  * the backward walks each tile back to front, keeps the per-(pixel, surfel)
+//    records in shared memory, accumulates each surfel's gradient in registers
+//    and issues one global atomic per (tile, surfel, component).
 #include "raster_common.cuh"
-#include "sm90_ptx.cuh"
 #include "device_once.cuh"
 #include <cstdlib>
 
@@ -96,7 +95,8 @@ __device__ __forceinline__ bool eval_pair(const float4 a, const float4 b, const 
 // LISTS: the kernel also records, per pixel, every surfel that contributed -- {position in the tile list, alpha,
 // depth} -- into a tile-major array (entry k of the tile's 256 pixels is one contiguous 4 KB row, so a warp's store is
 // four full 128-byte lines).  The backward then walks exactly these entries: no cull tests, no pair re-evaluation for
-// pairs that do not contribute, and the contribution decisions are the forward's own bits.
+// pairs that do not contribute, and the contribution decisions are the forward's own bits.  It also counts every
+// instance's contributions (inst_cnt), which sizes that instance's records in the backward exactly.
 template <int GS, bool LISTS>
 __global__ void __launch_bounds__(256, 4)
 render_fwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
@@ -106,13 +106,12 @@ render_fwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
     constexpr int GW = GS == 32 ? 8 : 4;                         // group block width / height in pixels
     constexpr int GH = GS == 8 ? 2 : 4;
     __shared__ float4 s_rec[7][CHUNK];
-    __shared__ uint32_t s_area;                                  // LISTS: sum of the clipped cull-box areas staged so far
+    __shared__ int s_cnt[LISTS ? CHUNK : 1];                     // LISTS: contributions of each staged instance
     if (ws.status[1]) return;
     const int view = blockIdx.z;
     const int tile = blockIdx.y * d.gx + blockIdx.x;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int grp = lane / GS, gl = lane % GS;
-    if (LISTS && threadIdx.x == 0) s_area = 0;
     const int ox = blockIdx.x * GA_BLOCK_X, oy = blockIdx.y * GA_BLOCK_Y;
     const int wx0 = (warp & 1) * 8, wy0 = (warp >> 1) * 4;       // warp's 8x4 block, tile-local
     // group blocks tile the warp block: GS=16 -> 2 side by side (4x4); GS=8 -> 2x2 arrangement of 4x2 blocks
@@ -139,7 +138,7 @@ render_fwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
     for (int c0 = 0; c0 < total; c0 += CHUNK) {
         if (__syncthreads_count(done) == 256) break;
         const int cnt = min(CHUNK, total - c0);
-        uint32_t area = 0;
+        if (LISTS) s_cnt[threadIdx.x] = 0;
         if ((int)threadIdx.x < cnt) {
             const uint32_t id = ws.ids[start + c0 + threadIdx.x];
             const float4 *src = reinterpret_cast<const float4 *>(rec_base + (size_t)id * GA_REC_F);
@@ -158,19 +157,6 @@ render_fwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
             s_rec[4][threadIdx.x] = make_float4(bb.x - oxf, bb.y - oxf, bb.z - oyf, bb.w - oyf);
             s_rec[5][threadIdx.x] = nr;
             s_rec[6][threadIdx.x] = gb;
-            if (LISTS) {
-                // slice length of this instance in the backward's record buffer = pixels of its cull box inside the tile
-                // (same formula as clipped_box_area(): box and tile in absolute coordinates)
-                const float x0 = fmaxf(bb.x, oxf), x1 = fminf(bb.y, oxf + 15.f);
-                const float y0 = fmaxf(bb.z, oyf), y1 = fminf(bb.w, oyf + 15.f);
-                const int wx = max(0, (int)floorf(x1) - (int)ceilf(x0) + 1), wy = max(0, (int)floorf(y1) - (int)ceilf(y0) + 1);
-                area = (uint32_t)(wx * wy);
-            }
-        }
-        if (LISTS) {
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) area += __shfl_xor_sync(0xffffffffu, area, o);
-            if (lane == 0 && area) atomicAdd(&s_area, area);
         }
         __syncthreads();
         for (int g0 = 0; g0 < cnt; g0 += 32) {
@@ -229,6 +215,7 @@ render_fwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
                         T = test_T;
                         last_contributor = contributor;
                         if (LISTS) {
+                            atomicAdd(&s_cnt[jj], 1);
                             if (nl < d.list_k) {
                                 const uint4 ent = make_uint4((uint32_t)(contributor - 1), __float_as_uint(alpha),
                                                              __float_as_uint(depth), 0u);
@@ -245,13 +232,13 @@ render_fwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
             }
         }
         __syncthreads();
+        // every chunk holding a position below the tile's deepest contributor is staged here, so the backward finds
+        // the exact record count of every instance it reads
+        if (LISTS && (int)threadIdx.x < cnt) ws.inst_cnt[start + c0 + threadIdx.x] = (uint32_t)s_cnt[threadIdx.x];
     }
     if (LISTS) {
         if (inside) ws.n_list[(size_t)view * d.H * d.W + (size_t)pyi * d.W + pxi] = nl;
         if (nl > d.list_k) ws.tile_flag[(size_t)view * d.T + tile] = 1u;      // this tile's backward recomputes
-        // every chunk the backward can reach (positions below the last contributor) has been staged here, so the sum
-        // covers its slices; bwd_scan_area_kernel turns the per-tile sums into offsets
-        if (threadIdx.x == 0) ws.tile_rec_start[(size_t)view * d.T + tile] = s_area;
     }
     if (inside) {
         const size_t HW = (size_t)d.H * d.W;
@@ -302,51 +289,44 @@ cudaError_t ga_launch_render_fwd(const RasterDims &d, const RasterWs &w, const f
 }
 
 // ---------------------------------------------------------------------------
-// K4 backward
+// K4 backward: one CTA of 256 threads per tile; each thread owns one pixel of the tile (a warp an 8x4 block).
 //
-// Two phases per group of G staged surfels (G = 128, 64, 32 or 16, picked per chunk so that a surfel's cull box
-// clipped to the tile never holds more pixels than its list capacity BWD_LIST_RECORDS/G):
-//   phase A (pixel-parallel, back to front): every lane walks its own stream of surfels whose cull box
-//     contains its pixel, recomputes alpha, runs the compositing recurrences and appends a 16-byte record
-//     (pixel, dL/dalpha, dL/dz, w) to the surfel's list in shared memory;
-//   phase B (surfel-parallel): 256/G threads share a surfel, re-derive the ray-splat geometry of each
-//     recorded pixel, accumulate the 18 gradient components in registers and reduce-scatter them over the
-//     256/G lanes; one global atomic per (tile, surfel, component).
-// This replaces a 32-lane reduction per (warp, surfel) hit -- where typically 8 of 32 lanes carried data --
-// by register accumulation over the pixels a surfel actually touches.
+// The tile's instances are staged back to front in chunks of 256 list positions (slot t = position hi-1-t) and each
+// chunk is cut into WINDOWS of consecutive slots whose records fit BWD_RECORDS 16-byte records in shared memory.  An
+// instance's record bound is its exact contribution count from the forward (LISTS) or the pixels of its cull box
+// inside the tile (recompute); both are <= 256 <= BWD_RECORDS, so every window holds at least one instance.  Per
+// window:
+//   phase A (pixel-parallel, back to front): every thread runs its pixel's compositing recurrences over the window's
+//     contributions -- from the per-pixel lists the forward recorded (LISTS), or by culling and re-evaluating the
+//     staged surfels -- and appends the record (pixel, dL/dalpha, dL/dz, w) to the instance's slice of the window's
+//     record buffer.  The recurrence state stays in registers from one window to the next.
+//   phase B (instance-parallel): the window's non-empty instances, sorted by record count so that the lane pairs of a
+//     warp get instances of similar length, are walked by BWD_TPI lanes each; they re-derive the ray-splat geometry
+//     of every record with the same eval_pair() as the forward (same bits), accumulate the 18 gradient components in
+//     registers, reduce-scatter them over the lanes and add them to grad_acc: one global atomic per (tile, instance,
+//     non-zero component).
+// The records never leave the SM.  Tiles whose lists overflowed (and callers with list_k == 0) take the recompute
+// path of the same launch.
 // ---------------------------------------------------------------------------
-#ifndef BWD_CTAS
-#define BWD_CTAS 2                  /* CTAs per SM the backward is sized for (registers and shared memory) */
-#endif
-#if BWD_CTAS >= 3
-#define BWD_LIST_RECORDS 2560
-#else
-#define BWD_LIST_RECORDS 4096
-#endif
-#define BWD_MAXG 128
-#ifndef BWD_A_CTAS
-#define BWD_A_CTAS 4                /* resident CTAs per SM kernel A is compiled for (64 registers, no spills) */
-#endif
-#ifndef BWD_B_UNROLL
-#define BWD_B_UNROLL 2              /* records per loop iteration and lane in kernel B */
-#endif
-#ifndef BWD_B_THREADS
-#define BWD_B_THREADS 128           /* threads per CTA (= per tile) in kernel B: 128 -> 6 CTAs per SM; 256: +22 us, 64: +56 us on C2 */
-#endif
-#ifndef BWD_B_CTAS
-#define BWD_B_CTAS (768 / BWD_B_THREADS)
-#endif
-#ifndef BWD_B_TPI
-#define BWD_B_TPI 2                 /* lanes per instance in kernel B (2: 364 us, 4: 375 us, 8: 400+ us on C2) */
-#endif
+// Two CTAs per SM: ~104 KB of shared memory and up to 128 registers each.  Three (2048 records, 80 registers) were
+// measured slower on C2, 0.465 against 0.407 ms: the recurrence state that phase A carries across phase B does not
+// fit next to phase B's accumulators in 80 registers (176 B of spills).
+#define BWD_RECORDS 4096            /* window record buffer, 64 KB */
+#define BWD_TPI 2                   /* lanes per instance in phase B */
 
 struct BwdSmem {
-    float4 rec[6][CHUNK];
-    uint4 list[BWD_LIST_RECORDS];
-    float4 up[2][256];              // per pixel: {dL/dcolor (3), dL/dnormal.x}, {dL/dnormal.yz, -, -}: two conflict-light LDS.128
-    uint32_t id[CHUNK];
-    int cnt[2][BWD_MAXG];
-    int maxc;
+    float4 rec[6][CHUNK];           // the chunk's staged surfel records, slot t = list position hi-1-t
+    uint4 recs[BWD_RECORDS];        // the window's records, instance by instance
+    // per pixel: {dL/dcolor (3), dL/dnormal.x}, {dL/dnormal.yz, dL/ddepth, dL/dalpha_acc}, {dL/ddist, dL/dmedian, M1, M2};
+    // phase A reads its pixel's constants from here, which keeps them out of the registers phase B needs
+    float4 up[3][256];
+    uint32_t id[CHUNK];             // surfel of every slot
+    int off[CHUNK];                 // start of every slot's record slice, relative to the chunk
+    int cnt[CHUNK];                 // records appended to it so far
+    int bin[64];                    // phase-B counting sort by record count
+    uint16_t perm[CHUNK];
+    int wsum[8];
+    int maxc, m;
 };
 
 // reduce-scatter of 18 components over TPI (2/4/8/16) consecutive lanes by recursive halving: after level l a lane
@@ -422,74 +402,22 @@ __device__ __forceinline__ void reduce_scatter18(const float (&g)[GA_GRAD_F], in
     }
 }
 
-template <int TPI>
-__device__ __forceinline__ void bwd_phase_b(BwdSmem &sm, const int *cnt, int g0, int gcnt, int cap, int ox, int oy,
-                                            float *__restrict__ acc_base)
+__device__ __forceinline__ int clipped_box_area(const float4 bb, int ox, int oy)
 {
-    const int tid = threadIdx.x, lane = tid & 31;
-    const int inst = tid / TPI, sub = tid % TPI;
-    const bool valid = inst < gcnt;
-    const int n = valid ? min(cnt[inst], cap) : 0;
-    float g[GA_GRAD_F];
-#pragma unroll
-    for (int f = 0; f < GA_GRAD_F; f++) g[f] = 0.f;
-    if (n > 0) {
-        const int jj = g0 + inst;
-        const float4 a = sm.rec[0][jj], b = sm.rec[1][jj], c = sm.rec[2][jj];
-        const float opa = c.w;
-        for (int r = sub; r < n; r += TPI) {
-            const uint4 rc = sm.list[inst * cap + r];
-            const int pix = (int)rc.x;
-            const float dL_dalpha = __uint_as_float(rc.y), dL_dz = __uint_as_float(rc.z), w = __uint_as_float(rc.w);
-            const float pfx = (float)(ox + (pix & 15)), pfy = (float)(oy + (pix >> 4));
-            PixelGeom pg;
-            float k0, k1, k2, l0, l1, l2;
-            eval_pair(a, b, c, pfx, pfy, pg, k0, k1, k2, l0, l1, l2);      // same code path as phase A: same bits
-            const float G = pg.G;
-            const float dL_dG = opa * dL_dalpha;                           // 0.99 clamp passed through (upstream)
-            if (pg.use3d) {
-                const float dL_ds0 = dL_dG * -G * pg.s0 + dL_dz * b.z;
-                const float dL_ds1 = dL_dG * -G * pg.s1 + dL_dz * b.w;
-                const float ip = fast_rcp(pg.p2);
-                const float q0 = dL_ds0 * ip, q1 = dL_ds1 * ip;
-                const float q2 = -(q0 * pg.s0 + q1 * pg.s1);
-                const float dk0 = l1 * q2 - l2 * q1, dk1 = l2 * q0 - l0 * q2, dk2 = l0 * q1 - l1 * q0;
-                const float dl0 = q1 * k2 - q2 * k1, dl1 = q2 * k0 - q0 * k2, dl2 = q0 * k1 - q1 * k0;
-                g[0] -= dk0; g[1] -= dk1; g[2] -= dk2;
-                g[3] -= dl0; g[4] -= dl1; g[5] -= dl2;
-                g[6] += pfx * dk0 + pfy * dl0 + dL_dz * pg.s0;
-                g[7] += pfx * dk1 + pfy * dl1 + dL_dz * pg.s1;
-                g[8] += pfx * dk2 + pfy * dl2 + dL_dz;
-            } else {
-                g[9] += dL_dG * (-G * GA_FILTER_INV_SQUARE * pg.dx);
-                g[10] += dL_dG * (-G * GA_FILTER_INV_SQUARE * pg.dy);
-                g[8] += dL_dz;
-            }
-            g[14] += G * dL_dalpha;
-            const float4 ua = sm.up[0][pix], ub = sm.up[1][pix];
-            g[15] += w * ua.x; g[16] += w * ua.y; g[17] += w * ua.z;
-            g[11] += w * ua.w; g[12] += w * ub.x; g[13] += w * ub.y;
-        }
-    }
-    // all lanes of the warp take part in the shuffles; groups whose surfel recorded nothing carry zeros
-    const int any = __any_sync(0xffffffffu, n > 0);
-    if (any) {
-        float *dst = acc_base + (size_t)(valid ? sm.id[g0 + inst] : 0) * GA_GRAD_F;
-        reduce_scatter18<TPI>(g, lane, dst);
-    }
+    const float x0 = fmaxf(bb.x, (float)ox), x1 = fminf(bb.y, (float)(ox + 15));
+    const float y0 = fmaxf(bb.z, (float)oy), y1 = fminf(bb.w, (float)(oy + 15));
+    const int wx = max(0, (int)floorf(x1) - (int)ceilf(x0) + 1), wy = max(0, (int)floorf(y1) - (int)ceilf(y0) + 1);
+    return wx * wy;
 }
 
-// Two CTAs per SM (96 KB of shared memory, 128 registers).  Three per SM (2560-record lists, 80 registers) were
-// measured at 0.85 ms against 0.55 ms: the phase-A recurrences do not fit 80 registers (192 B of spills).
-__global__ void __launch_bounds__(256, BWD_CTAS)
-render_bwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
-                  const float *__restrict__ dL_dcolor, const float *__restrict__ dL_dallmap,
-                  float *__restrict__ grad_acc, const uint32_t *__restrict__ split_total, uint32_t split_capacity)
+// LISTS = true: every thread walks ITS pixel's list entries -- {list position, alpha, depth}, the forward's own bits --
+// back to front with three entries in flight in registers, so there is no cull test and no pair evaluation for
+// surfels that do not reach alpha >= 1/255 at the pixel.  LISTS = false culls and re-evaluates every staged surfel.
+template <bool LISTS>
+__device__ __forceinline__ void bwd_tile(const RasterDims &d, const RasterWs &ws, BwdSmem &sm, const float *__restrict__ bg,
+                                         const float *__restrict__ dL_dcolor, const float *__restrict__ dL_dallmap,
+                                         float *__restrict__ grad_acc)
 {
-    extern __shared__ __align__(16) uint8_t bwd_smem_raw[];
-    BwdSmem &sm = *reinterpret_cast<BwdSmem *>(bwd_smem_raw);
-    if (ws.status[1]) return;
-    if (split_total && split_total[0] <= split_capacity) return;      // the split kernels (below) did the work
     const int view = blockIdx.z;
     const int tile = blockIdx.y * d.gx + blockIdx.x;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -500,8 +428,6 @@ render_bwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
     const int pix_local = lyi * 16 + lxi;
     const bool inside = pxi < d.W && pyi < d.H;
     const float pfx = (float)pxi, pfy = (float)pyi;
-    const float bx_lo = (float)(ox + lx0), bx_hi = (float)(ox + lx0 + 7);
-    const float by_lo = (float)(oy + ly0), by_hi = (float)(oy + ly0 + 3);
 
     const uint32_t start = ws.tile_start[(size_t)view * d.T + tile];
     const size_t HW = (size_t)d.H * d.W;
@@ -515,709 +441,262 @@ render_bwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
     float T = T_final;
     const int last_contributor = inside ? nc[pix] : 0;
     const int median_contributor = inside ? nc[pix + HW] : 0;
-    float dpx0 = 0, dpx1 = 0, dpx2 = 0, dL_ddepth = 0, dL_daccum = 0, dL_dreg = 0;
-    float dn0 = 0, dn1 = 0, dn2 = 0, dL_dmedian = 0;
-    if (inside) {
-        const float *gc = dL_dcolor + (size_t)view * 3 * HW;
-        const float *ga = dL_dallmap + (size_t)view * 7 * HW;
-        dpx0 = gc[pix]; dpx1 = gc[pix + HW]; dpx2 = gc[pix + 2 * HW];
-        dL_ddepth = ga[pix]; dL_daccum = ga[pix + HW];
-        dn0 = ga[pix + 2 * HW]; dn1 = ga[pix + 3 * HW]; dn2 = ga[pix + 4 * HW];
-        dL_dmedian = ga[pix + 5 * HW]; dL_dreg = ga[pix + 6 * HW];
+    float bg_dot_dpixel = 0.f;
+    {
+        float4 u0 = make_float4(0.f, 0.f, 0.f, 0.f), u1 = u0, u2 = u0;
+        if (inside) {
+            const float *gc = dL_dcolor + (size_t)view * 3 * HW;
+            const float *ga = dL_dallmap + (size_t)view * 7 * HW;
+            u0 = make_float4(gc[pix], gc[pix + HW], gc[pix + 2 * HW], ga[pix + 2 * HW]);
+            u1 = make_float4(ga[pix + 3 * HW], ga[pix + 4 * HW], ga[pix], ga[pix + HW]);
+            u2 = make_float4(ga[pix + 6 * HW], ga[pix + 5 * HW], fT[pix + HW], fT[pix + 2 * HW]);
+        }
+        sm.up[0][pix_local] = u0;
+        sm.up[1][pix_local] = u1;
+        sm.up[2][pix_local] = u2;
+        bg_dot_dpixel = bg[0] * u0.x + bg[1] * u0.y + bg[2] * u0.z;
     }
-    sm.up[0][pix_local] = make_float4(dpx0, dpx1, dpx2, dn0);
-    sm.up[1][pix_local] = make_float4(dn1, dn2, 0.f, 0.f);
-    const float final_D = inside ? fT[pix + HW] : 0.f, final_D2 = inside ? fT[pix + 2 * HW] : 0.f;
     const float final_A = 1 - T_final;
-    const float bg_dot_dpixel = bg[0] * dpx0 + bg[1] * dpx1 + bg[2] * dpx2;
     // Upstream keeps one suffix accumulator per output channel (colour 3, depth, alpha, normal 3), all with the same
     // recurrence acc = last_alpha * last_value + (1 - last_alpha) * acc, and adds (value - acc) * dL/dchannel to
     // dL/dalpha.  The sum over channels is linear, so ONE scalar recurrence on v = sum_ch value_ch * dL/dchannel does
     // the same work (8 recurrences and ~20 registers less per pair).
     float last_alpha = 0, v_last = 0, v_acc = 0, last_dL_dT = 0;
 
+    const uint4 *my_list = nullptr;
+    int kk = -1;                        // LISTS: this pixel's next entry, counting down
+    if (LISTS) {
+        my_list = ws.lists + ((size_t)view * d.T + tile) * (size_t)d.list_k * 256 + pix_local;
+        kk = (inside ? ws.n_list[(size_t)view * HW + pix] : 0) - 1;
+#pragma unroll
+        for (int q = 0; q < 8; q++)
+            if (kk >= q) asm volatile("prefetch.global.L2 [%0];" ::"l"(my_list + (size_t)(kk - q) * 256));
+    }
+
     // nothing behind the deepest contributor of the tile can receive gradient
     if (threadIdx.x == 0) sm.maxc = 0;
-    sm.cnt[threadIdx.x >> 7][threadIdx.x & 127] = 0;
     __syncthreads();
     {
-        int m = last_contributor;
+        int mc = last_contributor;
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
-        if (lane == 0) atomicMax(&sm.maxc, m);
+        for (int o = 16; o > 0; o >>= 1) mc = max(mc, __shfl_xor_sync(0xffffffffu, mc, o));
+        if (lane == 0) atomicMax(&sm.maxc, mc);
     }
     __syncthreads();
     const int total = sm.maxc;          // list positions [0,total) matter
-    int parity = 0;
 
     for (int hi = total; hi > 0; hi -= CHUNK) {
-        const int lo = max(0, hi - CHUNK);
-        const int cnt = hi - lo;
-        // stage positions lo..hi-1; slot t holds position hi-1-t (back to front)
-        int big0 = 0, big1 = 0, big2 = 0, big3 = 0;
+        const int cnt = min(CHUNK, hi);
+        // stage positions hi-cnt..hi-1, slot t = position hi-1-t, with the record bound of every slot
+        int bound = 0;
         if ((int)threadIdx.x < cnt) {
-            const uint32_t id = ws.ids[start + (hi - 1 - threadIdx.x)];
+            const int pos = hi - 1 - (int)threadIdx.x;
+            const uint32_t id = ws.ids[start + pos];
             sm.id[threadIdx.x] = id;
             const float4 *src = reinterpret_cast<const float4 *>(rec_base + (size_t)id * GA_REC_F);
             float4 q[6];
 #pragma unroll
             for (int k = 0; k < 6; k++) { q[k] = __ldg(src + k); sm.rec[k][threadIdx.x] = q[k]; }
-            // pixels of this tile inside the cull box (upper bound of the surfel's list length)
-            const float x0 = fmaxf(q[4].x, (float)ox), x1 = fminf(q[4].y, (float)(ox + 15));
-            const float y0 = fmaxf(q[4].z, (float)oy), y1 = fminf(q[4].w, (float)(oy + 15));
-            const int wx = max(0, (int)floorf(x1) - (int)ceilf(x0) + 1), wy = max(0, (int)floorf(y1) - (int)ceilf(y0) + 1);
-            const int area = wx * wy;
-            big0 = area > BWD_LIST_RECORDS / 128; big1 = area > BWD_LIST_RECORDS / 64;
-            big2 = area > BWD_LIST_RECORDS / 32; big3 = area > BWD_LIST_RECORDS / 16;
+            bound = LISTS ? (int)ws.inst_cnt[start + pos] : clipped_box_area(q[4], ox, oy);
         }
-        const int any0 = __syncthreads_or(big0);
-        const int any1 = __syncthreads_or(big1);
-        const int any2 = __syncthreads_or(big2);
-        const int any3 = __syncthreads_or(big3);
-        // list capacity per surfel = BWD_LIST_RECORDS / G must cover the pixels of its cull box inside the tile
-        // (G = 8: capacity >= 256 = the whole tile)
-        const int G = any3 ? 8 : (any2 ? 16 : (any1 ? 32 : (any0 ? 64 : 128)));
-        const int cap = BWD_LIST_RECORDS / G;
+        int incl = bound;               // inclusive scan of the bounds over the slots
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += y;
+        }
+        if (lane == 31) sm.wsum[warp] = incl;
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < 8; k++) incl += k < warp ? sm.wsum[k] : 0;
+        sm.off[threadIdx.x] = incl - bound;
+        sm.cnt[threadIdx.x] = 0;
 
-        for (int g0 = 0; g0 < cnt; g0 += G, parity ^= 1) {
-            const int gcnt = min(G, cnt - g0);
-            int *cntp = sm.cnt[parity];
-            // ---------------- phase A: sub-blocks of 32 surfels, no block barrier in between.  (Walking one per-lane
-            // list over the whole group of 128 instead needs 22 % fewer rounds, tools/raster_rounds.py, but was measured
-            // slower: 573 vs 537 us -- the list bookkeeping costs more than the rounds it saves.)
-            for (int sb = 0; sb < gcnt; sb += 32) {
-                const int base = g0 + sb;
-                bool hit = false;
-                if (sb + lane < gcnt) {
-                    const float4 bb = sm.rec[4][base + lane];
-                    hit = !(bb.y < bx_lo || bb.x > bx_hi || bb.w < by_lo || bb.z > by_hi);
+        int t0 = 0, base = 0;           // window = slots [t0, t1); base = offset of slot t0's slice
+        while (t0 < cnt) {
+            if (threadIdx.x < 64) sm.bin[threadIdx.x] = 0;
+            const int t1 = t0 + __syncthreads_count((int)threadIdx.x >= t0 && (int)threadIdx.x < cnt &&
+                                                    incl - base <= BWD_RECORDS);
+
+            // ---------------- phase A: one (pixel, surfel) contribution = the recurrences backwards + one record
+            auto contribute = [&](const int jj, const int contributor, const float alpha, const float c_d) {
+                const float4 nr = sm.rec[3][jj], gb = sm.rec[5][jj];
+                const float4 u0 = sm.up[0][pix_local], u1 = sm.up[1][pix_local], u2 = sm.up[2][pix_local];
+                const float dL_ddepth = u1.z, dL_dreg = u2.x, final_D = u2.z, final_D2 = u2.w;
+                const float inv1ma = fast_rcp(1.f - alpha);
+                T = T * inv1ma;
+                const float w = alpha * T;
+                float dL_dz = 0.0f;
+                const float inv_cd = fast_rcp(c_d);
+                const float m_d = GA_M_C0 - GA_M_C1 * inv_cd;
+                const float dmd_dd = GA_M_C1 * inv_cd * inv_cd;
+                if (contributor == median_contributor - 1) dL_dz += u2.y;
+                const float dL_dweight = (final_D2 + m_d * m_d * final_A - 2 * m_d * final_D) * dL_dreg;
+                const float dL_dmd = 2.0f * (T * alpha) * (m_d * final_A - final_D) * dL_dreg;
+                dL_dz += dL_dmd * dmd_dd;
+                // v = (colour . dL/dcolour) + depth dL/ddepth + 1 dL/dalpha_acc + (normal . dL/dnormal)
+                const float v = ((nr.w * u0.x + gb.x * u0.y) + (gb.y * u0.z + c_d * dL_ddepth)) +
+                                ((nr.x * u0.w + nr.y * u1.x) + (nr.z * u1.y + u1.w));
+                v_acc = last_alpha * v_last + (1.f - last_alpha) * v_acc;
+                v_last = v;
+                float dL_dalpha = (v - v_acc) + (dL_dweight - last_dL_dT);
+                last_dL_dT = dL_dweight * alpha + (1 - alpha) * last_dL_dT;
+                dL_dalpha *= T;
+                last_alpha = alpha;
+                dL_dalpha += (-T_final * inv1ma) * bg_dot_dpixel;
+                dL_dz += w * dL_ddepth;
+                const int slot = atomicAdd(&sm.cnt[jj], 1);          // < the slot's record bound
+                sm.recs[sm.off[jj] - base + slot] =
+                    make_uint4((uint32_t)pix_local, __float_as_uint(dL_dalpha), __float_as_uint(dL_dz), __float_as_uint(w));
+            };
+            if constexpr (LISTS) {
+                const int pos_lo = hi - t1;     // the window holds positions [hi - t1, hi - t0)
+                // three entries in flight; they are reloaded (from L1 / L2) per window rather than held through phase B
+                uint4 e = make_uint4(0u, 0u, 0u, 0u), e1 = e, e2 = e;
+                if (kk >= 0) e = __ldg(my_list + (size_t)kk * 256);
+                if (kk >= 1) e1 = __ldg(my_list + (size_t)(kk - 1) * 256);
+                if (kk >= 2) e2 = __ldg(my_list + (size_t)(kk - 2) * 256);
+                while (true) {
+                    const bool active = kk >= 0 && (int)e.x >= pos_lo;      // entries are in descending list position
+                    if (!__any_sync(0xffffffffu, active)) break;
+                    if (active) {
+                        const uint4 cur = e;
+                        e = e1; e1 = e2;
+                        if (kk >= 3) e2 = __ldg(my_list + (size_t)(kk - 3) * 256);   // entries kk-1, kk-2, kk-3 are in flight
+                        // ... and the row 8 below is asked into L2 (the list rows stream from HBM exactly once)
+                        if (kk >= 8) asm volatile("prefetch.global.L2 [%0];" ::"l"(my_list + (size_t)(kk - 8) * 256));
+                        kk--;
+                        contribute(hi - 1 - (int)cur.x, (int)cur.x, __uint_as_float(cur.y), __uint_as_float(cur.z));
+                    }
                 }
-                unsigned mask = __ballot_sync(0xffffffffu, hit);
-                unsigned mine = 0;
-                while (mask) {
-                    const int b = __ffs(mask) - 1;
-                    mask &= mask - 1;
-                    const float4 bb = sm.rec[4][base + b];
-                    if (pfx >= bb.x && pfx <= bb.y && pfy >= bb.z && pfy <= bb.w && (hi - 1 - (base + b)) < last_contributor)
-                        mine |= 1u << b;
-                }
-                if (!inside) mine = 0;
-                while (__any_sync(0xffffffffu, mine != 0)) {
-                    const bool active = mine != 0;
-                    const int bsel = active ? __ffs(mine) - 1 : 0;
-                    mine &= mine - 1;
-                    const int jj = base + bsel;
-                    const int contributor = hi - 1 - jj;       // 0-based list position
-                    const float4 a = sm.rec[0][jj], b = sm.rec[1][jj], c = sm.rec[2][jj];
-                    PixelGeom pg;
-                    float k0, k1, k2, l0, l1, l2;
-                    const bool ok = active && eval_pair(a, b, c, pfx, pfy, pg, k0, k1, k2, l0, l1, l2);
-                    if (ok) {
-                        const float4 nr = sm.rec[3][jj], gb = sm.rec[5][jj];
-                        const float alpha = pg.alpha, c_d = pg.depth;
-                        const float inv1ma = fast_rcp(1.f - alpha);
-                        T = T * inv1ma;
-                        const float w = alpha * T;
-                        float dL_dz = 0.0f;
-                        const float inv_cd = fast_rcp(c_d);
-                        const float m_d = GA_M_C0 - GA_M_C1 * inv_cd;
-                        const float dmd_dd = GA_M_C1 * inv_cd * inv_cd;
-                        if (contributor == median_contributor - 1) dL_dz += dL_dmedian;
-                        const float dL_dweight = (final_D2 + m_d * m_d * final_A - 2 * m_d * final_D) * dL_dreg;
-                        const float dL_dmd = 2.0f * (T * alpha) * (m_d * final_A - final_D) * dL_dreg;
-                        dL_dz += dL_dmd * dmd_dd;
-                        // v = (colour . dL/dcolour) + depth dL/ddepth + 1 dL/dalpha_acc + (normal . dL/dnormal)
-                        const float v = ((nr.w * dpx0 + gb.x * dpx1) + (gb.y * dpx2 + c_d * dL_ddepth)) +
-                                        ((nr.x * dn0 + nr.y * dn1) + (nr.z * dn2 + dL_daccum));
-                        v_acc = last_alpha * v_last + (1.f - last_alpha) * v_acc;
-                        v_last = v;
-                        float dL_dalpha = (v - v_acc) + (dL_dweight - last_dL_dT);
-                        last_dL_dT = dL_dweight * alpha + (1 - alpha) * last_dL_dT;
-                        dL_dalpha *= T;
-                        last_alpha = alpha;
-                        dL_dalpha += (-T_final * inv1ma) * bg_dot_dpixel;
-                        dL_dz += w * dL_ddepth;
-                        const int li = sb + bsel;                      // surfel index inside the group
-                        const int slot = atomicAdd(&cntp[li], 1);
-                        if (slot < cap)
-                            sm.list[li * cap + slot] = make_uint4((uint32_t)pix_local, __float_as_uint(dL_dalpha),
-                                                                  __float_as_uint(dL_dz), __float_as_uint(w));
+            } else {
+                const float bx_lo = (float)(ox + lx0), bx_hi = (float)(ox + lx0 + 7);
+                const float by_lo = (float)(oy + ly0), by_hi = (float)(oy + ly0 + 3);
+                for (int sb = t0; sb < t1; sb += 32) {
+                    bool hit = false;
+                    if (sb + lane < t1) {
+                        const float4 bb = sm.rec[4][sb + lane];
+                        hit = !(bb.y < bx_lo || bb.x > bx_hi || bb.w < by_lo || bb.z > by_hi);
+                    }
+                    unsigned mask = __ballot_sync(0xffffffffu, hit);
+                    unsigned mine = 0;
+                    while (mask) {
+                        const int b = __ffs(mask) - 1;
+                        mask &= mask - 1;
+                        const float4 bb = sm.rec[4][sb + b];
+                        if (pfx >= bb.x && pfx <= bb.y && pfy >= bb.z && pfy <= bb.w && (hi - 1 - (sb + b)) < last_contributor)
+                            mine |= 1u << b;
+                    }
+                    if (!inside) mine = 0;
+                    while (__any_sync(0xffffffffu, mine != 0)) {
+                        const bool active = mine != 0;
+                        const int bsel = active ? __ffs(mine) - 1 : 0;
+                        mine &= mine - 1;
+                        const int jj = sb + bsel;
+                        const float4 a = sm.rec[0][jj], b = sm.rec[1][jj], c = sm.rec[2][jj];
+                        PixelGeom pg;
+                        float k0, k1, k2, l0, l1, l2;
+                        const bool ok = active && eval_pair(a, b, c, pfx, pfy, pg, k0, k1, k2, l0, l1, l2);
+                        if (ok) contribute(jj, hi - 1 - jj, pg.alpha, pg.depth);
                     }
                 }
             }
             __syncthreads();
-            // ---------------- phase B
-            if (threadIdx.x < BWD_MAXG) sm.cnt[parity ^ 1][threadIdx.x] = 0;      // counters of the next group
-            if (G == 128) bwd_phase_b<2>(sm, cntp, g0, gcnt, cap, ox, oy, acc_base);
-            else if (G == 64) bwd_phase_b<4>(sm, cntp, g0, gcnt, cap, ox, oy, acc_base);
-            else if (G == 32) bwd_phase_b<8>(sm, cntp, g0, gcnt, cap, ox, oy, acc_base);
-            else bwd_phase_b<16>(sm, cntp, g0, gcnt, cap, ox, oy, acc_base);     // G = 16, and G = 8 with half the threads idle
+
+            // ---------------- phase B: counting sort of the window's non-empty slots by record count, descending
+            const int myc = ((int)threadIdx.x >= t0 && (int)threadIdx.x < t1) ? sm.cnt[threadIdx.x] : 0;
+            if (myc > 0) atomicAdd(&sm.bin[min(myc, 63)], 1);
             __syncthreads();
+            if (threadIdx.x < 32) {
+                // exclusive prefix over the bins in descending count order (bin 63 first); bin 0 is unused
+                const int hi_bin = 63 - 2 * (int)threadIdx.x, lo_bin = hi_bin - 1;
+                const int vh = sm.bin[hi_bin], vl = lo_bin >= 1 ? sm.bin[lo_bin] : 0;
+                int x = vh + vl;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    const int y = __shfl_up_sync(0xffffffffu, x, o);
+                    if ((int)threadIdx.x >= o) x += y;
+                }
+                const int excl = x - (vh + vl);
+                sm.bin[hi_bin] = excl;
+                if (lo_bin >= 1) sm.bin[lo_bin] = excl + vh;
+                if (threadIdx.x == 31) sm.m = x;
+            }
+            __syncthreads();
+            if (myc > 0) sm.perm[atomicAdd(&sm.bin[min(myc, 63)], 1)] = (uint16_t)threadIdx.x;
+            __syncthreads();
+            const int m = sm.m, sub = threadIdx.x % BWD_TPI;
+            for (int b0 = 0; b0 < m; b0 += 256 / BWD_TPI) {
+                const int slot = b0 + (int)threadIdx.x / BWD_TPI;
+                const int jj = slot < m ? (int)sm.perm[slot] : 0;
+                const int n = slot < m ? sm.cnt[jj] : 0;
+                float g[GA_GRAD_F];
+#pragma unroll
+                for (int f = 0; f < GA_GRAD_F; f++) g[f] = 0.f;
+                if (n > 0) {
+                    const float4 a = sm.rec[0][jj], b = sm.rec[1][jj], c = sm.rec[2][jj];
+                    const float opa = c.w;
+                    const uint4 *lst = sm.recs + (sm.off[jj] - base);
+                    for (int r = sub; r < n; r += BWD_TPI) {
+                        const uint4 rc = lst[r];
+                        const int p = (int)rc.x;
+                        const float dL_dalpha = __uint_as_float(rc.y), dL_dz = __uint_as_float(rc.z), w = __uint_as_float(rc.w);
+                        const float qx = (float)(ox + (p & 15)), qy = (float)(oy + (p >> 4));
+                        PixelGeom pg;
+                        float k0, k1, k2, l0, l1, l2;
+                        eval_pair(a, b, c, qx, qy, pg, k0, k1, k2, l0, l1, l2);      // same code path as phase A: same bits
+                        const float G = pg.G;
+                        const float dL_dG = opa * dL_dalpha;                         // 0.99 clamp passed through (upstream)
+                        if (pg.use3d) {
+                            const float dL_ds0 = dL_dG * -G * pg.s0 + dL_dz * b.z;
+                            const float dL_ds1 = dL_dG * -G * pg.s1 + dL_dz * b.w;
+                            const float ip = fast_rcp(pg.p2);
+                            const float q0 = dL_ds0 * ip, q1 = dL_ds1 * ip;
+                            const float q2 = -(q0 * pg.s0 + q1 * pg.s1);
+                            const float dk0 = l1 * q2 - l2 * q1, dk1 = l2 * q0 - l0 * q2, dk2 = l0 * q1 - l1 * q0;
+                            const float dl0 = q1 * k2 - q2 * k1, dl1 = q2 * k0 - q0 * k2, dl2 = q0 * k1 - q1 * k0;
+                            g[0] -= dk0; g[1] -= dk1; g[2] -= dk2;
+                            g[3] -= dl0; g[4] -= dl1; g[5] -= dl2;
+                            g[6] += qx * dk0 + qy * dl0 + dL_dz * pg.s0;
+                            g[7] += qx * dk1 + qy * dl1 + dL_dz * pg.s1;
+                            g[8] += qx * dk2 + qy * dl2 + dL_dz;
+                        } else {
+                            g[9] += dL_dG * (-G * GA_FILTER_INV_SQUARE * pg.dx);
+                            g[10] += dL_dG * (-G * GA_FILTER_INV_SQUARE * pg.dy);
+                            g[8] += dL_dz;
+                        }
+                        g[14] += G * dL_dalpha;
+                        const float4 ua = sm.up[0][p], ub = sm.up[1][p];
+                        g[15] += w * ua.x; g[16] += w * ua.y; g[17] += w * ua.z;
+                        g[11] += w * ua.w; g[12] += w * ub.x; g[13] += w * ub.y;
+                    }
+                }
+                // all lanes of the warp take part in the shuffles; lanes without records carry zeros (adds skipped)
+                if (__any_sync(0xffffffffu, n > 0))
+                    reduce_scatter18<BWD_TPI>(g, lane, acc_base + (size_t)(n > 0 ? sm.id[jj] : 0) * GA_GRAD_F);
+            }
+            t0 = t1;
+            if (t0 < cnt) base = sm.off[t0];
+            __syncthreads();            // the next window's phase A rewrites recs and bin; the next chunk rewrites the rest
         }
     }
 }
 
-// ---------------------------------------------------------------------------
-// K4 split variant (default): the two phases as two kernels, with the per-(tile, surfel) record lists in GLOBAL
-// memory (the fused kernel above remains the fallback when the list budget does not cover the scene).
-//
-// Why: in the fused kernel the lists live in 64 KB of shared memory and both phases share one register budget
-// (125 registers, 2 CTAs = 16 warps per SM); its top stall reason is the block barrier between the phases
-// (profiles/r02_raster.md: barrier 2.1, wait 1.7 warps per issue at 47 % issue utilisation).  HBM, on the other
-// hand, is idle (5 % DRAM utilisation).  So:
-//   kernel A (pixel-parallel, back to front)  = phase A; records go to the instance's slice of a global buffer.
-//     The slice length is the instance's cull-box area inside the tile -- exact, so there is no capacity rule, no
-//     group size G, no phase-B barrier: three block barriers per chunk of 256 surfels instead of seven.
-//   kernel B (instance-parallel)              = phase B; TPI lanes walk an instance's records (contiguous 16-byte
-//     entries), re-derive the geometry with the same eval_pair() (same bits), reduce-scatter, global atomics.
-// Slices are laid out tile by tile: a warp-per-tile pre-pass sums the clipped cull-box areas, one block scans the
-// tile totals.  If the total exceeds the buffer, a device flag routes the launch to the fused kernel instead (no
-// host synchronisation either way).  Extra traffic: 16 B written + read per record, ~2 x 26 M records on C2.
-// ---------------------------------------------------------------------------
-__device__ __forceinline__ int clipped_box_area(const float4 bb, int ox, int oy)
+__global__ void __launch_bounds__(256, 2)
+render_bwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg, const float *__restrict__ dL_dcolor,
+                  const float *__restrict__ dL_dallmap, float *__restrict__ grad_acc)
 {
-    const float x0 = fmaxf(bb.x, (float)ox), x1 = fminf(bb.y, (float)(ox + 15));
-    const float y0 = fmaxf(bb.z, (float)oy), y1 = fminf(bb.w, (float)(oy + 15));
-    const int wx = max(0, (int)floorf(x1) - (int)ceilf(x0) + 1), wy = max(0, (int)floorf(y1) - (int)ceilf(y0) + 1);
-    return wx * wy;
-}
-
-// one warp per tile: sum of the clipped cull-box areas of the tile's instances
-__global__ void __launch_bounds__(256)
-bwd_tile_area_kernel(RasterDims d, RasterWs ws, uint32_t *__restrict__ tile_rec_start)
-{
+    extern __shared__ __align__(16) uint8_t bwd_smem_raw[];
+    BwdSmem &sm = *reinterpret_cast<BwdSmem *>(bwd_smem_raw);
     if (ws.status[1]) return;
-    const size_t t = (size_t)blockIdx.x * 8 + (threadIdx.x >> 5);
-    if (t >= (size_t)d.NV * d.T) return;
-    const int lane = threadIdx.x & 31;
-    const int view = (int)(t / d.T), tile = (int)(t % d.T);
-    const int ox = (tile % d.gx) * GA_BLOCK_X, oy = (tile / d.gx) * GA_BLOCK_Y;
-    const uint32_t start = ws.tile_start[t], end = ws.tile_start[t + 1];
-    const float *rec_base = ws.rec + (size_t)view * d.P * GA_REC_F;
-    uint32_t sum = 0;
-    for (uint32_t i = start + lane; i < end; i += 32) {
-        const float4 bb = __ldg(reinterpret_cast<const float4 *>(rec_base + (size_t)ws.ids[i] * GA_REC_F) + 4);
-        sum += (uint32_t)clipped_box_area(bb, ox, oy);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    if (lane == 0) tile_rec_start[t] = sum;
-}
-
-// exclusive scan of the tile totals (one block); sets the fallback flag when the buffer is too small
-__global__ void __launch_bounds__(1024)
-bwd_scan_area_kernel(RasterDims d, RasterWs ws, uint32_t *__restrict__ tile_rec_start)
-{
-    __shared__ uint32_t s_warp[32];
-    __shared__ uint32_t s_carry;
-    if (ws.status[1]) return;
-    const int n = d.NV * d.T;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int base = 0; base < n; base += 1024) {
-        const int i = base + threadIdx.x;
-        const uint32_t v = i < n ? tile_rec_start[i] : 0u;
-        uint32_t x = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-            if (lane >= o) x += y;
-        }
-        if (lane == 31) s_warp[warp] = x;
-        __syncthreads();
-        if (warp == 0) {
-            const uint32_t wv = s_warp[lane];
-            uint32_t wx = wv;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t y = __shfl_up_sync(0xffffffffu, wx, o);
-                if (lane >= o) wx += y;
-            }
-            s_warp[lane] = wx - wv;
-        }
-        __syncthreads();
-        const uint32_t excl = s_carry + s_warp[warp] + x - v;
-        if (i < n) tile_rec_start[i] = excl;
-        __syncthreads();
-        if (threadIdx.x == 1023) s_carry = excl + v;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) tile_rec_start[n] = s_carry;     // total records needed; > capacity -> the fused kernel runs instead
-}
-
-// the record buffer of the split backward is too small for this launch: every split kernel exits, the fused one runs
-__device__ __forceinline__ bool bwd_lists_overflow(const RasterDims &d, const BwdLists &L)
-{
-    return L.tile_rec_start[d.NV * d.T] > L.capacity;
-}
-
-// LISTS: only the normal / colour records are needed in shared memory (alpha and depth come from the list entries);
-// the 16 KB that frees pay for a deeper ring of list rows
-template <bool LISTS>
-struct BwdASmem {
-    float4 rec[LISTS ? 2 : 6][CHUNK];
-    uint32_t off[CHUNK];            // start of the instance's slice, relative to the tile's base
-    int cnt[CHUNK];
-    uint32_t wsum[8];
-    int maxc, maxn;
-};
-
-#ifndef GA_BWD_A_TMA
-#define GA_BWD_A_TMA 1              /* list rows of single-chunk tiles through cp.async.bulk + mbarriers */
-#endif
-#define BWD_A_RING 9                /* 4 KB list rows in flight per CTA (static shared memory stays below 48 KB) */
-
-// 1-D bulk copy global -> shared with mbarrier completion (SASS: UBLKCP): one 4 KB list row per call
-__device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gsrc, uint32_t bytes, uint64_t *bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(
-                     sm90::smem_u32(smem_dst)),
-                 "l"(gsrc), "r"(bytes), "r"(sm90::smem_u32(bar))
-                 : "memory");
-}
-
-// LISTS = true: the pairs come from the per-pixel contribution lists the forward recorded (RasterWs.lists): every lane
-// walks ITS pixel's entries back to front -- {list position, alpha, depth} -- so there is no cull test, no pair
-// evaluation and no wasted round on a surfel that does not reach alpha >= 1/255 at this pixel; alpha and depth are
-// the forward's own bits.  LISTS = false recomputes (tiles whose lists overflowed, or list_k == 0).
-template <bool LISTS>
-__global__ void __launch_bounds__(256, BWD_A_CTAS)
-render_bwd_a_kernel(RasterDims d, RasterWs ws, BwdLists L, const float *__restrict__ bg,
-                    const float *__restrict__ dL_dcolor, const float *__restrict__ dL_dallmap)
-{
-    __shared__ BwdASmem<LISTS> sm;
-    constexpr int REC_NR = LISTS ? 0 : 3, REC_GB = LISTS ? 1 : 5;
-    if (ws.status[1] || bwd_lists_overflow(d, L)) return;
-    const int view = blockIdx.z;
-    const int tile = blockIdx.y * d.gx + blockIdx.x;
-    {
-        const bool listed = d.list_k > 0 && ws.tile_flag[(size_t)view * d.T + tile] == 0;
-        if (listed != LISTS) return;                   // block-uniform: the other instantiation handles this tile
-    }
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int ox = blockIdx.x * GA_BLOCK_X, oy = blockIdx.y * GA_BLOCK_Y;
-    const int lx0 = (warp & 1) * 8, ly0 = (warp >> 1) * 4;
-    const int lxi = lx0 + (lane & 7), lyi = ly0 + (lane >> 3);
-    const int pxi = ox + lxi, pyi = oy + lyi;
-    const int pix_local = lyi * 16 + lxi;
-    const bool inside = pxi < d.W && pyi < d.H;
-    const float pfx = (float)pxi, pfy = (float)pyi;
-    const float bx_lo = (float)(ox + lx0), bx_hi = (float)(ox + lx0 + 7);
-    const float by_lo = (float)(oy + ly0), by_hi = (float)(oy + ly0 + 3);
-
-    const size_t gt = (size_t)view * d.T + tile;
-    const uint32_t start = ws.tile_start[gt];
-    const uint32_t tile_base = L.tile_rec_start[gt];
-    const size_t HW = (size_t)d.H * d.W;
-    const size_t pix = inside ? (size_t)pyi * d.W + pxi : 0;
-    const float *fT = ws.final_T + (size_t)view * 3 * HW;
-    const int32_t *nc = ws.n_contrib + (size_t)view * 2 * HW;
-    const float *rec_base = ws.rec + (size_t)view * d.P * GA_REC_F;
-
-    const float T_final = inside ? fT[pix] : 0.f;
-    float T = T_final;
-    const int last_contributor = inside ? nc[pix] : 0;
-    const int median_contributor = inside ? nc[pix + HW] : 0;
-    float dpx0 = 0, dpx1 = 0, dpx2 = 0, dL_ddepth = 0, dL_daccum = 0, dL_dreg = 0;
-    float dn0 = 0, dn1 = 0, dn2 = 0, dL_dmedian = 0;
-    if (inside) {
-        const float *gc = dL_dcolor + (size_t)view * 3 * HW;
-        const float *ga = dL_dallmap + (size_t)view * 7 * HW;
-        dpx0 = gc[pix]; dpx1 = gc[pix + HW]; dpx2 = gc[pix + 2 * HW];
-        dL_ddepth = ga[pix]; dL_daccum = ga[pix + HW];
-        dn0 = ga[pix + 2 * HW]; dn1 = ga[pix + 3 * HW]; dn2 = ga[pix + 4 * HW];
-        dL_dmedian = ga[pix + 5 * HW]; dL_dreg = ga[pix + 6 * HW];
-    }
-    const float final_D = inside ? fT[pix + HW] : 0.f, final_D2 = inside ? fT[pix + 2 * HW] : 0.f;
-    const float final_A = 1 - T_final;
-    const float bg_dot_dpixel = bg[0] * dpx0 + bg[1] * dpx1 + bg[2] * dpx2;
-    float last_alpha = 0, v_last = 0, v_acc = 0, last_dL_dT = 0;        // one scalar suffix recurrence (see the fused kernel)
-    // LISTS: this pixel's entries, walked from the last contribution to the first.
-    //  * tiles whose surfel list fits one chunk (nearly all): ROW mode.  Row k of the tile's list array is one
-    //    contiguous 4 KB block {entry k of the 256 pixels}; thread 0 streams the rows the tile uses, last row first,
-    //    through a ring of BWD_A_RING shared-memory slots with cp.async.bulk + full/empty mbarriers (three rows ahead
-    //    of the consumers); at row k the lanes whose pixel has more than k contributions take their entry from the slot.
-    //  * longer tiles: every lane walks its own list with three entries in flight in registers (`e`, `e1`, `e2`).
-    const uint4 *my_list = nullptr;
-    const char *tile_rows = nullptr;
-    int kk = -1, nl = 0;
-    uint4 e = make_uint4(0u, 0u, 0u, 0u), e1 = e, e2 = e;
-    __shared__ __align__(128) uint4 s_rows[LISTS ? BWD_A_RING : 1][LISTS ? 256 : 1];
-    __shared__ uint64_t s_full[BWD_A_RING], s_empty[BWD_A_RING];
-    if (LISTS) {
-        const uint4 *tl = ws.lists + ((size_t)view * d.T + tile) * (size_t)d.list_k * 256;
-        tile_rows = reinterpret_cast<const char *>(tl);
-        my_list = tl + pix_local;
-        nl = inside ? ws.n_list[(size_t)view * HW + pix] : 0;
-    }
-
-    if (threadIdx.x == 0) {
-        sm.maxc = 0;
-        sm.maxn = 0;
-        if (LISTS) {
-#pragma unroll
-            for (int i = 0; i < BWD_A_RING; i++) { sm90::mbar_init(&s_full[i], 1); sm90::mbar_init(&s_empty[i], 8); }
-            sm90::fence_barrier_init();
-        }
-    }
-    __syncthreads();
-    {
-        int m = last_contributor, mn = nl;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
-            mn = max(mn, __shfl_xor_sync(0xffffffffu, mn, o));
-        }
-        if (lane == 0) { atomicMax(&sm.maxc, m); atomicMax(&sm.maxn, mn); }
-    }
-    __syncthreads();
-    const int total = sm.maxc;          // list positions [0,total) matter; the rest keep inst_cnt == 0 (memset)
-    uint32_t run = 0;                   // records handed out to the chunks staged so far
-    const bool rows_mode = LISTS && GA_BWD_A_TMA && total <= CHUNK;          // block-uniform
-    const int maxn = sm.maxn;
-    auto issue_row = [&](const int j) {                                   // thread 0 only: j-th row in processing order
-        const int slot = j % BWD_A_RING, use = j / BWD_A_RING;
-        if (use > 0) sm90::mbar_wait(&s_empty[slot], (uint32_t)((use - 1) & 1));      // all 8 warps are done with its last row
-        sm90::mbar_expect_tx(&s_full[slot], 4096u);
-        bulk_g2s(&s_rows[slot][0], tile_rows + (size_t)(maxn - 1 - j) * 4096, 4096u, &s_full[slot]);
-    };
-    if (LISTS) {
-        if (rows_mode) {
-            if (threadIdx.x == 0)
-                for (int j = 0; j < min(maxn, BWD_A_RING - 2); j++) issue_row(j);
-        } else {
-            kk = nl - 1;
-            if (kk >= 0) e = __ldg(my_list + (size_t)kk * 256);
-            if (kk >= 1) e1 = __ldg(my_list + (size_t)(kk - 1) * 256);
-            if (kk >= 2) e2 = __ldg(my_list + (size_t)(kk - 2) * 256);
-#pragma unroll
-            for (int q = 3; q < 8; q++)
-                if (kk >= q) asm volatile("prefetch.global.L2 [%0];" ::"l"(my_list + (size_t)(kk - q) * 256));
-        }
-    }
-
-    for (int hi = total; hi > 0; hi -= CHUNK) {
-        const int lo = max(0, hi - CHUNK);
-        const int cnt = hi - lo;
-        // stage positions lo..hi-1; slot t holds position hi-1-t (back to front); slice length = clipped box area
-        uint32_t area = 0;
-        if ((int)threadIdx.x < cnt) {
-            const uint32_t id = ws.ids[start + (hi - 1 - threadIdx.x)];
-            const float4 *src = reinterpret_cast<const float4 *>(rec_base + (size_t)id * GA_REC_F);
-            float4 q4;
-            if (LISTS) {
-                sm.rec[REC_NR][threadIdx.x] = __ldg(src + 3);
-                sm.rec[REC_GB][threadIdx.x] = __ldg(src + 5);
-                q4 = __ldg(src + 4);
-            } else {
-                float4 q[6];
-#pragma unroll
-                for (int k = 0; k < 6; k++) { q[k] = __ldg(src + k); sm.rec[k][threadIdx.x] = q[k]; }
-                q4 = q[4];
-            }
-            area = (uint32_t)clipped_box_area(q4, ox, oy);
-        }
-        uint32_t x = area;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-            if (lane >= o) x += y;
-        }
-        if (lane == 31) sm.wsum[warp] = x;
-        __syncthreads();
-        uint32_t wbase = 0, chunk_total = 0;
-#pragma unroll
-        for (int k = 0; k < 8; k++) { const uint32_t wv = sm.wsum[k]; if (k < warp) wbase += wv; chunk_total += wv; }
-        const uint32_t my_off = run + wbase + x - area;
-        sm.off[threadIdx.x] = my_off;
-        sm.cnt[threadIdx.x] = 0;
-        if ((int)threadIdx.x < cnt) L.inst_off[start + (hi - 1 - threadIdx.x)] = tile_base + my_off;
-        __syncthreads();
-
-        // one (pixel, surfel) contribution: the compositing recurrences backwards + the 16-byte record for kernel B
-        auto contribute = [&](const int jj, const int contributor, const float alpha, const float c_d) {
-                    const float4 nr = sm.rec[REC_NR][jj], gb = sm.rec[REC_GB][jj];
-                    const float inv1ma = fast_rcp(1.f - alpha);
-                    T = T * inv1ma;
-                    const float w = alpha * T;
-                    float dL_dz = 0.0f;
-                    const float inv_cd = fast_rcp(c_d);
-                    const float m_d = GA_M_C0 - GA_M_C1 * inv_cd;
-                    const float dmd_dd = GA_M_C1 * inv_cd * inv_cd;
-                    if (contributor == median_contributor - 1) dL_dz += dL_dmedian;
-                    const float dL_dweight = (final_D2 + m_d * m_d * final_A - 2 * m_d * final_D) * dL_dreg;
-                    const float dL_dmd = 2.0f * (T * alpha) * (m_d * final_A - final_D) * dL_dreg;
-                    dL_dz += dL_dmd * dmd_dd;
-                    const float v = ((nr.w * dpx0 + gb.x * dpx1) + (gb.y * dpx2 + c_d * dL_ddepth)) +
-                                    ((nr.x * dn0 + nr.y * dn1) + (nr.z * dn2 + dL_daccum));
-                    v_acc = last_alpha * v_last + (1.f - last_alpha) * v_acc;
-                    v_last = v;
-                    float dL_dalpha = (v - v_acc) + (dL_dweight - last_dL_dT);
-                    last_dL_dT = dL_dweight * alpha + (1 - alpha) * last_dL_dT;
-                    dL_dalpha *= T;
-                    last_alpha = alpha;
-                    dL_dalpha += (-T_final * inv1ma) * bg_dot_dpixel;
-                    dL_dz += w * dL_ddepth;
-                    const int slot = atomicAdd(&sm.cnt[jj], 1);          // < the instance's clipped box area by construction
-                    L.records[(size_t)tile_base + sm.off[jj] + (uint32_t)slot] =
-                        make_uint4((uint32_t)pix_local, __float_as_uint(dL_dalpha), __float_as_uint(dL_dz), __float_as_uint(w));
-        };
-        if (LISTS && rows_mode) {
-            for (int j = 0; j < maxn; j++) {
-                const int k = maxn - 1 - j, slot = j % BWD_A_RING;
-                if (threadIdx.x == 0 && j + BWD_A_RING - 2 < maxn) issue_row(j + BWD_A_RING - 2);
-                sm90::mbar_wait(&s_full[slot], (uint32_t)((j / BWD_A_RING) & 1));
-                if (nl > k) {
-                    const uint4 cur = s_rows[slot][pix_local];
-                    contribute(hi - 1 - (int)cur.x, (int)cur.x, __uint_as_float(cur.y), __uint_as_float(cur.z));
-                }
-                __syncwarp();
-                if (lane == 0) sm90::mbar_arrive(&s_empty[slot]);          // this warp has read row k out of the slot
-            }
-        } else if (LISTS) {
-            while (true) {
-                const bool active = kk >= 0 && (int)e.x >= lo;      // entries are in descending list position
-                if (!__any_sync(0xffffffffu, active)) break;
-                if (active) {
-                    const uint4 cur = e;
-                    e = e1; e1 = e2;
-                    if (kk >= 3) e2 = __ldg(my_list + (size_t)(kk - 3) * 256);   // entries kk-1, kk-2, kk-3 are in flight
-                    // ... and the row 8 below is asked into L2 (the list rows stream from HBM exactly once)
-                    if (kk >= 8) asm volatile("prefetch.global.L2 [%0];" ::"l"(my_list + (size_t)(kk - 8) * 256));
-                    kk--;
-                    contribute(hi - 1 - (int)cur.x, (int)cur.x, __uint_as_float(cur.y), __uint_as_float(cur.z));
-                }
-            }
-        } else if constexpr (!LISTS) {
-        for (int sb = 0; sb < cnt; sb += 32) {
-            bool hit = false;
-            if (sb + lane < cnt) {
-                const float4 bb = sm.rec[4][sb + lane];
-                hit = !(bb.y < bx_lo || bb.x > bx_hi || bb.w < by_lo || bb.z > by_hi);
-            }
-            unsigned mask = __ballot_sync(0xffffffffu, hit);
-            unsigned mine = 0;
-            while (mask) {
-                const int b = __ffs(mask) - 1;
-                mask &= mask - 1;
-                const float4 bb = sm.rec[4][sb + b];
-                if (pfx >= bb.x && pfx <= bb.y && pfy >= bb.z && pfy <= bb.w && (hi - 1 - (sb + b)) < last_contributor)
-                    mine |= 1u << b;
-            }
-            if (!inside) mine = 0;
-            while (__any_sync(0xffffffffu, mine != 0)) {
-                const bool active = mine != 0;
-                const int bsel = active ? __ffs(mine) - 1 : 0;
-                mine &= mine - 1;
-                const int jj = sb + bsel;
-                const float4 a = sm.rec[0][jj], b = sm.rec[1][jj], c = sm.rec[2][jj];
-                PixelGeom pg;
-                float k0, k1, k2, l0, l1, l2;
-                const bool ok = active && eval_pair(a, b, c, pfx, pfy, pg, k0, k1, k2, l0, l1, l2);
-                if (ok) contribute(jj, hi - 1 - jj, pg.alpha, pg.depth);
-            }
-        }
-        }
-        __syncthreads();
-        if ((int)threadIdx.x < cnt) L.inst_cnt[start + (hi - 1 - threadIdx.x)] = (uint32_t)sm.cnt[threadIdx.x];
-        run += chunk_total;
-        // sm.rec / off / cnt are rewritten by the next chunk's staging only after every thread passed the barrier above
-        // and read its own cnt entry -- the staging below writes rec first, and off/cnt after its own barrier
-    }
-}
-
-template <int TPI>
-__global__ void __launch_bounds__(BWD_B_THREADS, BWD_B_CTAS)
-render_bwd_b_kernel(RasterDims d, RasterWs ws, BwdLists L, const float *__restrict__ dL_dcolor,
-                    const float *__restrict__ dL_dallmap, float *__restrict__ grad_acc, const int tile_filter)
-{
-    __shared__ float4 s_up[2][256];
-    if (ws.status[1] || bwd_lists_overflow(d, L)) return;
-    const int view = blockIdx.z;
-    const int tile = blockIdx.y * d.gx + blockIdx.x;
-    // tile_filter 1: only tiles whose records came from the list-walking kernel A; 2: only the flagged (recomputed)
-    // ones -- the two chains A<true> -> B(1) and A<false> -> B(2) run on two streams; 0: every tile
-    if (tile_filter && (ws.tile_flag[(size_t)view * d.T + tile] != 0) != (tile_filter == 2)) return;
-    const int ox = blockIdx.x * GA_BLOCK_X, oy = blockIdx.y * GA_BLOCK_Y;
-    const size_t gt = (size_t)view * d.T + tile;
-    const uint32_t start = ws.tile_start[gt], end = ws.tile_start[gt + 1];
-    const int total = (int)(end - start);
-    if (total == 0) return;
-    {
-      for (int px = threadIdx.x; px < 256; px += BWD_B_THREADS) {
-        const int lxi = px & 15, lyi = px >> 4;
-        const int pxi = ox + lxi, pyi = oy + lyi;
-        float4 ua = make_float4(0.f, 0.f, 0.f, 0.f), ub = ua;
-        if (pxi < d.W && pyi < d.H) {
-            const size_t HW = (size_t)d.H * d.W, pix = (size_t)pyi * d.W + pxi;
-            const float *gc = dL_dcolor + (size_t)view * 3 * HW;
-            const float *ga = dL_dallmap + (size_t)view * 7 * HW;
-            ua = make_float4(gc[pix], gc[pix + HW], gc[pix + 2 * HW], ga[pix + 2 * HW]);
-            ub = make_float4(ga[pix + 3 * HW], ga[pix + 4 * HW], 0.f, 0.f);
-        }
-        s_up[0][px] = ua;              // index = ly * 16 + lx = the records' pixel field
-        s_up[1][px] = ub;
-      }
-    }
-    __syncthreads();
-    const float *rec_base = ws.rec + (size_t)view * d.P * GA_REC_F;
-    float *acc_base = grad_acc + (size_t)view * d.P * GA_GRAD_F;
-    const int lane = threadIdx.x & 31;
-    const int sub = threadIdx.x % TPI;
-    constexpr int IPB = BWD_B_THREADS / TPI;    // instances per pass
-    constexpr int NH = 512 / BWD_B_THREADS;     // instances each thread files in the counting sort
-    // Instances carry 0 .. ~30 records; a warp's pass lasts as long as its longest instance.  So the tile's instances
-    // are handled in super-chunks of 512: a counting sort by record count (descending, empty ones dropped) decides
-    // which instance each lane group takes, and every warp gets instances of similar length.
-    __shared__ int s_bin[64];
-    __shared__ uint16_t s_perm[512];
-    __shared__ int s_m;
-    // count / surfel id / slice start of the super-chunk's instances, loaded together while the sort runs: a pass then
-    // starts with ONE round trip (geometry record + first list records, independent) instead of four dependent ones
-    __shared__ uint32_t s_cnt[512], s_id[512], s_off[512];
-    for (int c0 = 0; c0 < total; c0 += 512) {
-        const int cn = min(512, total - c0);
-        if (threadIdx.x < 64) s_bin[threadIdx.x] = 0;
-        __syncthreads();
-        int myn[NH];
-#pragma unroll
-        for (int h = 0; h < NH; h++) {
-            const int i = h * BWD_B_THREADS + threadIdx.x;
-            myn[h] = i < cn ? (int)L.inst_cnt[start + c0 + i] : 0;
-            if (i < cn) {
-                s_cnt[i] = (uint32_t)myn[h];
-                s_id[i] = ws.ids[start + c0 + i];
-                s_off[i] = L.inst_off[start + c0 + i];
-            }
-            if (myn[h] > 0) atomicAdd(&s_bin[min(myn[h], 63)], 1);
-        }
-        __syncthreads();
-        if (threadIdx.x < 32) {
-            // exclusive prefix over the bins in DESCENDING count order (bin 63 first); bin 0 is unused
-            const int hi_bin = 63 - 2 * threadIdx.x, lo_bin = hi_bin - 1;
-            const int vh = s_bin[hi_bin], vl = lo_bin >= 1 ? s_bin[lo_bin] : 0;
-            int x = vh + vl;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int y = __shfl_up_sync(0xffffffffu, x, o);
-                if ((int)threadIdx.x >= o) x += y;
-            }
-            const int excl = x - (vh + vl);
-            s_bin[hi_bin] = excl;
-            if (lo_bin >= 1) s_bin[lo_bin] = excl + vh;
-            if (threadIdx.x == 31) s_m = x;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int h = 0; h < NH; h++)
-            if (myn[h] > 0) s_perm[atomicAdd(&s_bin[min(myn[h], 63)], 1)] = (uint16_t)(h * BWD_B_THREADS + threadIdx.x);
-        __syncthreads();
-        const int m = s_m;
-    for (int base = 0; base < m; base += IPB) {
-        const int slot = base + threadIdx.x / TPI;
-        const bool valid = slot < m;
-        const int li = valid ? (int)s_perm[slot] : 0;
-        const int n = valid ? (int)s_cnt[li] : 0;
-        float g[GA_GRAD_F];
-#pragma unroll
-        for (int f = 0; f < GA_GRAD_F; f++) g[f] = 0.f;
-        uint32_t id = 0;
-        if (n > 0) {
-            id = s_id[li];
-            const float4 *src = reinterpret_cast<const float4 *>(rec_base + (size_t)id * GA_REC_F);
-            const float4 a = __ldg(src), b = __ldg(src + 1), c = __ldg(src + 2);
-            const float opa = c.w;
-            const uint4 *lst = L.records + s_off[li];
-            auto process = [&](const uint4 rc) {
-                const int pix = (int)rc.x;
-                const float dL_dalpha = __uint_as_float(rc.y), dL_dz = __uint_as_float(rc.z), w = __uint_as_float(rc.w);
-                const float pfx = (float)(ox + (pix & 15)), pfy = (float)(oy + (pix >> 4));
-                PixelGeom pg;
-                float k0, k1, k2, l0, l1, l2;
-                eval_pair(a, b, c, pfx, pfy, pg, k0, k1, k2, l0, l1, l2);      // same code path as kernel A: same bits
-                const float G = pg.G;
-                const float dL_dG = opa * dL_dalpha;                           // 0.99 clamp passed through (upstream)
-                if (pg.use3d) {
-                    const float dL_ds0 = dL_dG * -G * pg.s0 + dL_dz * b.z;
-                    const float dL_ds1 = dL_dG * -G * pg.s1 + dL_dz * b.w;
-                    const float ip = fast_rcp(pg.p2);
-                    const float q0 = dL_ds0 * ip, q1 = dL_ds1 * ip;
-                    const float q2 = -(q0 * pg.s0 + q1 * pg.s1);
-                    const float dk0 = l1 * q2 - l2 * q1, dk1 = l2 * q0 - l0 * q2, dk2 = l0 * q1 - l1 * q0;
-                    const float dl0 = q1 * k2 - q2 * k1, dl1 = q2 * k0 - q0 * k2, dl2 = q0 * k1 - q1 * k0;
-                    g[0] -= dk0; g[1] -= dk1; g[2] -= dk2;
-                    g[3] -= dl0; g[4] -= dl1; g[5] -= dl2;
-                    g[6] += pfx * dk0 + pfy * dl0 + dL_dz * pg.s0;
-                    g[7] += pfx * dk1 + pfy * dl1 + dL_dz * pg.s1;
-                    g[8] += pfx * dk2 + pfy * dl2 + dL_dz;
-                } else {
-                    g[9] += dL_dG * (-G * GA_FILTER_INV_SQUARE * pg.dx);
-                    g[10] += dL_dG * (-G * GA_FILTER_INV_SQUARE * pg.dy);
-                    g[8] += dL_dz;
-                }
-                g[14] += G * dL_dalpha;
-                const float4 ua = s_up[0][pix], ub = s_up[1][pix];
-                g[15] += w * ua.x; g[16] += w * ua.y; g[17] += w * ua.z;
-                g[11] += w * ua.w; g[12] += w * ub.x; g[13] += w * ub.y;
-            };
-#if BWD_B_UNROLL == 2
-            // two records per iteration: two independent dependency chains per lane (the kernel is latency bound)
-            uint4 n0 = sub < n ? __ldg(lst + sub) : make_uint4(0u, 0u, 0u, 0u);
-            uint4 n1 = sub + TPI < n ? __ldg(lst + sub + TPI) : n0;
-            for (int r = sub; r < n; r += 2 * TPI) {
-                const uint4 r0 = n0;
-                // no second record: reuse the first one's pixel with zero upstream terms (adds exact zeros), so both
-                // bodies run unconditionally and the compiler can interleave them
-                const uint4 r1 = (r + TPI < n) ? n1 : make_uint4(n0.x, 0u, 0u, 0u);
-                if (r + 2 * TPI < n) n0 = __ldg(lst + r + 2 * TPI);
-                if (r + 3 * TPI < n) n1 = __ldg(lst + r + 3 * TPI);
-                process(r0);
-                process(r1);
-            }
-#else
-            uint4 nxt = sub < n ? __ldg(lst + sub) : make_uint4(0u, 0u, 0u, 0u);
-            for (int r = sub; r < n; r += TPI) {
-                const uint4 rc = nxt;
-                if (r + TPI < n) nxt = __ldg(lst + r + TPI);           // the next record's load overlaps this one's math
-                process(rc);
-            }
-#endif
-        }
-        if (__any_sync(0xffffffffu, n > 0)) {
-            float *dst = acc_base + (size_t)id * GA_GRAD_F;          // lanes without records carry zeros (id 0, adds skipped)
-            reduce_scatter18<TPI>(g, lane, dst);
-        }
-    }
-        __syncthreads();                         // s_bin / s_perm are rebuilt for the next super-chunk
-    }
-}
-
-static int g_bwd_split = -1;
-
-// slice layout of the split backward's record buffer: per-tile sums of the clipped cull-box areas + their scan.
-// Called by the forward (list_k > 0) on a side stream, concurrently with the composite, or by the backward.
-cudaError_t ga_launch_bwd_slices(const RasterDims &d, const RasterWs &w, uint32_t *tile_rec_start, cudaStream_t s)
-{
-    const int tiles = d.NV * d.T;
-    bwd_tile_area_kernel<<<(tiles + 7) / 8, 256, 0, s>>>(d, w, tile_rec_start);
-    bwd_scan_area_kernel<<<1, 1024, 0, s>>>(d, w, tile_rec_start);
-    return cudaGetLastError();
-}
-
-cudaError_t ga_launch_render_fwd_with_slices(const RasterDims &d, const RasterWs &w, const float *bg, float *out_color,
-                                             float *out_allmap, cudaStream_t s)
-{
-    // the LISTS forward kernel leaves every tile's slice total in tile_rec_start; one small block turns them into offsets
-    cudaError_t e = ga_launch_render_fwd(d, w, bg, out_color, out_allmap, s);
-    if (e != cudaSuccess) return e;
-    bwd_scan_area_kernel<<<1, 1024, 0, s>>>(d, w, w.tile_rec_start);
-    return cudaGetLastError();
+    if (d.list_k > 0 && ws.tile_flag[(size_t)blockIdx.z * d.T + blockIdx.y * d.gx + blockIdx.x] == 0)
+        bwd_tile<true>(d, ws, sm, bg, dL_dcolor, dL_dallmap, grad_acc);
+    else
+        bwd_tile<false>(d, ws, sm, bg, dL_dcolor, dL_dallmap, grad_acc);
 }
 
 cudaError_t ga_launch_render_bwd(const RasterDims &d, const RasterWs &w, const float *bg,
-                                 const float *dL_dcolor, const float *dL_dallmap,
-                                 float *grad_acc, const BwdLists &lists_in, cudaStream_t s)
+                                 const float *dL_dcolor, const float *dL_dallmap, float *grad_acc, cudaStream_t s)
 {
     static GaPerDevice attr_set;
     if (ga_first_use_on_device(attr_set)) {
@@ -1225,47 +704,7 @@ cudaError_t ga_launch_render_bwd(const RasterDims &d, const RasterWs &w, const f
                                              (int)sizeof(BwdSmem));
         if (e != cudaSuccess) return e;
     }
-    if (g_bwd_split < 0) {
-        const char *e = getenv("GA_B200_BWD_SPLIT");        // 0: always the fused kernel (A/B comparisons)
-        g_bwd_split = (e && e[0] == '0') ? 0 : 1;
-    }
     dim3 grid(d.gx, d.gy, d.NV);
-    BwdLists lists = lists_in;
-    const bool split = g_bwd_split && lists.records && lists.capacity > 0;
-    if (split) {
-        cudaError_t e;
-        if (d.list_k > 0) {
-            lists.tile_rec_start = w.tile_rec_start;                 // laid out by the forward
-        } else if ((e = ga_launch_bwd_slices(d, w, lists.tile_rec_start, s)) != cudaSuccess) {
-            return e;
-        }
-        if (d.list_k > 0) {
-            // tiles whose per-pixel lists overflowed are few and long: their recompute kernel runs beside the
-            // list-walking one instead of after it
-            // tiles whose per-pixel lists overflowed are few and long: their chain (recompute kernel A -> kernel B on
-            // those tiles) runs on the side stream beside the list-walking chain instead of in front of / behind it
-            GaSide *g = ga_side();
-            if (g) {
-                cudaEventRecord(g->fork, s);
-                cudaStreamWaitEvent(g->st, g->fork, 0);
-                render_bwd_a_kernel<false><<<grid, 256, 0, g->st>>>(d, w, lists, bg, dL_dcolor, dL_dallmap);
-                render_bwd_b_kernel<BWD_B_TPI><<<grid, BWD_B_THREADS, 0, g->st>>>(d, w, lists, dL_dcolor, dL_dallmap, grad_acc, 2);
-                cudaEventRecord(g->join, g->st);
-                render_bwd_a_kernel<true><<<grid, 256, 0, s>>>(d, w, lists, bg, dL_dcolor, dL_dallmap);
-                render_bwd_b_kernel<BWD_B_TPI><<<grid, BWD_B_THREADS, 0, s>>>(d, w, lists, dL_dcolor, dL_dallmap, grad_acc, 1);
-                cudaStreamWaitEvent(s, g->join, 0);
-            } else {
-                render_bwd_a_kernel<true><<<grid, 256, 0, s>>>(d, w, lists, bg, dL_dcolor, dL_dallmap);
-                render_bwd_a_kernel<false><<<grid, 256, 0, s>>>(d, w, lists, bg, dL_dcolor, dL_dallmap);
-                render_bwd_b_kernel<BWD_B_TPI><<<grid, BWD_B_THREADS, 0, s>>>(d, w, lists, dL_dcolor, dL_dallmap, grad_acc, 0);
-            }
-        } else {
-            render_bwd_a_kernel<false><<<grid, 256, 0, s>>>(d, w, lists, bg, dL_dcolor, dL_dallmap);
-            render_bwd_b_kernel<BWD_B_TPI><<<grid, BWD_B_THREADS, 0, s>>>(d, w, lists, dL_dcolor, dL_dallmap, grad_acc, 0);
-        }
-    }
-    // fused kernel: the whole job when the split path is off, a no-op or the fallback (record buffer too small) otherwise
-    render_bwd_kernel<<<grid, 256, sizeof(BwdSmem), s>>>(d, w, bg, dL_dcolor, dL_dallmap, grad_acc,
-                                                         split ? lists.tile_rec_start + d.NV * d.T : nullptr, lists.capacity);
+    render_bwd_kernel<<<grid, 256, sizeof(BwdSmem), s>>>(d, w, bg, dL_dcolor, dL_dallmap, grad_acc);
     return cudaGetLastError();
 }

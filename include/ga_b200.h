@@ -48,11 +48,11 @@ typedef struct GaRasterLayout {
     size_t ids;         /* uint32[max_instances]  sorted surfel index per instance */
     size_t final_T;     /* float[NV][3][H*W]  T, M1, M2 */
     size_t n_contrib;   /* int32[NV][2][H*W]  last contributor, median contributor */
-    size_t inst_off;    /* uint32[max_instances]  backward: start of the instance's record slice */
-    size_t inst_cnt;    /* uint32[max_instances]  backward: records in it */
+    size_t inst_off;    /* unused (0 bytes) */
+    size_t inst_cnt;    /* uint32[max_instances]  (list_k > 0) contributions of every instance, counted by the forward */
     size_t n_list;      /* int32[NV][H*W]         (list_k > 0) contributions recorded per pixel */
     size_t tile_flag;   /* uint32[NV*T]           (list_k > 0) 1: a pixel of the tile had more than list_k */
-    size_t tile_rec_start; /* uint32[NV*T+1]      (list_k > 0) slice layout of the backward's record buffer */
+    size_t tile_rec_start; /* unused (0 bytes) */
     size_t lists;       /* uint4[NV*T][list_k][256] (list_k > 0) {list position, alpha bits, depth bits, 0} */
 } GaRasterLayout;
 
@@ -163,9 +163,8 @@ int ga_raster_get_variant(int *radius_formula, int *quat_norm_grad);
  */
 int ga_raster_set_tuning(int fwd_group);
 
-/* Bytes of scratch the backward wants: gradient accumulators [NV*P][18] (mandatory) + the global record lists of
- * the split backward (64 records of 16 bytes per (surfel, view)).  A smaller buffer that still holds the
- * accumulators is accepted: the backward then runs its fused shared-memory kernel. */
+/* Bytes of scratch the backward wants: the gradient accumulators [NV*P][18].  A larger buffer is accepted; the
+ * rest of it is not used. */
 size_t ga_raster_backward_scratch_bytes(int batch, int P, int views);
 
 /*
