@@ -4,24 +4,20 @@
 // Restates upstream forward.cu / backward.cu renderCUDA
 // (github.com/hbb1/diff-surfel-rasterization; called from
 // /root/reference/nsr/gs_surfel.py:100-114).  Differences in HOW, not WHAT:
-//  * each warp owns an 8x4 pixel block; for every group of 32 staged surfels
-//    the lanes test the surfels' conservative cull boxes (computed in K1)
-//    against the warp's block and the warp only evaluates the hits.  The cull
-//    box contains every pixel that can reach alpha >= 1/255, so results are
-//    identical to evaluating every (pixel, surfel) pair.
+//  * the forward evaluates only the (pixel, surfel) pairs inside each surfel's
+//    conservative cull box (computed in K1), all of them in parallel, and then
+//    composites every pixel from shared memory.  The cull box contains every
+//    pixel that can reach alpha >= 1/255, so results are identical to
+//    evaluating every (pixel, surfel) pair.
 //  * the backward walks each tile back to front, keeps the per-(pixel, surfel)
 //    records in shared memory, accumulates each surfel's gradient in registers
 //    and issues one global atomic per (tile, surfel, component).
 #include "raster_common.cuh"
 #include "device_once.cuh"
-#include <cstdlib>
 
 #define CHUNK 256
 #ifndef GA_LIST_STCS
 #define GA_LIST_STCS 0
-#endif
-#ifndef GA_FWD_GROUP_DEFAULT
-#define GA_FWD_GROUP_DEFAULT 8
 #endif
 
 // single-instruction approximations (MUFU.RCP / MUFU.EX2, <= 2 ulp): the IEEE division and the range-checked
@@ -74,52 +70,77 @@ __device__ __forceinline__ bool eval_pair(const float4 a, const float4 b, const 
     return o.alpha >= 1.0f / 255.0f;
 }
 
+// A surfel's cull box clipped to the pixels [ox, xmax] x [oy, ymax] of a tile, as tile-local integers.  A pixel
+// (px, py) of that range lies in the box exactly when bb.x <= px <= bb.y and bb.z <= py <= bb.w.  w = h = 0 when the
+// box misses the range (also for the empty box +-1e30 of a surfel that can never reach alpha >= 1/255).
+struct TileBox { int x0, y0, w, h; };
+__device__ __forceinline__ TileBox clip_box(const float4 bb, int ox, int oy, int xmax, int ymax)
+{
+    const float x0 = ceilf(fmaxf(bb.x, (float)ox)), x1 = floorf(fminf(bb.y, (float)xmax));
+    const float y0 = ceilf(fmaxf(bb.z, (float)oy)), y1 = floorf(fminf(bb.w, (float)ymax));
+    if (!(x1 >= x0 && y1 >= y0)) return {0, 0, 0, 0};
+    return {(int)x0 - ox, (int)y0 - oy, (int)(x1 - x0) + 1, (int)(y1 - y0) + 1};
+}
+
 // Forward staging record (tile-local, computed once per (tile, surfel) by the
 // staging thread): with o = tile origin, k_o = o.x*Tw - Tu, l_o = o.y*Tw - Tv,
 //   p(dx,dy) = (k_o + dx*Tw) x (l_o + dy*Tw) = C + dx*A + dy*B,
 //   C = k_o x l_o, A = Tw x l_o, B = k_o x Tw            (Tw x Tw = 0)
 // which is upstream's cross(k, l) re-associated around the tile origin (all
 // terms stay O(tile size), so no precision is lost) and costs 6 FMAs per pixel.
-//  f0 = C.x C.y C.z A.x | f1 = A.y A.z B.x B.y | f2 = B.z Tw.x Tw.y Tw.z
-//  f3 = xy.x-o.x xy.y-o.y opacity - | f4 = cull box (tile-local x0 x1 y0 y1)
-//  f5 = n.x n.y n.z r | f6 = g b - -
-// Lane groups.  A warp owns an 8x4 pixel block; GS = 32 evaluates one surfel per round for the whole block
-// (warp-uniform shared-memory reads).  With the C2 scene a surfel's cull box covers ~25 pixels, so only ~9 of the 32
-// lanes of a hit carry a contributing pixel.  GS = 16 splits the warp into two 4x4 blocks, GS = 8 into four 4x2
-// blocks; every group walks ITS OWN list of hits, so a round evaluates up to 32 / GS different surfels (2 or 4
-// distinct shared-memory addresses per load instead of one).  C2 scene (tools/raster_rounds.py): 44 rounds per warp
-// and chunk with GS = 32, 32 with GS = 16, 26 with GS = 8 (17.5 with one list per lane, but per-lane lists make every
-// load a 32-address gather: 0.208 vs 0.199 ms in round 1).  Measured: 209 / 181 / 176 us per 6-view launch.  Results do not depend on GS:
-// the per-pixel sequence of contributing surfels is the same.
+//  rec[0] = C.x C.y C.z A.x | rec[1] = A.y A.z B.x B.y | rec[2] = B.z Tw.x Tw.y Tw.z
+//  rec[3] = xy.x-o.x xy.y-o.y opacity - | rec[4] = n.x n.y n.z r | rec[5] = g b - -
+//
+// The tile's instances are staged in chunks of 256 list positions.  Each slot also gets its cull box clipped to the
+// tile's pixels inside the image (origin, width, a reciprocal for the division by the width) and its pair count
+// w * h; an exclusive scan of the counts gives each slot's pair base.  The chunk is cut into WINDOWS of consecutive
+// slots whose pairs fit FWD_PAIRS.  A box holds at most 256 pixels, so every window holds at least one slot.  Per
+// window:
+//   phase 1 (pair-parallel): the threads take consecutive pairs of the window's (slot, pixel of the clipped box)
+//     enumeration, find the slot by a binary search over the pair bases and evaluate the pair.  A pair that reaches
+//     alpha >= 1/255 stores {alpha, depth} at its pair index and sets the slot's bit in its pixel's slot mask.
+//     Pixels outside a box never reach alpha >= 1/255 (the box is conservative), so nothing else is evaluated.
+//   phase 2 (pixel-parallel): every thread composites its pixel's set bits in ascending slot order, i.e. list order,
+//     reading {alpha, depth} back from the pair buffer.  The compositing state stays in registers across windows.
+// C2 scene (tools/raster_rounds.py): phase 1 needs about half the warp rounds of evaluating every surfel whose box
+// meets a 4x2 pixel group, and no compositing round waits on an evaluation.
 //
 // LISTS: the kernel also records, per pixel, every surfel that contributed -- {position in the tile list, alpha,
 // depth} -- into a tile-major array (entry k of the tile's 256 pixels is one contiguous 4 KB row, so a warp's store is
 // four full 128-byte lines).  The backward then walks exactly these entries: no cull tests, no pair re-evaluation for
 // pairs that do not contribute, and the contribution decisions are the forward's own bits.  It also counts every
 // instance's contributions (inst_cnt), which sizes that instance's records in the backward exactly.
-template <int GS, bool LISTS>
-__global__ void __launch_bounds__(256, 4)
+// Three CTAs per SM: FwdSmem is about 67 KB.  A 2048-pair buffer fits four CTAs per SM, but on C2 it measured slower
+// (render_fwd 0.343 against 0.318 ms, H100 SXM at 400 W): more chunks need a second window, and each window costs
+// barriers and a pass over the masks.
+#define FWD_PAIRS 4096              /* window pair buffer, 32 KB */
+
+struct FwdSmem {
+    float4 rec[6][CHUNK];           // the chunk's staged records, see above
+    float2 pair[FWD_PAIRS];         // {alpha, depth} of the window's passing pairs, by pair index
+    uint32_t mask[CHUNK / 32][256]; // per pixel: the window's slots whose pair passed, slot t at bit t & 31 of word t >> 5
+    int base[CHUNK + 1];            // pair base of every slot relative to the chunk; base[CHUNK] = the chunk's pairs
+    uint32_t box[CHUNK];            // clipped box: x0 | y0 << 4 | w << 8 | (65536 / w + 1) << 13
+    int cnt[CHUNK];                 // LISTS: contributions of each staged instance
+    int wsum[8];
+};
+
+template <bool LISTS>
+__global__ void __launch_bounds__(256, 3)
 render_fwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
                   float *__restrict__ out_color, float *__restrict__ out_allmap)
 {
-    constexpr int NG = 32 / GS;                                  // groups per warp
-    constexpr int GW = GS == 32 ? 8 : 4;                         // group block width / height in pixels
-    constexpr int GH = GS == 8 ? 2 : 4;
-    __shared__ float4 s_rec[7][CHUNK];
-    __shared__ int s_cnt[LISTS ? CHUNK : 1];                     // LISTS: contributions of each staged instance
+    extern __shared__ __align__(16) uint8_t fwd_smem_raw[];
+    FwdSmem &sm = *reinterpret_cast<FwdSmem *>(fwd_smem_raw);
     if (ws.status[1]) return;
     const int view = blockIdx.z;
     const int tile = blockIdx.y * d.gx + blockIdx.x;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int grp = lane / GS, gl = lane % GS;
     const int ox = blockIdx.x * GA_BLOCK_X, oy = blockIdx.y * GA_BLOCK_Y;
-    const int wx0 = (warp & 1) * 8, wy0 = (warp >> 1) * 4;       // warp's 8x4 block, tile-local
-    // group blocks tile the warp block: GS=16 -> 2 side by side (4x4); GS=8 -> 2x2 arrangement of 4x2 blocks
-    const int lx0 = wx0 + (GS == 32 ? 0 : (grp & 1) * 4), ly0 = wy0 + (GS == 8 ? (grp >> 1) * 2 : 0);
-    const int lxi = lx0 + (gl % GW), lyi = ly0 + (gl / GW);
+    const int lxi = (warp & 1) * 8 + (lane & 7), lyi = (warp >> 1) * 4 + (lane >> 3);   // a warp owns an 8x4 block
+    const int pix_local = lyi * 16 + lxi;
     const int pxi = ox + lxi, pyi = oy + lyi;
     const bool inside = pxi < d.W && pyi < d.H;
-    const float dxf = (float)lxi, dyf = (float)lyi;
     const float oxf = (float)ox, oyf = (float)oy;
 
     const uint32_t start = ws.tile_start[(size_t)view * d.T + tile];
@@ -133,12 +154,13 @@ render_fwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
     int last_contributor = 0, median_contributor = -1;
     int nl = 0;                                                    // LISTS: contributions of this pixel so far
     uint4 *my_list = nullptr;
-    if (LISTS) my_list = ws.lists + ((size_t)view * d.T + tile) * (size_t)d.list_k * 256 + (lyi * 16 + lxi);
+    if (LISTS) my_list = ws.lists + ((size_t)view * d.T + tile) * (size_t)d.list_k * 256 + pix_local;
 
     for (int c0 = 0; c0 < total; c0 += CHUNK) {
         if (__syncthreads_count(done) == 256) break;
         const int cnt = min(CHUNK, total - c0);
-        if (LISTS) s_cnt[threadIdx.x] = 0;
+        if (LISTS) sm.cnt[threadIdx.x] = 0;
+        int npairs = 0;
         if ((int)threadIdx.x < cnt) {
             const uint32_t id = ws.ids[start + c0 + threadIdx.x];
             const float4 *src = reinterpret_cast<const float4 *>(rec_base + (size_t)id * GA_REC_F);
@@ -150,36 +172,49 @@ render_fwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
             const float Cx = k1 * l2 - k2 * l1, Cy = k2 * l0 - k0 * l2, Cz = k0 * l1 - k1 * l0;
             const float Ax = b.w * l2 - c.x * l1, Ay = c.x * l0 - b.z * l2, Az = b.z * l1 - b.w * l0;
             const float Bx = k1 * c.x - k2 * b.w, By = k2 * b.z - k0 * c.x, Bz = k0 * b.w - k1 * b.z;
-            s_rec[0][threadIdx.x] = make_float4(Cx, Cy, Cz, Ax);
-            s_rec[1][threadIdx.x] = make_float4(Ay, Az, Bx, By);
-            s_rec[2][threadIdx.x] = make_float4(Bz, b.z, b.w, c.x);
-            s_rec[3][threadIdx.x] = make_float4(c.y - oxf, c.z - oyf, c.w, 0.f);
-            s_rec[4][threadIdx.x] = make_float4(bb.x - oxf, bb.y - oxf, bb.z - oyf, bb.w - oyf);
-            s_rec[5][threadIdx.x] = nr;
-            s_rec[6][threadIdx.x] = gb;
+            sm.rec[0][threadIdx.x] = make_float4(Cx, Cy, Cz, Ax);
+            sm.rec[1][threadIdx.x] = make_float4(Ay, Az, Bx, By);
+            sm.rec[2][threadIdx.x] = make_float4(Bz, b.z, b.w, c.x);
+            sm.rec[3][threadIdx.x] = make_float4(c.y - oxf, c.z - oyf, c.w, 0.f);
+            sm.rec[4][threadIdx.x] = nr;
+            sm.rec[5][threadIdx.x] = gb;
+            const TileBox q = clip_box(bb, ox, oy, min(ox + 15, d.W - 1), min(oy + 15, d.H - 1));
+            npairs = q.w * q.h;
+            sm.box[threadIdx.x] = npairs ? (uint32_t)(q.x0 | q.y0 << 4 | q.w << 8 | (65536 / q.w + 1) << 13) : 0u;
         }
-        __syncthreads();
-        for (int g0 = 0; g0 < cnt; g0 += 32) {
-            if (__all_sync(0xffffffffu, done)) break;
-            const int j = g0 + lane;
-            // lane tests surfel j against the block of every group of the warp; each lane keeps its group's ballot
-            unsigned mask = 0;
-            {
-                float4 bb = make_float4(1e30f, -1e30f, 1e30f, -1e30f);
-                if (j < cnt) bb = s_rec[4][j];
+        int incl = npairs;              // inclusive scan of the pair counts over the slots
 #pragma unroll
-                for (int q = 0; q < NG; q++) {
-                    const float qx0 = (float)(wx0 + (GS == 32 ? 0 : (q & 1) * 4)), qy0 = (float)(wy0 + (GS == 8 ? (q >> 1) * 2 : 0));
-                    const bool hit = !(bb.y < qx0 || bb.x > qx0 + (float)(GW - 1) || bb.w < qy0 || bb.z > qy0 + (float)(GH - 1));
-                    const unsigned m = __ballot_sync(0xffffffffu, hit);
-                    if (q == grp) mask = m;
-                }
-            }
-            while (__any_sync(0xffffffffu, mask != 0)) {
-                const bool active = mask != 0;
-                const int jj = g0 + (active ? __ffs(mask) - 1 : 0);
-                mask &= mask - 1;
-                const float4 f0 = s_rec[0][jj], f1 = s_rec[1][jj], f2 = s_rec[2][jj], f3 = s_rec[3][jj];
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += y;
+        }
+        if (lane == 31) sm.wsum[warp] = incl;
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < 8; k++) incl += k < warp ? sm.wsum[k] : 0;
+        sm.base[threadIdx.x] = incl - npairs;
+        if (threadIdx.x == CHUNK - 1) sm.base[CHUNK] = incl;
+
+        int t0 = 0, base = 0;           // window = slots [t0, t1); base = pair base of slot t0
+        while (t0 < cnt) {
+#pragma unroll
+            for (int k = 0; k < CHUNK / 32; k++) sm.mask[k][threadIdx.x] = 0u;
+            const int t1 = t0 + __syncthreads_count((int)threadIdx.x >= t0 && (int)threadIdx.x < cnt &&
+                                                    incl - base <= FWD_PAIRS);
+            // ---------------- phase 1: one thread per (slot, pixel) pair of the window
+            const int wpairs = sm.base[t1] - base;
+            for (int q = threadIdx.x; q < wpairs; q += 256) {
+                const int Q = base + q;
+                int jj = t0;            // the last slot whose base is <= Q: it has pairs, and Q is one of them
+#pragma unroll
+                for (int step = CHUNK / 2; step > 0; step >>= 1)
+                    if (jj + step < t1 && sm.base[jj + step] <= Q) jj += step;
+                const uint32_t bx = sm.box[jj];
+                const int k = Q - sm.base[jj], w = (bx >> 8) & 31;
+                const int ry = (k * (int)(bx >> 13)) >> 16;               // k / w for k < 256, w <= 16
+                const int lx = (int)(bx & 15) + k - ry * w, ly = (int)((bx >> 4) & 15) + ry;
+                const float dxf = (float)lx, dyf = (float)ly;
+                const float4 f0 = sm.rec[0][jj], f1 = sm.rec[1][jj], f2 = sm.rec[2][jj], f3 = sm.rec[3][jj];
                 const float p0 = f0.x + dxf * f0.w + dyf * f1.z;
                 const float p1 = f0.y + dxf * f1.x + dyf * f1.w;
                 const float p2 = f0.z + dxf * f1.y + dyf * f2.x;
@@ -187,54 +222,72 @@ render_fwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
                 const float s0 = p0 * ip, s1 = p1 * ip;
                 const float rho3d = s0 * s0 + s1 * s1;
                 const float ddx = f3.x - dxf, ddy = f3.y - dyf;
-                const float rho2d = GA_FILTER_INV_SQUARE * (ddx * ddx + ddy * ddy);
+                // contracted explicitly: which of the two products the compiler fuses otherwise depends on the
+                // surrounding code, and the images' last bits depend on it
+                const float rho2d = GA_FILTER_INV_SQUARE * __fmaf_rn(ddx, ddx, __fmul_rn(ddy, ddy));
                 const float rho = fminf(rho3d, rho2d);
                 const float depth = (rho3d <= rho2d) ? (s0 * f2.y + s1 * f2.z) + f2.w : f2.w;
                 // power = -0.5*rho > 0 never happens for rho >= 0; NaN rho (p2 == 0) fails the alpha test
                 const float alpha = fminf(0.99f, f3.z * fast_ex2(rho * GA_NEG_HALF_LOG2E));
-                bool ok = active && !done && p2 != 0.0f && depth >= GA_NEAR_N && alpha >= 1.0f / 255.0f;
-                float test_T = 0.f;
-                if (ok) {
-                    test_T = T * (1 - alpha);
-                    if (test_T < 0.0001f) { done = true; ok = false; }
+                if (p2 != 0.0f && depth >= GA_NEAR_N && alpha >= 1.0f / 255.0f) {
+                    sm.pair[q] = make_float2(alpha, depth);
+                    atomicOr(&sm.mask[jj >> 5][ly * 16 + lx], 1u << (jj & 31));
                 }
-                if (__any_sync(0xffffffffu, ok)) {
-                    const float4 nr = s_rec[5][jj], gb = s_rec[6][jj];
-                    if (ok) {
-                        const int contributor = c0 + jj + 1;
-                        const float w = alpha * T;
-                        const float A = 1 - T;
-                        const float m = GA_M_C0 - GA_M_C1 * fast_rcp(depth);
-                        dist += (m * m * A + M2 - 2 * m * M1) * w;
-                        Dacc += depth * w;
-                        M1 += m * w;
-                        M2 += m * m * w;
-                        if (T > 0.5f) { median_depth = depth; median_contributor = contributor; }
-                        N0 += nr.x * w; N1 += nr.y * w; N2 += nr.z * w;
-                        C0 += nr.w * w; C1 += gb.x * w; C2 += gb.y * w;
-                        T = test_T;
-                        last_contributor = contributor;
-                        if (LISTS) {
-                            atomicAdd(&s_cnt[jj], 1);
-                            if (nl < d.list_k) {
-                                const uint4 ent = make_uint4((uint32_t)(contributor - 1), __float_as_uint(alpha),
-                                                             __float_as_uint(depth), 0u);
+            }
+            __syncthreads();
+            // ---------------- phase 2: one thread per pixel, its passing pairs in list order
+            if (!done) {
+                int wi = t0 >> 5;
+                const int wlast = (t1 - 1) >> 5;
+                uint32_t m = sm.mask[wi][pix_local];
+                while (true) {
+                    while (m == 0u && wi < wlast) m = sm.mask[++wi][pix_local];
+                    if (m == 0u) break;
+                    const int jj = wi * 32 + __ffs(m) - 1;
+                    m &= m - 1;
+                    const uint32_t bx = sm.box[jj];
+                    const int k = (lyi - (int)((bx >> 4) & 15)) * (int)((bx >> 8) & 31) + (lxi - (int)(bx & 15));
+                    const float2 ad = sm.pair[sm.base[jj] - base + k];
+                    const float alpha = ad.x, depth = ad.y;
+                    const float test_T = T * (1 - alpha);
+                    if (test_T < 0.0001f) { done = true; break; }
+                    const float4 nr = sm.rec[4][jj], gb = sm.rec[5][jj];
+                    const int contributor = c0 + jj + 1;
+                    const float w = alpha * T;
+                    const float A = 1 - T;
+                    const float mm = GA_M_C0 - GA_M_C1 * fast_rcp(depth);
+                    dist += (mm * mm * A + M2 - 2 * mm * M1) * w;
+                    Dacc += depth * w;
+                    M1 += mm * w;
+                    M2 += mm * mm * w;
+                    if (T > 0.5f) { median_depth = depth; median_contributor = contributor; }
+                    N0 += nr.x * w; N1 += nr.y * w; N2 += nr.z * w;
+                    C0 += nr.w * w; C1 += gb.x * w; C2 += gb.y * w;
+                    T = test_T;
+                    last_contributor = contributor;
+                    if (LISTS) {
+                        atomicAdd(&sm.cnt[jj], 1);
+                        if (nl < d.list_k) {
+                            const uint4 ent = make_uint4((uint32_t)(contributor - 1), __float_as_uint(alpha),
+                                                         __float_as_uint(depth), 0u);
 #if GA_LIST_STCS
-                                __stcs(my_list + (size_t)nl * 256, ent);       // written once, read once by the backward
+                            __stcs(my_list + (size_t)nl * 256, ent);       // written once, read once by the backward
 #else
-                                my_list[(size_t)nl * 256] = ent;
+                            my_list[(size_t)nl * 256] = ent;
 #endif
-                            }
-                            nl++;
                         }
+                        nl++;
                     }
                 }
             }
+            t0 = t1;
+            if (t0 < cnt) base = sm.base[t0];
+            // the next window rewrites the masks and pairs; once every pixel is saturated the chunk ends here
+            if (__syncthreads_count(done) == 256) break;
         }
-        __syncthreads();
         // every chunk holding a position below the tile's deepest contributor is staged here, so the backward finds
         // the exact record count of every instance it reads
-        if (LISTS && (int)threadIdx.x < cnt) ws.inst_cnt[start + c0 + threadIdx.x] = (uint32_t)s_cnt[threadIdx.x];
+        if (LISTS && (int)threadIdx.x < cnt) ws.inst_cnt[start + c0 + threadIdx.x] = (uint32_t)sm.cnt[threadIdx.x];
     }
     if (LISTS) {
         if (inside) ws.n_list[(size_t)view * d.H * d.W + (size_t)pyi * d.W + pxi] = nl;
@@ -258,33 +311,27 @@ render_fwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
     }
 }
 
-// GA_B200_FWD_GROUP=32|16|8 (or ga_raster_set_tuning) selects the lane-group size; see the kernel comment
-static int g_fwd_group = -1;
+// Kept for ABI compatibility: the forward no longer has a lane-group mapping to select (see include/ga_b200.h).
 extern "C" int ga_raster_set_tuning(int fwd_group)
 {
-    if (fwd_group != 32 && fwd_group != 16 && fwd_group != 8) return -1;
-    g_fwd_group = fwd_group;
-    return 0;
+    return (fwd_group == 32 || fwd_group == 16 || fwd_group == 8) ? 0 : -1;
 }
 
 cudaError_t ga_launch_render_fwd(const RasterDims &d, const RasterWs &w, const float *bg,
                                  float *out_color, float *out_allmap, cudaStream_t s)
 {
-    if (g_fwd_group < 0) {
-        const char *e = getenv("GA_B200_FWD_GROUP");
-        const int v = e ? atoi(e) : GA_FWD_GROUP_DEFAULT;
-        g_fwd_group = (v == 32 || v == 16 || v == 8) ? v : GA_FWD_GROUP_DEFAULT;
+    static GaPerDevice attr_set;
+    if (ga_first_use_on_device(attr_set)) {
+        cudaError_t e = cudaFuncSetAttribute(render_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)sizeof(FwdSmem));
+        if (e == cudaSuccess)
+            e = cudaFuncSetAttribute(render_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)sizeof(FwdSmem));
+        if (e != cudaSuccess) return e;
     }
     dim3 grid(d.gx, d.gy, d.NV);
-    if (d.list_k > 0) {
-        if (g_fwd_group == 32) render_fwd_kernel<32, true><<<grid, 256, 0, s>>>(d, w, bg, out_color, out_allmap);
-        else if (g_fwd_group == 16) render_fwd_kernel<16, true><<<grid, 256, 0, s>>>(d, w, bg, out_color, out_allmap);
-        else render_fwd_kernel<8, true><<<grid, 256, 0, s>>>(d, w, bg, out_color, out_allmap);
-    } else {
-        if (g_fwd_group == 32) render_fwd_kernel<32, false><<<grid, 256, 0, s>>>(d, w, bg, out_color, out_allmap);
-        else if (g_fwd_group == 16) render_fwd_kernel<16, false><<<grid, 256, 0, s>>>(d, w, bg, out_color, out_allmap);
-        else render_fwd_kernel<8, false><<<grid, 256, 0, s>>>(d, w, bg, out_color, out_allmap);
-    }
+    if (d.list_k > 0) render_fwd_kernel<true><<<grid, 256, sizeof(FwdSmem), s>>>(d, w, bg, out_color, out_allmap);
+    else render_fwd_kernel<false><<<grid, 256, sizeof(FwdSmem), s>>>(d, w, bg, out_color, out_allmap);
     return cudaGetLastError();
 }
 
@@ -404,10 +451,8 @@ __device__ __forceinline__ void reduce_scatter18(const float (&g)[GA_GRAD_F], in
 
 __device__ __forceinline__ int clipped_box_area(const float4 bb, int ox, int oy)
 {
-    const float x0 = fmaxf(bb.x, (float)ox), x1 = fminf(bb.y, (float)(ox + 15));
-    const float y0 = fmaxf(bb.z, (float)oy), y1 = fminf(bb.w, (float)(oy + 15));
-    const int wx = max(0, (int)floorf(x1) - (int)ceilf(x0) + 1), wy = max(0, (int)floorf(y1) - (int)ceilf(y0) + 1);
-    return wx * wy;
+    const TileBox q = clip_box(bb, ox, oy, ox + 15, oy + 15);
+    return q.w * q.h;
 }
 
 // LISTS = true: every thread walks ITS pixel's list entries -- {list position, alpha, depth}, the forward's own bits --

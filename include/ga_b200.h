@@ -157,9 +157,9 @@ int ga_raster_set_variant(int radius_formula, int quat_norm_grad);
 int ga_raster_get_variant(int *radius_formula, int *quat_norm_grad);
 
 /*
- * Scheduling knob of the forward composite (results do not depend on it): lanes per group that walks its own list of
- * hits inside a warp's 8x4 pixel block -- 32 (one surfel per warp round), 16 or 8 (default; env GA_B200_FWD_GROUP).
- * Returns -1 for any other value.
+ * No longer selects anything: the forward composite evaluates its (pixel, surfel) pairs in parallel and has no
+ * lane-group mapping left to choose.  Kept so that existing callers still link.  Returns 0 for the former group
+ * sizes 32, 16 and 8 and -1 for any other value.
  */
 int ga_raster_set_tuning(int fwd_group);
 
