@@ -31,23 +31,6 @@ extern "C" int ga_profile_read(float *ms, int n)
     return 5;
 }
 
-// side stream + events for work that is independent of the main stream's next kernel (one set per device)
-GaSide *ga_side()
-{
-    static GaSide sides[64];
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) return nullptr;
-    GaSide &g = sides[dev];
-    if (!g.st) {
-        if (cudaStreamCreateWithFlags(&g.st, cudaStreamNonBlocking) != cudaSuccess) { g.st = nullptr; return nullptr; }
-        cudaEventCreateWithFlags(&g.fork, cudaEventDisableTiming);
-        cudaEventCreateWithFlags(&g.join, cudaEventDisableTiming);
-    }
-    return &g;
-}
-
-
 static int g_radius_formula = GA_RADIUS_FORMULA, g_quat_norm_grad = GA_QUAT_NORM_GRAD;
 
 extern "C" int ga_raster_set_variant(int radius_formula, int quat_norm_grad)
@@ -104,7 +87,7 @@ extern "C" int ga_raster_layout_ex(int batch, int P, int views, int H, int W,
     L->rec = off;        off = align_up(off + NVP * GA_REC_F * sizeof(float), 256);
     L->depth = off;      off = align_up(off + NVP * sizeof(float), 256);
     L->rect = off;       off = align_up(off + NVP * sizeof(uint32_t), 256);
-    L->tile_count = off; off = align_up(off + NVT * GA_TILE_REPLICAS * sizeof(uint32_t), 256);
+    L->tile_count = off; off = align_up(off + NVT * (GA_TILE_REPLICAS + 1) * sizeof(uint32_t), 256);   // + big_tiles
     L->tile_start = off; off = align_up(off + (NVT + 1) * sizeof(uint32_t), 256);
     L->keys = off;       off = align_up(off + mi * sizeof(uint64_t), 256);
     L->ids = off;        off = align_up(off + mi * sizeof(uint32_t), 256);
@@ -120,7 +103,7 @@ extern "C" int ga_raster_layout_ex(int batch, int P, int views, int H, int W,
     return 0;
 }
 
-static void carve(const GaRasterLayout &L, void *base, RasterWs *w)
+static void carve(const GaRasterLayout &L, const RasterDims &d, void *base, RasterWs *w)
 {
     char *p = (char *)base;
     w->status = (int32_t *)(p + L.status);
@@ -128,6 +111,7 @@ static void carve(const GaRasterLayout &L, void *base, RasterWs *w)
     w->depth = (float *)(p + L.depth);
     w->rect = (uint32_t *)(p + L.rect);
     w->tile_count = (uint32_t *)(p + L.tile_count);
+    w->big_tiles = w->tile_count + (size_t)d.NV * d.T * GA_TILE_REPLICAS;
     w->tile_start = (uint32_t *)(p + L.tile_start);
     w->keys = (unsigned long long *)(p + L.keys);
     w->ids = (uint32_t *)(p + L.ids);
@@ -155,7 +139,7 @@ static int raster_forward_impl(int stage, const float *gauss13, int batch, int P
     ga_raster_layout_ex(batch, P, views, H, W, max_instances, list_k, &L);
     if (workspace_bytes < L.total_bytes) return GA_ERR_WORKSPACE;
     RasterWs w;
-    carve(L, workspace, &w);
+    carve(L, d, workspace, &w);
     cudaStream_t s = (cudaStream_t)stream;
     cudaError_t e;
     if (stage == 0 || stage == 1) {
@@ -278,7 +262,7 @@ extern "C" int ga_raster_backward_ex(const float *gauss13, int batch, int P, int
     const size_t need = bwd_acc_bytes(batch, P, views);                 // a larger buffer is accepted; the rest is unused
     if (scratch_bytes < need) return GA_ERR_WORKSPACE;
     RasterWs w;
-    carve(L, const_cast<void *>(workspace), &w);
+    carve(L, d, const_cast<void *>(workspace), &w);
     cudaStream_t s = (cudaStream_t)stream;
     cudaError_t e;
     float *grad_acc = (float *)scratch;

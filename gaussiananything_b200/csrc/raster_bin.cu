@@ -14,8 +14,14 @@
 #include "device_once.cuh"
 
 #define SCAN_THREADS 1024
+#define SCAN_TILES_PER_THREAD 8    // tiles per thread and pass: one pass covers 8192 tiles (C2: 6144)
 #define SORT_WARP_MAX 512          // tiles up to this many instances are sorted by a single warp in registers
 
+// One CTA.  Thread t owns tiles base + j * SCAN_THREADS + t (j < SCAN_TILES_PER_THREAD), so every load and store
+// instruction is coalesced.  A pass loads all the replica counters of its tiles in one wave, scans the tile sums
+// round by round in shared memory, then reads the counters again (from cache) and writes the tile starts and
+// cursors in one wave.  Tiles above SORT_WARP_MAX are appended to ws.big_tiles (in no particular order) and counted
+// in status[3].
 __global__ void __launch_bounds__(SCAN_THREADS)
 scan_tiles_kernel(RasterDims d, RasterWs ws)
 {
@@ -23,69 +29,77 @@ scan_tiles_kernel(RasterDims d, RasterWs ws)
     __shared__ uint32_t s_carry;
     __shared__ int s_big;
     const int n = d.NV * d.T;
-    int big = 0;                                   // tiles of this thread that need the block-level sort
     if (threadIdx.x == 0) { s_carry = 0; s_big = 0; }
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int base = 0; base < n; base += SCAN_THREADS) {
-        const int i = base + threadIdx.x;
-        uint32_t rep[GA_TILE_REPLICAS];
-        uint32_t v = 0u;
-        if (i < n) {
-            const uint4 *src = reinterpret_cast<const uint4 *>(ws.tile_count + (size_t)i * GA_TILE_REPLICAS);
+    const uint4 *cnt4 = reinterpret_cast<const uint4 *>(ws.tile_count);
+    for (int base = 0; base < n; base += SCAN_THREADS * SCAN_TILES_PER_THREAD) {
+        uint32_t v[SCAN_TILES_PER_THREAD];
+#pragma unroll
+        for (int j = 0; j < SCAN_TILES_PER_THREAD; j++) {
+            const int i = base + j * SCAN_THREADS + threadIdx.x;
+            v[j] = 0u;
 #pragma unroll
             for (int q = 0; q < GA_TILE_REPLICAS / 4; q++) {
-                const uint4 c = src[q];
-                rep[4 * q] = c.x; rep[4 * q + 1] = c.y; rep[4 * q + 2] = c.z; rep[4 * q + 3] = c.w;
+                const uint4 c = i < n ? cnt4[(size_t)i * (GA_TILE_REPLICAS / 4) + q] : make_uint4(0u, 0u, 0u, 0u);
+                v[j] += ((c.x + c.y) + c.z) + c.w;
             }
-#pragma unroll
-            for (int q = 0; q < GA_TILE_REPLICAS; q++) v += rep[q];
-            big += v > SORT_WARP_MAX;
         }
-        uint32_t x = v;
+        uint32_t excl[SCAN_TILES_PER_THREAD];
 #pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-            if (lane >= o) x += y;
-        }
-        if (lane == 31) s_warp[warp] = x;
-        __syncthreads();
-        if (warp == 0) {
-            uint32_t wv = s_warp[lane], wx = wv;
+        for (int j = 0; j < SCAN_TILES_PER_THREAD; j++) {
+            if (base + j * SCAN_THREADS >= n) { excl[j] = 0u; continue; }        // block-uniform
+            if (v[j] > SORT_WARP_MAX) ws.big_tiles[atomicAdd(&s_big, 1)] = (uint32_t)(base + j * SCAN_THREADS + threadIdx.x);
+            uint32_t x = v[j];
 #pragma unroll
             for (int o = 1; o < 32; o <<= 1) {
-                uint32_t y = __shfl_up_sync(0xffffffffu, wx, o);
-                if (lane >= o) wx += y;
+                uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
+                if (lane >= o) x += y;
             }
-            s_warp[lane] = wx - wv;   // exclusive warp offsets
+            if (lane == 31) s_warp[warp] = x;
+            __syncthreads();
+            if (warp == 0) {
+                uint32_t wv = s_warp[lane], wx = wv;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    uint32_t y = __shfl_up_sync(0xffffffffu, wx, o);
+                    if (lane >= o) wx += y;
+                }
+                s_warp[lane] = wx - wv;   // exclusive warp offsets
+            }
+            __syncthreads();
+            excl[j] = s_carry + s_warp[warp] + x - v[j];
+            __syncthreads();
+            if (threadIdx.x == SCAN_THREADS - 1) s_carry = excl[j] + v[j];
+            __syncthreads();
         }
-        __syncthreads();
-        const uint32_t carry = s_carry;
-        const uint32_t excl = carry + s_warp[warp] + x - v;
-        if (i < n) {
-            ws.tile_start[i] = excl;
+#pragma unroll
+        for (int j = 0; j < SCAN_TILES_PER_THREAD; j++) {
+            const int i = base + j * SCAN_THREADS + threadIdx.x;
+            if (i >= n) continue;
+            ws.tile_start[i] = excl[j];
             // every replica becomes the absolute fill cursor of its own sub-range of the tile's slots
-            uint32_t run = excl;
-            uint32_t cur[GA_TILE_REPLICAS];
+            uint32_t run = excl[j];
+            uint4 *dst = reinterpret_cast<uint4 *>(ws.tile_count) + (size_t)i * (GA_TILE_REPLICAS / 4);
 #pragma unroll
-            for (int q = 0; q < GA_TILE_REPLICAS; q++) { cur[q] = run; run += rep[q]; }
-            uint4 *dst = reinterpret_cast<uint4 *>(ws.tile_count + (size_t)i * GA_TILE_REPLICAS);
-#pragma unroll
-            for (int q = 0; q < GA_TILE_REPLICAS / 4; q++)
-                dst[q] = make_uint4(cur[4 * q], cur[4 * q + 1], cur[4 * q + 2], cur[4 * q + 3]);
+            for (int q = 0; q < GA_TILE_REPLICAS / 4; q++) {
+                const uint4 c = cnt4[(size_t)i * (GA_TILE_REPLICAS / 4) + q];
+                uint4 cur;
+                cur.x = run; run += c.x;
+                cur.y = run; run += c.y;
+                cur.z = run; run += c.z;
+                cur.w = run; run += c.w;
+                dst[q] = cur;
+            }
         }
-        __syncthreads();
-        if (threadIdx.x == SCAN_THREADS - 1) s_carry = excl + v;
-        __syncthreads();
     }
-    if (big) atomicAdd(&s_big, big);
     __syncthreads();
     if (threadIdx.x == 0) {
         const uint32_t total = s_carry;
         ws.tile_start[n] = total;
         ws.status[0] = (int32_t)total;
         ws.status[1] = ((int64_t)total > d.max_instances) ? 1 : 0;
-        ws.status[3] = s_big;                      // 0: sort_tiles_kernel has nothing to do and exits at once
+        ws.status[3] = s_big;                      // entries of ws.big_tiles
     }
 }
 
@@ -213,18 +227,45 @@ __device__ __forceinline__ void warp_sort_tile(unsigned long long *gk, uint32_t 
     }
 }
 
-// one warp per tile (tiles with more than SORT_WARP_MAX instances are left to sort_tiles_kernel)
-#ifndef SORT_WARP_THREADS
-#define SORT_WARP_THREADS 256
-#endif
-#ifndef SORT_WARP_CTAS
-#define SORT_WARP_CTAS (512 / SORT_WARP_THREADS)
-#endif
-__global__ void __launch_bounds__(SORT_WARP_THREADS, SORT_WARP_CTAS)
-sort_tiles_warp_kernel(RasterDims d, RasterWs ws)
+// One launch sorts every tile.  CTAs [0, big_ctas) take the tiles above SORT_WARP_MAX from ws.big_tiles, one block per
+// tile in shared memory (global memory above SORT_SMEM_KEYS); they are dispatched first, so their long tail runs
+// beside the warp-per-tile CTAs that follow, one warp per tile in registers.
+#define SORT_THREADS 256
+__global__ void __launch_bounds__(SORT_THREADS, 3)
+sort_tiles_kernel(RasterDims d, RasterWs ws, int big_ctas)
 {
+    __shared__ unsigned long long s_keys[SORT_SMEM_KEYS];
     if (ws.status[1]) return;
-    const size_t t = (size_t)blockIdx.x * (SORT_WARP_THREADS / 32) + (threadIdx.x >> 5);
+    if ((int)blockIdx.x < big_ctas) {
+        const int nbig = ws.status[3];
+        for (int b = blockIdx.x; b < nbig; b += big_ctas) {
+            const uint32_t t = ws.big_tiles[b];
+            const uint32_t start = ws.tile_start[t], end = ws.tile_start[t + 1];
+            const int n = (int)(end - start);
+            unsigned long long *gk = ws.keys + start;
+            if (n <= SORT_SMEM_KEYS) {
+                for (int i = threadIdx.x; i < n; i += blockDim.x) s_keys[i] = gk[i];
+                __syncthreads();
+                block_bitonic_sort(s_keys, n);
+                for (int i = threadIdx.x; i < n; i += blockDim.x) {
+                    const unsigned long long k = s_keys[i];
+                    gk[i] = k;
+                    ws.ids[start + i] = (uint32_t)(k & 0xffffffffull);
+                }
+                __syncthreads();                            // s_keys is reused by the next tile
+            } else {
+                // rare: a tile with more instances than fit in shared memory is sorted
+                // in place in global memory (L2 resident) by the same network.
+                if (threadIdx.x == 0) atomicAdd(&ws.status[2], 1);
+                block_bitonic_sort(gk, n);
+                for (int i = threadIdx.x; i < n; i += blockDim.x)
+                    ws.ids[start + i] = (uint32_t)(gk[i] & 0xffffffffull);
+                __syncthreads();
+            }
+        }
+        return;
+    }
+    const size_t t = (size_t)(blockIdx.x - big_ctas) * (SORT_THREADS / 32) + (threadIdx.x >> 5);
     if (t >= (size_t)d.NV * d.T) return;
     const int lane = threadIdx.x & 31;
     const uint32_t start = ws.tile_start[t], end = ws.tile_start[t + 1];
@@ -236,39 +277,6 @@ sort_tiles_warp_kernel(RasterDims d, RasterWs ws)
     else if (n <= 128) warp_sort_tile<4>(gk, gid, n, lane);
     else if (n <= 256) warp_sort_tile<8>(gk, gid, n, lane);
     else warp_sort_tile<16>(gk, gid, n, lane);
-}
-
-// tiles with more than SORT_WARP_MAX instances: one block per tile, a small persistent grid walks all tiles
-__global__ void __launch_bounds__(256)
-sort_tiles_kernel(RasterDims d, RasterWs ws)
-{
-    __shared__ unsigned long long s_keys[SORT_SMEM_KEYS];
-    if (ws.status[1] || ws.status[3] == 0) return;          // overflow, or no tile above the warp-sort limit
-    const size_t tiles = (size_t)d.NV * d.T;
-    for (size_t t = blockIdx.x; t < tiles; t += gridDim.x) {
-        const uint32_t start = ws.tile_start[t], end = ws.tile_start[t + 1];
-        const int n = (int)(end - start);
-        if (n <= SORT_WARP_MAX) continue;               // done by sort_tiles_warp_kernel (block-uniform branch)
-        unsigned long long *gk = ws.keys + start;
-        if (n <= SORT_SMEM_KEYS) {
-            for (int i = threadIdx.x; i < n; i += blockDim.x) s_keys[i] = gk[i];
-            __syncthreads();
-            block_bitonic_sort(s_keys, n);
-            for (int i = threadIdx.x; i < n; i += blockDim.x) {
-                const unsigned long long k = s_keys[i];
-                gk[i] = k;
-                ws.ids[start + i] = (uint32_t)(k & 0xffffffffull);
-            }
-            __syncthreads();                            // s_keys is reused by the next tile
-        } else {
-            // rare: a tile with more instances than fit in shared memory is sorted
-            // in place in global memory (L2 resident) by the same network.
-            if (threadIdx.x == 0) atomicAdd(&ws.status[2], 1);
-            block_bitonic_sort(gk, n);
-            for (int i = threadIdx.x; i < n; i += blockDim.x)
-                ws.ids[start + i] = (uint32_t)(gk[i] & 0xffffffffull);
-        }
-    }
 }
 
 cudaError_t ga_launch_binning(const RasterDims &d, const RasterWs &w, cudaStream_t s, int32_t *status_host,
@@ -285,20 +293,8 @@ cudaError_t ga_launch_binning(const RasterDims &d, const RasterWs &w, cudaStream
     }
     dim3 grid((d.P + 255) / 256, d.NV);
     scatter_kernel<<<grid, 256, 0, s>>>(d, w);
-    const int big_grid = d.NV * d.T < ga_sm_count() * 7 ? d.NV * d.T : ga_sm_count() * 7;      // 32 KB of keys per block: 7 blocks per SM
-    // the few tiles above the warp-sort limit are sorted by whole blocks (a long tail of a handful of CTAs): on the
-    // side stream, beside the warp-per-tile kernel that fills the GPU, instead of after it
-    GaSide *g = ga_side();
-    if (g) {
-        cudaEventRecord(g->fork, s);
-        cudaStreamWaitEvent(g->st, g->fork, 0);
-        sort_tiles_kernel<<<big_grid, 256, 0, g->st>>>(d, w);
-        cudaEventRecord(g->join, g->st);
-        sort_tiles_warp_kernel<<<(d.NV * d.T + SORT_WARP_THREADS / 32 - 1) / (SORT_WARP_THREADS / 32), SORT_WARP_THREADS, 0, s>>>(d, w);
-        cudaStreamWaitEvent(s, g->join, 0);
-    } else {
-        sort_tiles_warp_kernel<<<(d.NV * d.T + SORT_WARP_THREADS / 32 - 1) / (SORT_WARP_THREADS / 32), SORT_WARP_THREADS, 0, s>>>(d, w);
-        sort_tiles_kernel<<<big_grid, 256, 0, s>>>(d, w);
-    }
+    const int tiles = d.NV * d.T;
+    const int big_ctas = tiles < ga_sm_count() ? tiles : ga_sm_count();     // at most one big-tile CTA per SM
+    sort_tiles_kernel<<<big_ctas + (tiles + SORT_THREADS / 32 - 1) / (SORT_THREADS / 32), SORT_THREADS, 0, s>>>(d, w, big_ctas);
     return cudaGetLastError();
 }

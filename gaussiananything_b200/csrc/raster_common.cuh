@@ -45,6 +45,8 @@ struct RasterWs {
     float *depth;
     uint32_t *rect;
     uint32_t *tile_count;
+    uint32_t *big_tiles;       // tiles above the warp-sort limit, listed by the tile scan (status[3] entries); kept
+                               // in the tile_count region of the layout, after the counters
     uint32_t *tile_start;
     unsigned long long *keys;
     uint32_t *ids;
@@ -59,11 +61,6 @@ struct RasterWs {
     uint32_t *tile_flag;
     uint32_t *inst_cnt;        // (list_k > 0) contributions of every instance, counted by the forward
 };
-
-// a side stream + fork/join events per device for kernels that are independent of the main stream's next kernel
-// (few long CTAs that would otherwise serialise behind / in front of a grid-filling kernel); defined in raster_api.cu
-struct GaSide { cudaStream_t st = nullptr; cudaEvent_t fork = nullptr, join = nullptr; };
-GaSide *ga_side();
 
 // kernel launchers (defined in the .cu files, called from raster_api.cu)
 cudaError_t ga_launch_preprocess(const RasterDims &d, const RasterWs &w, const float *gauss13,

@@ -26,26 +26,40 @@ __device__ __forceinline__ void quat_to_rotmat(const float *q, float R[3][3])
     R[2][2] = 1.f - 2.f * (x * x + y * y);
 }
 
-__global__ void __launch_bounds__(256)
-preprocess_kernel(RasterDims d, RasterWs ws, const float *__restrict__ gauss13,
-                  const float *__restrict__ viewmats, const float *__restrict__ projmats,
-                  int32_t *__restrict__ out_radii)
+// T = (Tu, Tv, Tw): the surfel's ray-splat transform for one view.  K1 stores it in the record and K5 recomputes it
+// from the same inputs with the same operations (so with the same bits) instead of reading it back.
+__device__ __forceinline__ void surfel_transmat(const float R[3][3], float sx, float sy, float px, float py, float pz,
+                                                const float *pm, int W, int H, float Tu[3], float Tv[3], float Tw[3])
 {
-    __shared__ float s_g[256 * 13];
-    __shared__ float s_cam[32];
-    const int view = blockIdx.y;
-    const int b = view / d.views;
-    const int i0 = blockIdx.x * 256;
-    const int n = min(256, d.P - i0);
-    const float *src = gauss13 + ((size_t)b * d.P + i0) * 13;
-    for (int t = threadIdx.x; t < n * 13; t += 256) s_g[t] = src[t];
-    if (threadIdx.x < 16) s_cam[threadIdx.x] = viewmats[view * 16 + threadIdx.x];
-    else if (threadIdx.x < 32) s_cam[threadIdx.x] = projmats[view * 16 + threadIdx.x - 16];
-    __syncthreads();
-    if ((int)threadIdx.x >= n) return;
-    const int i = i0 + threadIdx.x;
+    float L0[3] = {R[0][0] * sx, R[1][0] * sx, R[2][0] * sx};
+    float L1[3] = {R[0][1] * sy, R[1][1] * sy, R[2][1] * sy};
+    const float hw = 0.5f * (float)W, hh = 0.5f * (float)H;
+    const float cw = 0.5f * (float)(W - 1), ch = 0.5f * (float)(H - 1);
+    {
+        float B0[3], B1[3], B3[3];   // columns j = 0,1,3 of B = M^T A
+        B0[0] = (L0[0] * pm[0] + L0[1] * pm[4]) + L0[2] * pm[8];
+        B0[1] = (L1[0] * pm[0] + L1[1] * pm[4]) + L1[2] * pm[8];
+        B0[2] = ((px * pm[0] + py * pm[4]) + pz * pm[8]) + pm[12];
+        B1[0] = (L0[0] * pm[1] + L0[1] * pm[5]) + L0[2] * pm[9];
+        B1[1] = (L1[0] * pm[1] + L1[1] * pm[5]) + L1[2] * pm[9];
+        B1[2] = ((px * pm[1] + py * pm[5]) + pz * pm[9]) + pm[13];
+        B3[0] = (L0[0] * pm[3] + L0[1] * pm[7]) + L0[2] * pm[11];
+        B3[1] = (L1[0] * pm[3] + L1[1] * pm[7]) + L1[2] * pm[11];
+        B3[2] = ((px * pm[3] + py * pm[7]) + pz * pm[11]) + pm[15];
+#pragma unroll
+        for (int r = 0; r < 3; r++) {
+            Tu[r] = B0[r] * hw + B3[r] * cw;
+            Tv[r] = B1[r] * hh + B3[r] * ch;
+            Tw[r] = B3[r];
+        }
+    }
+}
+
+__device__ __forceinline__ void preprocess_one(const RasterDims &d, const RasterWs &ws, const float *g,
+                                               const float *s_cam, int view, int i, float4 *rec_out,
+                                               int32_t *__restrict__ out_radii)
+{
     const size_t vi = (size_t)view * d.P + i;
-    const float *g = s_g + threadIdx.x * 13;
     const float *vm = s_cam, *pm = s_cam + 16;
     const int H = d.H, W = d.W;
 
@@ -66,30 +80,9 @@ preprocess_kernel(RasterDims d, RasterWs ws, const float *__restrict__ gauss13,
         float R[3][3];
         quat_to_rotmat(g + 6, R);
         const float sx = d.scale_modifier * g[4], sy = d.scale_modifier * g[5];
-        float L0[3] = {R[0][0] * sx, R[1][0] * sx, R[2][0] * sx};
-        float L1[3] = {R[0][1] * sy, R[1][1] * sy, R[2][1] * sy};
         float L2[3] = {R[0][2], R[1][2], R[2][2]};
-        const float hw = 0.5f * (float)W, hh = 0.5f * (float)H;
-        const float cw = 0.5f * (float)(W - 1), ch = 0.5f * (float)(H - 1);
         float Tu[3], Tv[3], Tw[3];
-        {
-            float B0[3], B1[3], B3[3];   // columns j = 0,1,3 of B = M^T A
-            B0[0] = (L0[0] * pm[0] + L0[1] * pm[4]) + L0[2] * pm[8];
-            B0[1] = (L1[0] * pm[0] + L1[1] * pm[4]) + L1[2] * pm[8];
-            B0[2] = ((px * pm[0] + py * pm[4]) + pz * pm[8]) + pm[12];
-            B1[0] = (L0[0] * pm[1] + L0[1] * pm[5]) + L0[2] * pm[9];
-            B1[1] = (L1[0] * pm[1] + L1[1] * pm[5]) + L1[2] * pm[9];
-            B1[2] = ((px * pm[1] + py * pm[5]) + pz * pm[9]) + pm[13];
-            B3[0] = (L0[0] * pm[3] + L0[1] * pm[7]) + L0[2] * pm[11];
-            B3[1] = (L1[0] * pm[3] + L1[1] * pm[7]) + L1[2] * pm[11];
-            B3[2] = ((px * pm[3] + py * pm[7]) + pz * pm[11]) + pm[15];
-#pragma unroll
-            for (int r = 0; r < 3; r++) {
-                Tu[r] = B0[r] * hw + B3[r] * cw;
-                Tv[r] = B1[r] * hh + B3[r] * ch;
-                Tw[r] = B3[r];
-            }
-        }
+        surfel_transmat(R, sx, sy, px, py, pz, pm, W, H, Tu, Tv, Tw);
         float nx = (vm[0] * L2[0] + vm[4] * L2[1]) + vm[8] * L2[2];
         float ny = (vm[1] * L2[0] + vm[5] * L2[1]) + vm[9] * L2[2];
         float nz = (vm[2] * L2[0] + vm[6] * L2[1]) + vm[10] * L2[2];
@@ -157,10 +150,9 @@ preprocess_kernel(RasterDims d, RasterWs ws, const float *__restrict__ gauss13,
     out_radii[vi] = radius_i;
     ws.depth[vi] = depth_out;
     ws.rect[vi] = rect_packed;
-    float4 *dst = reinterpret_cast<float4 *>(ws.rec + vi * GA_REC_F);
 #pragma unroll
-    for (int q = 0; q < 6; q++)
-        dst[q] = make_float4(rec[4 * q], rec[4 * q + 1], rec[4 * q + 2], rec[4 * q + 3]);
+    for (int q = 0; q < GA_REC_F / 4; q++)
+        rec_out[q] = make_float4(rec[4 * q], rec[4 * q + 1], rec[4 * q + 2], rec[4 * q + 3]);
     if (radius_i > 0) {
         const int x0 = rect_packed & 255, y0 = (rect_packed >> 8) & 255;
         const int x1 = (rect_packed >> 16) & 255, y1 = rect_packed >> 24;
@@ -168,6 +160,32 @@ preprocess_kernel(RasterDims d, RasterWs ws, const float *__restrict__ gauss13,
         for (int y = y0; y < y1; y++)
             for (int x = x0; x < x1; x++) atomicAdd(&tc[(y * d.gx + x) * GA_TILE_REPLICAS], 1u);
     }
+}
+
+// The CTA's 256 records are staged in shared memory and written out as whole lines (a thread's own record is
+// 96 bytes, so per-thread float4 stores would leave every store instruction touching 32 different lines).
+__global__ void __launch_bounds__(256, 4)
+preprocess_kernel(RasterDims d, RasterWs ws, const float *__restrict__ gauss13,
+                  const float *__restrict__ viewmats, const float *__restrict__ projmats,
+                  int32_t *__restrict__ out_radii)
+{
+    __shared__ float s_g[256 * 13];
+    __shared__ float s_cam[32];
+    __shared__ float4 s_rec[256 * GA_REC_F / 4];
+    const int view = blockIdx.y;
+    const int b = view / d.views;
+    const int i0 = blockIdx.x * 256;
+    const int n = min(256, d.P - i0);
+    const float *src = gauss13 + ((size_t)b * d.P + i0) * 13;
+    for (int t = threadIdx.x; t < n * 13; t += 256) s_g[t] = src[t];
+    if (threadIdx.x < 16) s_cam[threadIdx.x] = viewmats[view * 16 + threadIdx.x];
+    else if (threadIdx.x < 32) s_cam[threadIdx.x] = projmats[view * 16 + threadIdx.x - 16];
+    __syncthreads();
+    if ((int)threadIdx.x < n) preprocess_one(d, ws, s_g + threadIdx.x * 13, s_cam, view, i0 + threadIdx.x,
+                                             s_rec + threadIdx.x * (GA_REC_F / 4), out_radii);
+    __syncthreads();
+    float4 *dst = reinterpret_cast<float4 *>(ws.rec + ((size_t)view * d.P + i0) * GA_REC_F);
+    for (int t = threadIdx.x; t < n * (GA_REC_F / 4); t += 256) dst[t] = s_rec[t];
 }
 
 cudaError_t ga_launch_preprocess(const RasterDims &d, const RasterWs &w, const float *gauss13,
@@ -214,9 +232,9 @@ preprocess_bwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ gauss
             for (int r = 0; r < 3; r++) G[c][r] = ga[3 * c + r];
         const float gmx = ga[9], gmy = ga[10];
         if (gmx != 0.f || gmy != 0.f) {
-            const float *Tm = ws.rec + vi * GA_REC_F;
             const float t[3] = {9.f, 9.f, -1.f};
-            float Tu[3] = {Tm[0], Tm[1], Tm[2]}, Tv[3] = {Tm[3], Tm[4], Tm[5]}, Tw[3] = {Tm[6], Tm[7], Tm[8]};
+            float Tu[3], Tv[3], Tw[3];
+            surfel_transmat(R, sx, sy, px, py, pz, pm, d.W, d.H, Tu, Tv, Tw);
             float dd = 0.f;
 #pragma unroll
             for (int r = 0; r < 3; r++) dd += t[r] * Tw[r] * Tw[r];

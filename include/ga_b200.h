@@ -42,7 +42,7 @@ typedef struct GaRasterLayout {
     size_t rec;         /* float[NV*P][24]  Tu3 Tv3 Tw3 | xy2 opacity | normal3 | r | bbox x0 x1 y0 y1 | g b - - */
     size_t depth;       /* float[NV*P]      view-space z (0 when culled) */
     size_t rect;        /* uint32[NV*P]     x0 | y0<<8 | x1<<16 | y1<<24 (tile units) */
-    size_t tile_count;  /* uint32[NV*T*8]   scratch: per-tile counters, then fill cursors (8 replicas per tile) */
+    size_t tile_count;  /* uint32[NV*T*9]   scratch: per-tile counters, then fill cursors (8 replicas per tile); then the list of tiles above the warp-sort limit */
     size_t tile_start;  /* uint32[NV*T+1]   exclusive scan == tile ranges [start,end) */
     size_t keys;        /* uint64[max_instances]  (depth bits<<32 | surfel), sorted per tile */
     size_t ids;         /* uint32[max_instances]  sorted surfel index per instance */
