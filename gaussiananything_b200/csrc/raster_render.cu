@@ -349,7 +349,8 @@ cudaError_t ga_launch_render_fwd(const RasterDims &d, const RasterWs &w, const f
 //     record buffer.  The recurrence state stays in registers from one window to the next.
 //   phase B (instance-parallel): the window's non-empty instances, sorted by record count so that the lane pairs of a
 //     warp get instances of similar length, are walked by BWD_TPI lanes each; they re-derive the ray-splat geometry
-//     of every record with the same eval_pair() as the forward (same bits), accumulate the 18 gradient components in
+//     of every record with eval_pair() (upstream's cross(k, l) at the pixel; the forward's phase 1 evaluates the
+//     tile-origin form instead, so the bits can differ in the last place), accumulate the 18 gradient components in
 //     registers, reduce-scatter them over the lanes and add them to grad_acc: one global atomic per (tile, instance,
 //     non-zero component).
 // The records never leave the SM.  Tiles whose lists overflowed (and callers with list_k == 0) take the recompute

@@ -32,14 +32,32 @@ def layout(batch, P, views, H, W, max_instances, list_k=0):
     return L
 
 
-def workspace_views(ws, L, batch, P, views, H, W, max_instances):
-    """Typed views of the workspace sections (for tests / debugging)."""
+def tile_replicas():
+    """Counter replicas per tile in the workspace (GA_TILE_REPLICAS of the library build), read from the layout: with
+    64 tiles the counter region, R + 1 words per tile (the counters and the big-tile list), is a whole number of 256-byte
+    alignment units."""
+    L = layout(1, 1, 1, 128, 128, 1)
+    return (L.tile_start - L.tile_count) // (64 * 4) - 1
+
+
+def workspace_views(ws, L, batch, P, views, H, W, max_instances, list_k=0):
+    """Typed views of the workspace sections (for tests / debugging).  The list sections (lists, n_list, tile_flag)
+    exist only when the forward ran with list_k > 0; inst_cnt is written only then.  big_tiles holds status[3]
+    valid entries."""
     NV, T, HW = batch * views, ((W + 15) // 16) * ((H + 15) // 16), H * W
 
     def sec(off, dtype, n):
         esz = torch.empty(0, dtype=dtype).element_size()
         return ws[off:off + n * esz].view(dtype)
+    lists = {}
+    if list_k:
+        lists = dict(lists=sec(L.lists, torch.int32, NV * T * list_k * 256 * 4).view(NV * T, list_k, 256, 4),
+                     n_list=sec(L.n_list, torch.int32, NV * HW).view(NV, H, W),
+                     tile_flag=sec(L.tile_flag, torch.int32, NV * T))
     return dict(
+        lists,
+        big_tiles=sec(L.tile_count + NV * T * tile_replicas() * 4, torch.int32, NV * T),    # after the tile counters
+        inst_cnt=sec(L.inst_cnt, torch.int32, max_instances),
         status=sec(L.status, torch.int32, 16),
         rec=sec(L.rec, torch.float32, NV * P * 24).view(NV, P, 24),
         depth=sec(L.depth, torch.float32, NV * P).view(NV, P),

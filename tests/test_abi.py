@@ -41,6 +41,27 @@ def test_layout_is_host_only_and_monotonic():
     assert L.ga_raster_backward_scratch_bytes(1, 1000, 2) >= 1000 * 2 * 18 * 4
 
 
+def test_set_tuning_accepts_lane_groups_and_rejects_others():
+    """ga_raster_set_tuning stays in the C ABI for compatibility: it accepts the lane-group sizes 32 / 16 / 8 and
+    rejects anything else (it no longer selects anything in the forward)."""
+    from gaussiananything_b200 import _lib
+    L = _lib.lib()
+    L.ga_raster_set_tuning.argtypes = [C.c_int]
+    for grp in (32, 16, 8):
+        assert L.ga_raster_set_tuning(grp) == 0
+    assert L.ga_raster_set_tuning(7) != 0
+
+
+def test_tile_replicas_read_from_the_layout():
+    """raster.workspace_views finds the big-tile list after the tile counters, whose replica count it reads from the
+    layout; the layout grows by exactly that many words per tile plus one."""
+    from gaussiananything_b200 import raster
+    R = raster.tile_replicas()
+    assert R >= 1
+    a, b = raster.layout(1, 1, 1, 128, 128, 1), raster.layout(1, 1, 4, 128, 128, 1)      # 64 and 256 tiles
+    assert b.tile_start - b.tile_count == 256 * (R + 1) * 4 and a.tile_start - a.tile_count == 64 * (R + 1) * 4
+
+
 def test_forward_rejects_null_and_small_workspace():
     from gaussiananything_b200 import _lib
     L = _lib.lib()

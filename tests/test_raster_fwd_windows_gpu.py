@@ -42,7 +42,7 @@ def test_forward_multi_window_chunks_keep_state_and_match_oracle():
     nc0 = w0["n_contrib"].clone()
     c1, a1, r1, s1 = raster.forward_raw(g13, vm, pm, bgt, H, W, list_k=32)
     L, ws = s1["L"], s1["ws"]
-    w1 = raster.workspace_views(ws, L, 1, P, V, H, W, s1["max_instances"])
+    w1 = raster.workspace_views(ws, L, 1, P, V, H, W, s1["max_instances"], list_k=32)
 
     # the scene exercises what it is meant to: unbounded boxes, and chunks cut into several windows
     gx, gy = (W + 15) // 16, (H + 15) // 16
@@ -69,9 +69,9 @@ def test_forward_multi_window_chunks_keep_state_and_match_oracle():
     assert torch.equal(nc0, w1["n_contrib"])                       # last and median contributor
     # the per-instance counts add up to the per-pixel list lengths, tile by tile
     last = w1["n_contrib"][:, 0].cpu().numpy()
-    flags = ws[L.tile_flag:L.tile_flag + 4 * V * T].view(torch.int32).cpu().numpy()
-    n_list = ws[L.n_list:L.n_list + 4 * V * H * W].view(torch.int32).cpu().numpy().reshape(V, H, W)
-    inst_cnt = ws[L.inst_cnt:L.inst_cnt + 4 * int(tile_start[-1])].view(torch.int32).cpu().numpy()
+    flags = w1["tile_flag"].cpu().numpy()
+    n_list = w1["n_list"].cpu().numpy()
+    inst_cnt = w1["inst_cnt"].cpu().numpy()
     assert int(n_list.max()) > 3
     for v in range(V):
         for ty in range(gy):

@@ -509,36 +509,6 @@ def test_render_sharded_world1_matches_manual_loop():
             assert torch.equal(t, full[k][b, v]), (b, v, k)
 
 
-def test_forward_lane_groups_are_bit_identical():
-    """The forward kernel's lane-group size (32 = one surfel per warp round, 16 / 8 = two / four groups walking their
-    own hit lists) changes scheduling only: images, state and integers must be the same bits."""
-    import ctypes as C
-    from gaussiananything_b200 import _lib, raster
-    lib = _lib.lib()
-    lib.ga_raster_set_tuning.argtypes = [C.c_int]
-    dev = torch.device("cuda:0")
-    outs = {}
-    try:
-        for P, H, W, boost, seed in ((6000, 200, 176, 4.0, 70), (700, 96, 96, 40.0, 71)):
-            g = scene(P, seed, boost)
-            vs, ps, _, _ = cameras(2, start=seed)
-            g13 = torch.tensor(g, device=dev)[None]
-            for grp in (32, 16, 8):
-                assert lib.ga_raster_set_tuning(grp) == 0
-                c, a, r, st = raster.forward_raw(g13, torch.tensor(vs, device=dev)[None], torch.tensor(ps, device=dev)[None],
-                                                 torch.tensor([1.0, 0.4, 0.2], device=dev), H, W)
-                wsv = raster.workspace_views(st["ws"], st["L"], 1, P, 2, H, W, st["max_instances"])
-                outs[grp] = (c.clone(), a.clone(), wsv["n_contrib"].clone(), wsv["final_T"].clone())
-            for grp in (16, 8):
-                for x, y in zip(outs[32], outs[grp]):
-                    assert torch.equal(x, y), (P, grp)
-            o = oracle_view(g, vs[1], ps[1], [1.0, 0.4, 0.2], H, W)
-            assert rel_l2(outs[8][0][0, 1].cpu().numpy(), o["color"]) <= TOL
-        assert lib.ga_raster_set_tuning(7) != 0
-    finally:
-        lib.ga_raster_set_tuning(8)
-
-
 @pytest.mark.parametrize("list_k", [32, 3])
 def test_backward_from_recorded_lists_matches_recompute_and_oracle(list_k):
     """list_k > 0: the forward records every pixel's contributions and the backward walks them (no culling, no pair

@@ -23,12 +23,12 @@ def test_forward_inst_cnt_sums_match_pixel_lists():
     L, ws = st["L"], st["ws"]
     gx, gy = (W + 15) // 16, (H + 15) // 16
     T = gx * gy
-    wsv = raster.workspace_views(ws, L, 1, P, V, H, W, st["max_instances"])
+    wsv = raster.workspace_views(ws, L, 1, P, V, H, W, st["max_instances"], list_k=32)
     tile_start = wsv["tile_start"].cpu().numpy().astype(np.int64)
     last = wsv["n_contrib"][:, 0].cpu().numpy()                                   # [V, H, W]
-    flags = ws[L.tile_flag:L.tile_flag + 4 * V * T].view(torch.int32).cpu().numpy()
-    n_list = ws[L.n_list:L.n_list + 4 * V * H * W].view(torch.int32).cpu().numpy().reshape(V, H, W)
-    inst_cnt = ws[L.inst_cnt:L.inst_cnt + 4 * int(tile_start[-1])].view(torch.int32).cpu().numpy()
+    flags = wsv["tile_flag"].cpu().numpy()
+    n_list = wsv["n_list"].cpu().numpy()
+    inst_cnt = wsv["inst_cnt"].cpu().numpy()
     checked = 0
     for v in range(V):
         for ty in range(gy):
