@@ -17,11 +17,57 @@ _lib = None
 class GaRasterLayout(C.Structure):
     _fields_ = [(n, C.c_size_t) for n in (
         "total_bytes", "status", "rec", "depth", "rect", "tile_count", "tile_start",
-        "keys", "ids", "final_T", "n_contrib", "inst_off", "inst_cnt", "n_list", "tile_flag", "tile_rec_start", "lists")]
+        "keys", "ids", "final_T", "n_contrib", "inst_cnt", "n_list", "tile_flag", "lists")]
+
+
+class GaGemmEpilogue(C.Structure):
+    _fields_ = [("mode", C.c_int), ("bias", C.c_void_p), ("out", C.c_void_p), ("ld_out", C.c_int),
+                ("gate", C.c_void_p), ("gate_ld", C.c_int), ("rows_per_batch", C.c_int),
+                ("q", C.c_void_p), ("k", C.c_void_p), ("vt", C.c_void_p),
+                ("qn_w", C.c_void_p), ("kn_w", C.c_void_p), ("heads", C.c_int), ("first_part", C.c_int),
+                ("tok_pitch", C.c_int), ("eps", C.c_float)]
+
+
+vp, i32, i64, f32, sz = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_size_t
+_RASTER_IN = [vp, i32, i32, i32, vp, vp, vp, i32, i32, f32]   # gauss13, batch, P, views, viewmats, projmats, bg, H, W, scale
+
+# name: (restype, argtypes) of every function include/ga_b200.h declares, in its order
+# (tests/test_abi.py checks this table against the header)
+ABI = {
+    "ga_raster_layout_ex": (i32, [i32, i32, i32, i32, i32, i64, i32, C.POINTER(GaRasterLayout)]),
+    "ga_raster_forward_ex": (i32, _RASTER_IN + [vp, vp, vp, vp, sz, i64, i32, vp, vp, vp]),
+    "ga_raster_backward_scratch_bytes": (sz, [i32, i32, i32]),
+    "ga_raster_backward_ex": (i32, _RASTER_IN + [vp, vp, vp, vp, sz, i64, i32, vp, sz, vp, vp]),
+    "ga_render_post_forward": (i32, [vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp]),
+    "ga_render_post_backward": (i32, [vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "ga_raster_set_variant": (i32, [i32, i32]),
+    "ga_gemm_bf16_tn": (i32, [vp, i32, vp, i32, i32, i32, i32, C.POINTER(GaGemmEpilogue), i32, vp]),
+    "ga_attention_bf16": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, f32, vp]),
+    "ga_rmsnorm_modulate": (i32, [vp, vp, vp, vp, i32, i32, vp, i32, i32, f32, vp]),
+    "ga_linear_small": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
+    "ga_timestep_sinusoid": (i32, [vp, vp, i32, i32, vp]),
+    "ga_layernorm_rows": (i32, [vp, vp, vp, vp, i32, i32, f32, vp]),
+    "ga_add_tables": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
+    "ga_embed_fc1": (i32, [vp, i32, vp, i32, vp, vp, vp, i32, i32, vp]),
+    "ga_xyz_posenc": (i32, [vp, vp, i32, vp]),
+    "ga_final_layer": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp]),
+    "ga_cfg_combine": (i32, [vp, vp, i64, f32, vp]),
+    "ga_axpy": (i32, [vp, vp, f32, i64, vp]),
+    "ga_f32_to_bf16": (i32, [vp, vp, i64, vp]),
+    "ga_layernorm_modulate": (i32, [vp, vp, vp, vp, vp, i32, i32, vp, i32, i32, f32, vp]),
+    "ga_thin_linear": (i32, [vp, vp, vp, i32, vp, vp, vp, i32, i32, i32, f32, vp]),
+    "ga_micro_attention_bf16": (i32, [vp, vp, vp, vp, i32, i32, i32, f32, vp]),
+    "ga_micro_seq_build": (i32, [vp, i32, vp, vp, i64, i32, i32, vp]),
+    "ga_surfel_cascade_pack": (i32, [vp, i32, vp, vp, i32, i32, f32, f32, vp, vp, i64, vp]),
+    "ga_silu_to_bf16": (i32, [vp, vp, i64, vp]),
+    "ga_profile_enable": (i32, [i32]),
+    "ga_profile_read": (i32, [C.POINTER(f32), i32]),
+    "ga_b200_version": (C.c_char_p, []),
+}
 
 
 def lib():
-    """Returns the loaded library; raises loudly when it is not built."""
+    """Returns the loaded library with every function of ABI declared; raises loudly when it is not built."""
     global _lib
     if _lib is not None:
         return _lib
@@ -31,37 +77,13 @@ def lib():
             "`python -m gaussiananything_b200.build` (there is no CPU fallback)" % LIB_PATH)
     import torch  # noqa: F401  (loads libcudart / libcuda into the process first)
     L = C.CDLL(LIB_PATH)
-    vp, i32, i64, f32, sz = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_size_t
-    L.ga_raster_layout.argtypes = [i32, i32, i32, i32, i32, i64, C.POINTER(GaRasterLayout)]
-    L.ga_raster_layout.restype = i32
-    L.ga_raster_layout_ex.argtypes = [i32, i32, i32, i32, i32, i64, i32, C.POINTER(GaRasterLayout)]
-    L.ga_raster_layout_ex.restype = i32
-    L.ga_raster_forward_ex.argtypes = [vp, i32, i32, i32, vp, vp, vp, i32, i32, f32, vp, vp, vp, vp, sz, i64, i32, vp, vp, vp]
-    L.ga_raster_forward_ex.restype = i32
-    L.ga_raster_backward_ex.argtypes = [vp, i32, i32, i32, vp, vp, vp, i32, i32, f32, vp, vp, vp, vp, sz, i64, i32, vp, sz, vp, vp]
-    L.ga_raster_backward_ex.restype = i32
-    L.ga_raster_forward.argtypes = [vp, i32, i32, i32, vp, vp, vp, i32, i32, f32,
-                                    vp, vp, vp, vp, sz, i64, vp]
-    L.ga_raster_forward.restype = i32
-    for n in ("ga_raster_forward_bin", "ga_raster_forward_render"):
-        getattr(L, n).argtypes = L.ga_raster_forward.argtypes
-        getattr(L, n).restype = i32
-    L.ga_raster_forward_async.argtypes = L.ga_raster_forward.argtypes[:-1] + [vp, vp, vp]
-    L.ga_raster_forward_async.restype = i32
-    L.ga_raster_backward_scratch_bytes.argtypes = [i32, i32, i32]
-    L.ga_raster_backward_scratch_bytes.restype = sz
-    L.ga_raster_backward.argtypes = [vp, i32, i32, i32, vp, vp, vp, i32, i32, f32,
-                                     vp, vp, vp, vp, sz, i64, vp, sz, vp, vp]
-    L.ga_raster_backward.restype = i32
-    L.ga_render_post_forward.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp]
-    L.ga_render_post_forward.restype = i32
-    L.ga_render_post_backward.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]
-    L.ga_render_post_backward.restype = i32
-    L.ga_b200_version.restype = C.c_char_p
+    for name, (restype, argtypes) in ABI.items():
+        fn = getattr(L, name)
+        fn.restype, fn.argtypes = restype, argtypes
     _lib = L
     return L
 
 
 def check(rc, what):
     if rc != 0:
-        raise RuntimeError("%s failed with code %d" % (what, rc))
+        raise RuntimeError("libga_b200: %s failed with code %d" % (what, rc))

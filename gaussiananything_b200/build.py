@@ -35,7 +35,7 @@ def sources():
 
 
 def build(force: bool = False, verbose: bool = False, variant: str = "", extra_flags=()) -> str:
-    """variant != "": a tuning build libga_b200_<variant>.so with `extra_flags` (e.g. -DGA_LIST_STCS=1) in its own object
+    """variant != "": a tuning build libga_b200_<variant>.so with `extra_flags` (e.g. -DGA_TILE_REPLICAS=4) in its own object
     directory; load it with GA_B200_LIB=<path> (gaussiananything_b200/_lib.py).  The default build is the product."""
     nvcc = _nvcc()
     OUT = os.path.join(HERE, "libga_b200%s.so" % (("_" + variant) if variant else ""))

@@ -40,15 +40,8 @@ extern "C" int ga_raster_set_variant(int radius_formula, int quat_norm_grad)
     return 0;
 }
 
-extern "C" int ga_raster_get_variant(int *radius_formula, int *quat_norm_grad)
-{
-    if (!radius_formula || !quat_norm_grad) return GA_ERR_BADARG;
-    *radius_formula = g_radius_formula; *quat_norm_grad = g_quat_norm_grad;
-    return 0;
-}
-
 static int make_dims(int batch, int P, int views, int H, int W, float scale_modifier,
-                     int64_t max_instances, RasterDims *d, int list_k = 0)
+                     int64_t max_instances, RasterDims *d, int list_k)
 {
     if (list_k < 0 || list_k > 1024) return GA_ERR_BADARG;
     d->list_k = list_k;
@@ -65,12 +58,6 @@ static int make_dims(int batch, int P, int views, int H, int W, float scale_modi
     if ((int64_t)d->NV * P > 0x7fffffffLL || max_instances > 0xfffffff0LL) return GA_ERR_SIZE;
     if (d->NV > 65535) return GA_ERR_SIZE;
     return 0;
-}
-
-extern "C" int ga_raster_layout(int batch, int P, int views, int H, int W,
-                                int64_t max_instances, GaRasterLayout *L)
-{
-    return ga_raster_layout_ex(batch, P, views, H, W, max_instances, 0, L);
 }
 
 extern "C" int ga_raster_layout_ex(int batch, int P, int views, int H, int W,
@@ -93,11 +80,9 @@ extern "C" int ga_raster_layout_ex(int batch, int P, int views, int H, int W,
     L->ids = off;        off = align_up(off + mi * sizeof(uint32_t), 256);
     L->final_T = off;    off = align_up(off + (size_t)d.NV * 3 * HW * sizeof(float), 256);
     L->n_contrib = off;  off = align_up(off + (size_t)d.NV * 2 * HW * sizeof(int32_t), 256);
-    L->inst_off = off;                                                       // unused, 0 bytes
     L->inst_cnt = off;   off = align_up(off + mi * sizeof(uint32_t), 256);
     L->n_list = off;     off = align_up(off + (list_k ? (size_t)d.NV * HW * sizeof(int32_t) : 0), 256);
     L->tile_flag = off;  off = align_up(off + (list_k ? NVT * sizeof(uint32_t) : 0), 256);
-    L->tile_rec_start = off;                                                 // unused, 0 bytes
     L->lists = off;      off = align_up(off + (size_t)list_k * NVT * 256 * 16, 256);
     L->total_bytes = off;
     return 0;
@@ -123,13 +108,14 @@ static void carve(const GaRasterLayout &L, const RasterDims &d, void *base, Rast
     w->lists = (uint4 *)(p + L.lists);
 }
 
-static int raster_forward_impl(int stage, const float *gauss13, int batch, int P, int views,
-                               const float *viewmats, const float *projmats, const float *bg,
-                               int H, int W, float scale_modifier,
-                               float *out_color, float *out_allmap, int32_t *out_radii,
-                               void *workspace, size_t workspace_bytes, int64_t max_instances,
-                               void *stream, int32_t *status_host = nullptr, void *status_event = nullptr, int list_k = 0)
+extern "C" int ga_raster_forward_ex(const float *gauss13, int batch, int P, int views,
+                                    const float *viewmats, const float *projmats, const float *bg,
+                                    int H, int W, float scale_modifier,
+                                    float *out_color, float *out_allmap, int32_t *out_radii,
+                                    void *workspace, size_t workspace_bytes, int64_t max_instances, int list_k,
+                                    int32_t *status_host, void *status_event, void *stream)
 {
+    if ((status_host == nullptr) != (status_event == nullptr)) return GA_ERR_BADARG;
     RasterDims d;
     int rc = make_dims(batch, P, views, H, W, scale_modifier, max_instances, &d, list_k);
     if (rc) return rc;
@@ -142,80 +128,17 @@ static int raster_forward_impl(int stage, const float *gauss13, int batch, int P
     carve(L, d, workspace, &w);
     cudaStream_t s = (cudaStream_t)stream;
     cudaError_t e;
-    if (stage == 0 || stage == 1) {
-        if ((e = cudaMemsetAsync(w.status, 0, 16 * sizeof(int32_t), s)) != cudaSuccess) return (int)e;
-        if ((e = cudaMemsetAsync(w.tile_count, 0, (size_t)d.NV * d.T * GA_TILE_REPLICAS * sizeof(uint32_t), s)) != cudaSuccess) return (int)e;
-        prof(0, s);
-        if ((e = ga_launch_preprocess(d, w, gauss13, viewmats, projmats, out_radii, s)) != cudaSuccess) return (int)e;
-        prof(1, s);
-        if ((e = ga_launch_binning(d, w, s, status_host, (cudaEvent_t)status_event)) != cudaSuccess) return (int)e;
-        prof(2, s);
-    }
-    if (stage == 0 || stage == 2) {
-        if (list_k && (e = cudaMemsetAsync(w.tile_flag, 0, (size_t)d.NV * d.T * sizeof(uint32_t), s)) != cudaSuccess) return (int)e;
-        if ((e = ga_launch_render_fwd(d, w, bg, out_color, out_allmap, s)) != cudaSuccess) return (int)e;
-        prof(3, s);
-    }
+    if ((e = cudaMemsetAsync(w.status, 0, 16 * sizeof(int32_t), s)) != cudaSuccess) return (int)e;
+    if ((e = cudaMemsetAsync(w.tile_count, 0, (size_t)d.NV * d.T * GA_TILE_REPLICAS * sizeof(uint32_t), s)) != cudaSuccess) return (int)e;
+    prof(0, s);
+    if ((e = ga_launch_preprocess(d, w, gauss13, viewmats, projmats, out_radii, s)) != cudaSuccess) return (int)e;
+    prof(1, s);
+    if ((e = ga_launch_binning(d, w, s, status_host, (cudaEvent_t)status_event)) != cudaSuccess) return (int)e;
+    prof(2, s);
+    if (list_k && (e = cudaMemsetAsync(w.tile_flag, 0, (size_t)d.NV * d.T * sizeof(uint32_t), s)) != cudaSuccess) return (int)e;
+    if ((e = ga_launch_render_fwd(d, w, bg, out_color, out_allmap, s)) != cudaSuccess) return (int)e;
+    prof(3, s);
     return 0;
-}
-
-extern "C" int ga_raster_forward(const float *gauss13, int batch, int P, int views,
-                                 const float *viewmats, const float *projmats, const float *bg,
-                                 int H, int W, float scale_modifier,
-                                 float *out_color, float *out_allmap, int32_t *out_radii,
-                                 void *workspace, size_t workspace_bytes, int64_t max_instances,
-                                 void *stream)
-{
-    return raster_forward_impl(0, gauss13, batch, P, views, viewmats, projmats, bg, H, W, scale_modifier, out_color,
-                               out_allmap, out_radii, workspace, workspace_bytes, max_instances, stream);
-}
-
-extern "C" int ga_raster_forward_async(const float *gauss13, int batch, int P, int views,
-                                       const float *viewmats, const float *projmats, const float *bg,
-                                       int H, int W, float scale_modifier,
-                                       float *out_color, float *out_allmap, int32_t *out_radii,
-                                       void *workspace, size_t workspace_bytes, int64_t max_instances,
-                                       int32_t *status_host, void *status_event, void *stream)
-{
-    if (!status_host || !status_event) return GA_ERR_BADARG;
-    return raster_forward_impl(0, gauss13, batch, P, views, viewmats, projmats, bg, H, W, scale_modifier, out_color,
-                               out_allmap, out_radii, workspace, workspace_bytes, max_instances, stream, status_host,
-                               status_event);
-}
-
-extern "C" int ga_raster_forward_ex(const float *gauss13, int batch, int P, int views,
-                                    const float *viewmats, const float *projmats, const float *bg,
-                                    int H, int W, float scale_modifier,
-                                    float *out_color, float *out_allmap, int32_t *out_radii,
-                                    void *workspace, size_t workspace_bytes, int64_t max_instances, int list_k,
-                                    int32_t *status_host, void *status_event, void *stream)
-{
-    if ((status_host == nullptr) != (status_event == nullptr)) return GA_ERR_BADARG;
-    return raster_forward_impl(0, gauss13, batch, P, views, viewmats, projmats, bg, H, W, scale_modifier, out_color,
-                               out_allmap, out_radii, workspace, workspace_bytes, max_instances, stream, status_host,
-                               status_event, list_k);
-}
-
-extern "C" int ga_raster_forward_bin(const float *gauss13, int batch, int P, int views,
-                                     const float *viewmats, const float *projmats, const float *bg,
-                                     int H, int W, float scale_modifier,
-                                     float *out_color, float *out_allmap, int32_t *out_radii,
-                                     void *workspace, size_t workspace_bytes, int64_t max_instances,
-                                     void *stream)
-{
-    return raster_forward_impl(1, gauss13, batch, P, views, viewmats, projmats, bg, H, W, scale_modifier, out_color,
-                               out_allmap, out_radii, workspace, workspace_bytes, max_instances, stream);
-}
-
-extern "C" int ga_raster_forward_render(const float *gauss13, int batch, int P, int views,
-                                        const float *viewmats, const float *projmats, const float *bg,
-                                        int H, int W, float scale_modifier,
-                                        float *out_color, float *out_allmap, int32_t *out_radii,
-                                        void *workspace, size_t workspace_bytes, int64_t max_instances,
-                                        void *stream)
-{
-    return raster_forward_impl(2, gauss13, batch, P, views, viewmats, projmats, bg, H, W, scale_modifier, out_color,
-                               out_allmap, out_radii, workspace, workspace_bytes, max_instances, stream);
 }
 
 // Backward scratch = gradient accumulators [NV*P][18]; the per-(pixel, surfel) records stay in shared memory
@@ -225,20 +148,6 @@ extern "C" size_t ga_raster_backward_scratch_bytes(int batch, int P, int views)
 {
     if (batch <= 0 || P <= 0 || views <= 0) return 0;
     return bwd_acc_bytes(batch, P, views);
-}
-
-extern "C" int ga_raster_backward(const float *gauss13, int batch, int P, int views,
-                                  const float *viewmats, const float *projmats, const float *bg,
-                                  int H, int W, float scale_modifier,
-                                  const int32_t *radii,
-                                  const float *dL_dcolor, const float *dL_dallmap,
-                                  const void *workspace, size_t workspace_bytes, int64_t max_instances,
-                                  void *scratch, size_t scratch_bytes,
-                                  float *grad_gauss13, void *stream)
-{
-    return ga_raster_backward_ex(gauss13, batch, P, views, viewmats, projmats, bg, H, W, scale_modifier, radii, dL_dcolor,
-                                 dL_dallmap, workspace, workspace_bytes, max_instances, 0, scratch, scratch_bytes,
-                                 grad_gauss13, stream);
 }
 
 extern "C" int ga_raster_backward_ex(const float *gauss13, int batch, int P, int views,
@@ -276,4 +185,4 @@ extern "C" int ga_raster_backward_ex(const float *gauss13, int batch, int P, int
     return 0;
 }
 
-extern "C" const char *ga_b200_version(void) { return "ga_b200 0.1 (sm_90a)"; }
+extern "C" const char *ga_b200_version(void) { return "ga_b200 0.2 (sm_90a)"; }

@@ -26,9 +26,9 @@ struct RasterDims {
     int H, W, gx, gy, T;       // T = gx*gy tiles per image
     float scale_modifier;
     int64_t max_instances;
+    int list_k;                // > 0: the forward records every pixel's contributions (<= list_k per pixel), see RasterWs.lists
     // the two unpinned judgement calls of the restatement (oracle/surfel_oracle.c), switchable so that pinning against
     // upstream is a flip of the defaults below; ga_raster_set_variant() overrides them at run time (tests)
-    int list_k;                // > 0: the forward records every pixel's contributions (<= list_k per pixel), see RasterWs.lists
     int radius_formula;        // 0: ceil(max(ex, ey, 3*FilterSize))   1: ceil(3*max(ex, ey, FilterSize))
     int quat_norm_grad;        // 0: quaternion vjp not chained through q/|q| (upstream)   1: chained
 };
@@ -66,9 +66,9 @@ struct RasterWs {
 cudaError_t ga_launch_preprocess(const RasterDims &d, const RasterWs &w, const float *gauss13,
                                  const float *viewmats, const float *projmats,
                                  int32_t *out_radii, cudaStream_t s);
-// status_host / status_event (both optional): after the tile scan -- the first point where the instance count and
-// the overflow flag are known -- status[0..3] is copied to pinned host memory and the event recorded, so the host
-// can look at them while the scatter / sort / composite kernels are still running.
+// status_host / status_event (both NULL, or both set): after the tile scan -- the first point where the instance
+// count and the overflow flag are known -- status[0..3] is copied to pinned host memory and the event recorded, so
+// the host can look at them while the scatter / sort / composite kernels are still running.
 // Tile counters / scatter cursors are kept in GA_TILE_REPLICAS copies per tile (replica = warp index mod R): the
 // 1.05M atomics of the C2 scene otherwise queue up on 6144 addresses, ~170 deep, and L2 serialises same-address
 // atomics (scatter: 48 us for 1M atomics).  The scan sums the replicas of a tile and hands every replica its own
@@ -77,13 +77,10 @@ cudaError_t ga_launch_preprocess(const RasterDims &d, const RasterWs &w, const f
 #define GA_TILE_REPLICAS 8
 #endif
 
-cudaError_t ga_launch_binning(const RasterDims &d, const RasterWs &w, cudaStream_t s, int32_t *status_host = nullptr,
-                              cudaEvent_t status_event = nullptr);
+cudaError_t ga_launch_binning(const RasterDims &d, const RasterWs &w, cudaStream_t s, int32_t *status_host,
+                              cudaEvent_t status_event);
 cudaError_t ga_launch_render_fwd(const RasterDims &d, const RasterWs &w, const float *bg,
                                  float *out_color, float *out_allmap, cudaStream_t s);
-#ifndef GA_LIST_K
-#define GA_LIST_K 32               /* default per-pixel list capacity callers pass as list_k */
-#endif
 cudaError_t ga_launch_render_bwd(const RasterDims &d, const RasterWs &w, const float *bg,
                                  const float *dL_dcolor, const float *dL_dallmap,
                                  float *grad_acc, cudaStream_t s);

@@ -16,9 +16,6 @@
 #include "device_once.cuh"
 
 #define CHUNK 256
-#ifndef GA_LIST_STCS
-#define GA_LIST_STCS 0
-#endif
 
 // single-instruction approximations (MUFU.RCP / MUFU.EX2, <= 2 ulp): the IEEE division and the range-checked
 // __expf cost ~10 instructions each in the inner loop; parity with the oracle stays ~1e-6 relative.
@@ -267,15 +264,9 @@ render_fwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
                     last_contributor = contributor;
                     if (LISTS) {
                         atomicAdd(&sm.cnt[jj], 1);
-                        if (nl < d.list_k) {
-                            const uint4 ent = make_uint4((uint32_t)(contributor - 1), __float_as_uint(alpha),
-                                                         __float_as_uint(depth), 0u);
-#if GA_LIST_STCS
-                            __stcs(my_list + (size_t)nl * 256, ent);       // written once, read once by the backward
-#else
-                            my_list[(size_t)nl * 256] = ent;
-#endif
-                        }
+                        if (nl < d.list_k)
+                            my_list[(size_t)nl * 256] = make_uint4((uint32_t)(contributor - 1), __float_as_uint(alpha),
+                                                                   __float_as_uint(depth), 0u);
                         nl++;
                     }
                 }
@@ -309,12 +300,6 @@ render_fwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
         oa[pix + 5 * HW] = median_depth;
         oa[pix + 6 * HW] = dist;
     }
-}
-
-// Kept for ABI compatibility: the forward no longer has a lane-group mapping to select (see include/ga_b200.h).
-extern "C" int ga_raster_set_tuning(int fwd_group)
-{
-    return (fwd_group == 32 || fwd_group == 16 || fwd_group == 8) ? 0 : -1;
 }
 
 cudaError_t ga_launch_render_fwd(const RasterDims &d, const RasterWs &w, const float *bg,

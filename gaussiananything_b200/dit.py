@@ -23,54 +23,15 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from ._lib import GaGemmEpilogue
 
 
 def _p(t):
     return C.c_void_p(t.data_ptr() if t is not None else 0)
 
 
-class GaGemmEpilogue(C.Structure):
-    _fields_ = [("mode", C.c_int), ("bias", C.c_void_p), ("out", C.c_void_p), ("ld_out", C.c_int),
-                ("gate", C.c_void_p), ("gate_ld", C.c_int), ("rows_per_batch", C.c_int),
-                ("q", C.c_void_p), ("k", C.c_void_p), ("vt", C.c_void_p),
-                ("qn_w", C.c_void_p), ("kn_w", C.c_void_p), ("heads", C.c_int), ("first_part", C.c_int),
-                ("tok_pitch", C.c_int), ("eps", C.c_float)]
-
-
 EPI_BF16, EPI_GELU_BF16, EPI_F32, EPI_RESID_GATE_F32, EPI_HEADS = 0, 1, 2, 3, 4
-_bound = False
-
-
-def _bind():
-    global _bound
-    L = _lib.lib()
-    if _bound:
-        return L
-    vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_int64, C.c_float
-    L.ga_gemm_bf16_tn.argtypes = [vp, i32, vp, i32, i32, i32, i32, C.POINTER(GaGemmEpilogue), i32, vp]
-    L.ga_attention_bf16.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, f32, vp]
-    L.ga_rmsnorm_modulate.argtypes = [vp, vp, vp, vp, i32, i32, vp, i32, i32, f32, vp]
-    L.ga_linear_small.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
-    L.ga_timestep_sinusoid.argtypes = [vp, vp, i32, i32, vp]
-    L.ga_layernorm_rows.argtypes = [vp, vp, vp, vp, i32, i32, f32, vp]
-    L.ga_add_tables.argtypes = [vp, vp, vp, i32, i32, i32, i32, vp]
-    L.ga_embed_fc1.argtypes = [vp, i32, vp, i32, vp, vp, vp, i32, i32, vp]
-    L.ga_xyz_posenc.argtypes = [vp, vp, i32, vp]
-    L.ga_final_layer.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp]
-    L.ga_cfg_combine.argtypes = [vp, vp, i64, f32, vp]
-    L.ga_axpy.argtypes = [vp, vp, f32, i64, vp]
-    L.ga_f32_to_bf16.argtypes = [vp, vp, i64, vp]
-    for n in ("ga_gemm_bf16_tn", "ga_attention_bf16", "ga_rmsnorm_modulate", "ga_linear_small",
-              "ga_timestep_sinusoid", "ga_layernorm_rows", "ga_add_tables", "ga_embed_fc1", "ga_xyz_posenc",
-              "ga_final_layer", "ga_cfg_combine", "ga_axpy", "ga_f32_to_bf16"):
-        getattr(L, n).restype = i32
-    _bound = True
-    return L
-
-
-def _ck(rc, what):
-    if rc != 0:
-        raise RuntimeError("libga_b200: %s failed with code %d" % (what, rc))
+_bind = _lib.lib
 
 
 _GEMM_CFG_ENV = None
@@ -440,7 +401,7 @@ class _DiTEngine:
     def _gemm(self, A, W, M, N, K, epi, st, bn=None):
         if bn is None:
             bn = _gemm_config(M, N, epi.mode)
-        _ck(self.L.ga_gemm_bf16_tn(_p(A), K, _p(W), K, M, N, K, C.byref(epi), bn, st), "ga_gemm_bf16_tn")
+        _lib.check(self.L.ga_gemm_bf16_tn(_p(A), K, _p(W), K, M, N, K, C.byref(epi), bn, st), "ga_gemm_bf16_tn")
 
     def _epi(self, mode, **kw):
         e = GaGemmEpilogue()
@@ -464,21 +425,21 @@ class _DiTEngine:
         B, N, M = self._shape
         D, H, R = self.D, self.H, B * N
         # ---- prologue: timestep + pooled vector -> adaLN tables
-        _ck(L.ga_timestep_sinusoid(_p(s["t_in"]), _p(s["sinus"]), B, 256, st), "sinusoid")
-        _ck(L.ga_linear_small(_p(s["sinus"]), _p(w["t0_w"]), _p(w["t0_b"]), _p(s["h1"]), B, D, 256, 0, 1, 0, st), "t0")
-        _ck(L.ga_linear_small(_p(s["h1"]), _p(w["t2_w"]), _p(w["t2_b"]), _p(s["temb"]), B, D, D, 0, 0, 0, st), "t2")
-        _ck(L.ga_layernorm_rows(_p(s["vec_in"]), _p(w["pv_ln_w"]), _p(w["pv_ln_b"]), _p(s["vln"]), B, self.Dc, 1e-5, st), "ln")
-        _ck(L.ga_linear_small(_p(s["vln"]), _p(w["pv_w"]), _p(w["pv_b"]), _p(s["temb"]), B, D, self.Dc, 0, 0, 1, st), "pv")
-        _ck(L.ga_linear_small(_p(s["temb"]), _p(w["ada_w"]), _p(w["ada_b"]), _p(s["t0"]), B, 6 * D, D, 1, 0, 0, st), "ada")
-        _ck(L.ga_add_tables(_p(w["tables"]), _p(s["t0"]), _p(s["mod"]), self.depth, B, 6 * D, 6 * D, st), "tables")
-        _ck(L.ga_add_tables(_p(w["table_f"]), _p(s["temb"]), _p(s["modf"]), 1, B, 2 * D, D, st), "table_f")
+        _lib.check(L.ga_timestep_sinusoid(_p(s["t_in"]), _p(s["sinus"]), B, 256, st), "sinusoid")
+        _lib.check(L.ga_linear_small(_p(s["sinus"]), _p(w["t0_w"]), _p(w["t0_b"]), _p(s["h1"]), B, D, 256, 0, 1, 0, st), "t0")
+        _lib.check(L.ga_linear_small(_p(s["h1"]), _p(w["t2_w"]), _p(w["t2_b"]), _p(s["temb"]), B, D, D, 0, 0, 0, st), "t2")
+        _lib.check(L.ga_layernorm_rows(_p(s["vec_in"]), _p(w["pv_ln_w"]), _p(w["pv_ln_b"]), _p(s["vln"]), B, self.Dc, 1e-5, st), "ln")
+        _lib.check(L.ga_linear_small(_p(s["vln"]), _p(w["pv_w"]), _p(w["pv_b"]), _p(s["temb"]), B, D, self.Dc, 0, 0, 1, st), "pv")
+        _lib.check(L.ga_linear_small(_p(s["temb"]), _p(w["ada_w"]), _p(w["ada_b"]), _p(s["t0"]), B, 6 * D, D, 1, 0, 0, st), "ada")
+        _lib.check(L.ga_add_tables(_p(w["tables"]), _p(s["t0"]), _p(s["mod"]), self.depth, B, 6 * D, 6 * D, st), "tables")
+        _lib.check(L.ga_add_tables(_p(w["table_f"]), _p(s["temb"]), _p(s["modf"]), 1, B, 2 * D, D, st), "table_f")
         # ---- token embedder
         concat = self.stage2 and not self.use_pe
-        _ck(L.ga_embed_fc1(_p(s["x_in"]), self.Cin, _p(s["xyz_in"]) if concat else None, 3 if concat else 0,
-                           _p(w["fc1_w"]), _p(w["fc1_b"]), _p(s["e1"]), R, D, st), "embed_fc1")
+        _lib.check(L.ga_embed_fc1(_p(s["x_in"]), self.Cin, _p(s["xyz_in"]) if concat else None, 3 if concat else 0,
+                                  _p(w["fc1_w"]), _p(w["fc1_b"]), _p(s["e1"]), R, D, st), "embed_fc1")
         self._gemm(s["e1"], w["fc2_w"], R, D, D, self._epi(EPI_F32, bias=w["fc2_b"], out=s["xres"], ld_out=D), st)
         if self.use_pe:
-            _ck(L.ga_xyz_posenc(_p(s["xyz_in"]), _p(s["pe"]), R, st), "xyz_pe")
+            _lib.check(L.ga_xyz_posenc(_p(s["xyz_in"]), _p(s["pe"]), R, st), "xyz_pe")
             self._gemm(s["pe"], w["xyz_w"], R, D, 64,
                        self._epi(EPI_RESID_GATE_F32, bias=w["xyz_b"], out=s["xres"], ld_out=D, rows_per_batch=N), st)
         # ---- blocks
@@ -487,28 +448,28 @@ class _DiTEngine:
             mod = s["mod"][l]                       # [B, 6D]
             ch = lambda j: mod[:, j * D:(j + 1) * D]
             # cross attention (pre-norm, residual)
-            _ck(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["pre_w"]), None, None, 0, N, _p(s["h"]), R, D, 1e-5, st), "prenorm")
+            _lib.check(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["pre_w"]), None, None, 0, N, _p(s["h"]), R, D, 1e-5, st), "prenorm")
             self._gemm(s["h"], wb["caq_w"], R, D, D,
                        self._epi(EPI_HEADS, q=s["q"], qn_w=wb["caq_n"], heads=H, first_part=0, tok_pitch=self.Np,
                                  rows_per_batch=N), st)
-            _ck(L.ga_attention_bf16(_p(s["q"]), _p(s["kc"][l]), _p(s["vtc"][l]), _p(s["ao"]), B, H, N, M, self.Np,
-                                    self.Mp, scale, wb["ca_bound"], st), "cross attention")
+            _lib.check(L.ga_attention_bf16(_p(s["q"]), _p(s["kc"][l]), _p(s["vtc"][l]), _p(s["ao"]), B, H, N, M, self.Np,
+                                           self.Mp, scale, wb["ca_bound"], st), "cross attention")
             self._gemm(s["ao"], wb["cao_w"], R, D, D,
                        self._epi(EPI_RESID_GATE_F32, bias=wb["cao_b"], out=s["xres"], ld_out=D, rows_per_batch=N), st)
             # gated self attention
-            _ck(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["n1_w"]), _p(ch(0)), _p(ch(1)), 6 * D, N, _p(s["h"]), R, D,
-                                      1e-5, st), "norm1")
+            _lib.check(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["n1_w"]), _p(ch(0)), _p(ch(1)), 6 * D, N, _p(s["h"]), R, D,
+                                             1e-5, st), "norm1")
             self._gemm(s["h"], wb["qkv_w"], R, 3 * D, D,
                        self._epi(EPI_HEADS, bias=wb["qkv_b"], q=s["q"], k=s["k"], vt=s["vt"], qn_w=wb["q_n"],
                                  kn_w=wb["k_n"], heads=H, first_part=0, tok_pitch=self.Np, rows_per_batch=N), st)
-            _ck(L.ga_attention_bf16(_p(s["q"]), _p(s["k"]), _p(s["vt"]), _p(s["ao"]), B, H, N, N, self.Np, self.Np,
-                                    scale, wb["sa_bound"], st), "self attention")
+            _lib.check(L.ga_attention_bf16(_p(s["q"]), _p(s["k"]), _p(s["vt"]), _p(s["ao"]), B, H, N, N, self.Np, self.Np,
+                                           scale, wb["sa_bound"], st), "self attention")
             self._gemm(s["ao"], wb["proj_w"], R, D, D,
                        self._epi(EPI_RESID_GATE_F32, bias=wb["proj_b"], out=s["xres"], ld_out=D, gate=ch(2),
                                  gate_ld=6 * D, rows_per_batch=N), st)
             # gated FFN
-            _ck(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["n2_w"]), _p(ch(3)), _p(ch(4)), 6 * D, N, _p(s["h"]), R, D,
-                                      1e-5, st), "norm2")
+            _lib.check(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["n2_w"]), _p(ch(3)), _p(ch(4)), 6 * D, N, _p(s["h"]), R, D,
+                                             1e-5, st), "norm2")
             self._gemm(s["h"], wb["w1"], R, 4 * D, D,
                        self._epi(EPI_GELU_BF16, bias=wb["b1"], out=s["hid"], ld_out=4 * D), st)
             self._gemm(s["hid"], wb["w2"], R, D, 4 * D,
@@ -517,10 +478,10 @@ class _DiTEngine:
             if self.tap_blocks:
                 s["taps"][l].copy_(s["xres"])
         # ---- final layer (+ CFG combine)
-        _ck(L.ga_final_layer(_p(s["xres"]), _p(s["modf"]), _p(w["fin_w"]), _p(w["fin_b"]), _p(s["y"]), R, D,
-                             self.Cout, N, 1e-6, st), "final layer")
+        _lib.check(L.ga_final_layer(_p(s["xres"]), _p(s["modf"]), _p(w["fin_w"]), _p(w["fin_b"]), _p(s["y"]), R, D,
+                                    self.Cout, N, 1e-6, st), "final layer")
         if cfg_scale is not None:
-            _ck(L.ga_cfg_combine(_p(s["y"]), _p(s["y_cfg"]), (B // 2) * N * self.Cout, cfg_scale, st), "cfg")
+            _lib.check(L.ga_cfg_combine(_p(s["y"]), _p(s["y_cfg"]), (B // 2) * N * self.Cout, cfg_scale, st), "cfg")
 
     @staticmethod
     def _version(t):
@@ -590,7 +551,7 @@ class _DiTEngine:
             s["xyz_in"].copy_(context["fps-xyz"].reshape(B, N, 3).to(torch.float32))
         if not self._context_is_cached(ctx_tok):
             c32 = ctx_tok.reshape(B * M, self.Dc).to(torch.float32).contiguous()
-            _ck(self.L.ga_f32_to_bf16(_p(c32), _p(s["ctx"]), c32.numel(), st), "ctx->bf16")
+            _lib.check(self.L.ga_f32_to_bf16(_p(c32), _p(s["ctx"]), c32.numel(), st), "ctx->bf16")
             self._context_kv(st)
             self._ctx_ref, self._ctx_ver = ctx_tok, self._version(ctx_tok)
         gkey = (cfg_scale, self.tap_blocks)

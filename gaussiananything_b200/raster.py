@@ -74,7 +74,7 @@ _status_slots = {}
 
 
 def _status_slot(dev):
-    """Pinned 4-int buffer + event for the overlapped status read-back of ga_raster_forward_async."""
+    """Pinned 4-int buffer + event for the overlapped status read-back of ga_raster_forward_ex."""
     # one slot per (device, stream): calls on different streams may overlap on the host
     key = (dev.index if dev.index is not None else torch.cuda.current_device(),
            torch.cuda.current_stream(dev).cuda_stream)
@@ -171,7 +171,7 @@ def backward_raw(state, grad_color, grad_allmap):
                                     _ptr(scratch), nbytes, _ptr(grad), _stream(dev))
     if len(_scratch_pool[pool_key]) < 2:
         _scratch_pool[pool_key].append(scratch)          # reused by later calls on the same stream: stream-ordered, safe
-    _lib.check(rc, "ga_raster_backward")
+    _lib.check(rc, "ga_raster_backward_ex")
     return grad
 
 

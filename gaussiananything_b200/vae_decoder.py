@@ -16,29 +16,10 @@ import os
 
 import torch
 
+from . import _lib
 from . import dit as _dit
-from .dit import EPI_BF16, EPI_F32, EPI_GELU_BF16, EPI_HEADS, EPI_RESID_GATE_F32, GaGemmEpilogue, _ck, _p, _round_up
-
-_bound = False
-
-
-def _bind():
-    global _bound
-    L = _dit._bind()
-    if _bound:
-        return L
-    vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_int64, C.c_float
-    L.ga_layernorm_modulate.argtypes = [vp, vp, vp, vp, vp, i32, i32, vp, i32, i32, f32, vp]
-    L.ga_thin_linear.argtypes = [vp, vp, vp, i32, vp, vp, vp, i32, i32, i32, f32, vp]
-    L.ga_micro_attention_bf16.argtypes = [vp, vp, vp, vp, i32, i32, i32, f32, vp]
-    L.ga_micro_seq_build.argtypes = [vp, i32, vp, vp, i64, i32, i32, vp]
-    L.ga_surfel_cascade_pack.argtypes = [vp, i32, vp, vp, i32, i32, f32, f32, vp, vp, i64, vp]
-    L.ga_silu_to_bf16.argtypes = [vp, vp, i64, vp]
-    for n in ("ga_layernorm_modulate", "ga_thin_linear", "ga_micro_attention_bf16", "ga_micro_seq_build",
-              "ga_surfel_cascade_pack", "ga_silu_to_bf16"):
-        getattr(L, n).restype = i32
-    _bound = True
-    return L
+from ._lib import GaGemmEpilogue
+from .dit import EPI_BF16, EPI_F32, EPI_GELU_BF16, EPI_HEADS, EPI_RESID_GATE_F32, _p, _round_up
 
 
 class SurfelDecoder:
@@ -46,7 +27,7 @@ class SurfelDecoder:
     MAX_GRAPHS = 4                 # captured batch sizes kept at a time (oldest dropped first)
 
     def __init__(self, state_dict, num_heads, depth, scene_max=0.45, skip_weight=0.1, device="cuda:0"):
-        self.L = _bind()
+        self.L = _lib.lib()
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise RuntimeError("gaussiananything_b200 needs a CUDA device (no CPU fallback)")
@@ -110,8 +91,8 @@ class SurfelDecoder:
 
     # ---- launch helpers
     def _gemm(self, A, W, M, N, K, epi, st):
-        _ck(self.L.ga_gemm_bf16_tn(_p(A), K, _p(W), K, M, N, K, C.byref(epi), _dit._gemm_config(M, N, epi.mode), st),
-            "ga_gemm_bf16_tn")
+        _lib.check(self.L.ga_gemm_bf16_tn(_p(A), K, _p(W), K, M, N, K, C.byref(epi), _dit._gemm_config(M, N, epi.mode), st),
+                   "ga_gemm_bf16_tn")
 
     @staticmethod
     def _epi(mode, **kw):
@@ -179,12 +160,12 @@ class SurfelDecoder:
         xyz = query_pcd_xyz.reshape(R, 3).contiguous().float()
         # ---- post_quant_conv
         h0 = z(R, self.pq_k, dt=bf)
-        _ck(L.ga_embed_fc1(_p(lat), zc, None, 0, _p(w["pq_w1"]), _p(w["pq_b1"]), _p(h0), R, self.pq_k, st), "post_quant fc1")
+        _lib.check(L.ga_embed_fc1(_p(lat), zc, None, 0, _p(w["pq_w1"]), _p(w["pq_b1"]), _p(h0), R, self.pq_k, st), "post_quant fc1")
         c = z(R, D)
         self._gemm(h0, w["pq_w2"], R, D, self.pq_k, self._epi(EPI_F32, bias=w["pq_b2"], out=c, ld_out=D), st)
         # ---- DiT2: per-token adaLN tables of every block in one GEMM on silu(c)
         cs = z(R, D, dt=bf)
-        _ck(L.ga_silu_to_bf16(_p(c), _p(cs), R * D, st), "silu")
+        _lib.check(L.ga_silu_to_bf16(_p(c), _p(cs), R * D, st), "silu")
         MW = dep * 6 * D
         mod = z(R, MW)
         self._gemm(cs, w["ada_w"], R, MW, D, self._epi(EPI_F32, bias=w["ada_b"], out=mod, ld_out=MW), st)
@@ -196,25 +177,25 @@ class SurfelDecoder:
         vtb = torch.zeros(B * H, 64, Np, device=dev, dtype=bf)
         for l, wb in enumerate(self.blocks):
             ch = lambda j: mod[:, (l * 6 + j) * D:(l * 6 + j + 1) * D]
-            _ck(L.ga_layernorm_modulate(_p(x), None, None, _p(ch(0)), _p(ch(1)), MW, 1, _p(h), R, D, 1e-6, st), "norm1")
+            _lib.check(L.ga_layernorm_modulate(_p(x), None, None, _p(ch(0)), _p(ch(1)), MW, 1, _p(h), R, D, 1e-6, st), "norm1")
             self._gemm(h, wb["qkv_w"], R, 3 * D, D,
                        self._epi(EPI_HEADS, bias=wb["qkv_b"], q=qb, k=kb, vt=vtb, qn_w=wb["q_n"], kn_w=wb["k_n"], heads=H,
                                  first_part=0, tok_pitch=Np, rows_per_batch=N), st)
-            _ck(L.ga_attention_bf16(_p(qb), _p(kb), _p(vtb), _p(ao), B, H, N, N, Np, Np, 0.125, wb["bound"], st), "attention")
+            _lib.check(L.ga_attention_bf16(_p(qb), _p(kb), _p(vtb), _p(ao), B, H, N, N, Np, Np, 0.125, wb["bound"], st), "attention")
             self._gemm(ao, wb["proj_w"], R, D, D,
                        self._epi(EPI_RESID_GATE_F32, bias=wb["proj_b"], out=x, ld_out=D, gate=ch(2), gate_ld=MW,
                                  rows_per_batch=1), st)
-            _ck(L.ga_layernorm_modulate(_p(x), None, None, _p(ch(3)), _p(ch(4)), MW, 1, _p(h), R, D, 1e-6, st), "norm2")
+            _lib.check(L.ga_layernorm_modulate(_p(x), None, None, _p(ch(3)), _p(ch(4)), MW, 1, _p(h), R, D, 1e-6, st), "norm2")
             self._gemm(h, wb["w1"], R, 4 * D, D, self._epi(EPI_GELU_BF16, bias=wb["b1"], out=hid, ld_out=4 * D), st)
             self._gemm(hid, wb["w2"], R, D, 4 * D,
                        self._epi(EPI_RESID_GATE_F32, bias=wb["b2"], out=x, ld_out=D, gate=ch(5), gate_ld=MW,
                                  rows_per_batch=1), st)
         # ---- base surfels
         base_pre = z(R, 13)
-        _ck(L.ga_thin_linear(_p(x), None, None, 1, _p(w["sr_w"]), _p(w["sr_b"]), _p(base_pre), R, D, 13, 0.0, st), "conv_sr")
+        _lib.check(L.ga_thin_linear(_p(x), None, None, 1, _p(w["sr_w"]), _p(w["sr_b"]), _p(base_pre), R, D, 13, 0.0, st), "conv_sr")
         base = z(R, 13)
-        _ck(L.ga_surfel_cascade_pack(_p(base_pre), 0, None, _p(xyz), 3, 1, self.scene_max * 0.5 * self.skip,
-                                     self.scale_factor, _p(base), None, R, st), "base pack")
+        _lib.check(L.ga_surfel_cascade_pack(_p(base_pre), 0, None, _p(xyz), 3, 1, self.scene_max * 0.5 * self.skip,
+                                            self.scale_factor, _p(base), None, R, st), "base pack")
         out = {"latent_from_vit": x.view(B, N, D), "gaussian_base_pre_activate": base_pre.view(B, N, 13),
                "gaussians_base": base.view(B, N, 13)}
         # ---- cascaded up-samplers
@@ -224,25 +205,25 @@ class SurfelDecoder:
             Lq = 1 + f
             Ms = S * Lq
             seq = z(Ms, D)
-            _ck(L.ga_micro_seq_build(_p(parents), prev_f, _p(stg["queries"]), _p(seq), S, f, D, st), "seq build")
+            _lib.check(L.ga_micro_seq_build(_p(parents), prev_f, _p(stg["queries"]), _p(seq), S, f, D, st), "seq build")
             hs, qkv, aos, hids = z(Ms, D, dt=bf), z(Ms, 3 * D, dt=bf), z(Ms, D, dt=bf), z(Ms, 4 * D, dt=bf)
             for lw in stg["layers"]:
-                _ck(L.ga_layernorm_modulate(_p(seq), _p(lw["n1_w"]), _p(lw["n1_b"]), None, None, 0, 1, _p(hs), Ms, D, 1e-5, st), "sr norm1")
+                _lib.check(L.ga_layernorm_modulate(_p(seq), _p(lw["n1_w"]), _p(lw["n1_b"]), None, None, 0, 1, _p(hs), Ms, D, 1e-5, st), "sr norm1")
                 self._gemm(hs, lw["qkv_w"], Ms, 3 * D, D, self._epi(EPI_BF16, bias=lw["qkv_b"], out=qkv, ld_out=3 * D), st)
-                _ck(L.ga_micro_attention_bf16(_p(qkv), _p(lw["q_n"]), _p(lw["k_n"]), _p(aos), S, Lq, H, 1e-5, st), "micro attention")
+                _lib.check(L.ga_micro_attention_bf16(_p(qkv), _p(lw["q_n"]), _p(lw["k_n"]), _p(aos), S, Lq, H, 1e-5, st), "micro attention")
                 self._gemm(aos, lw["proj_w"], Ms, D, D,
                            self._epi(EPI_RESID_GATE_F32, bias=lw["proj_b"], out=seq, ld_out=D, rows_per_batch=1), st)
-                _ck(L.ga_layernorm_modulate(_p(seq), _p(lw["n2_w"]), _p(lw["n2_b"]), None, None, 0, 1, _p(hs), Ms, D, 1e-5, st), "sr norm2")
+                _lib.check(L.ga_layernorm_modulate(_p(seq), _p(lw["n2_w"]), _p(lw["n2_b"]), None, None, 0, 1, _p(hs), Ms, D, 1e-5, st), "sr norm2")
                 self._gemm(hs, lw["w1"], Ms, 4 * D, D, self._epi(EPI_GELU_BF16, bias=lw["b1"], out=hids, ld_out=4 * D), st)
                 self._gemm(hids, lw["w2"], Ms, D, 4 * D,
                            self._epi(EPI_RESID_GATE_F32, bias=lw["b2"], out=seq, ld_out=D, rows_per_batch=1), st)
             res = z(Ms, 13)
-            _ck(L.ga_thin_linear(_p(seq), _p(stg["hn_w"]), _p(stg["hn_b"]), 0, _p(stg["h_w"]), _p(stg["h_b"]), _p(res), Ms, D, 13,
-                                 1e-5, st), "residual head")
+            _lib.check(L.ga_thin_linear(_p(seq), _p(stg["hn_w"]), _p(stg["hn_b"]), 0, _p(stg["h_w"]), _p(stg["h_b"]), _p(res), Ms, D, 13,
+                                        1e-5, st), "residual head")
             Rc = S * f
             g, pre = z(Rc, 13), z(Rc, 13)
-            _ck(L.ga_surfel_cascade_pack(_p(res), 1, _p(parent_pre), _p(parent_g), 13, f, self.scene_max * 0.5,
-                                         self.scale_factor, _p(g), _p(pre), Rc, st), "cascade pack")
+            _lib.check(L.ga_surfel_cascade_pack(_p(res), 1, _p(parent_pre), _p(parent_g), 13, f, self.scene_max * 0.5,
+                                                self.scale_factor, _p(g), _p(pre), Rc, st), "cascade pack")
             out["gaussians_upsampled" + ("" if si == 0 else "_%d" % (si + 1))] = g.view(B, Rc // B, 13)
             parents, prev_f, parent_g, parent_pre, S = seq, f, g, pre, Rc
         return out

@@ -48,22 +48,17 @@ typedef struct GaRasterLayout {
     size_t ids;         /* uint32[max_instances]  sorted surfel index per instance */
     size_t final_T;     /* float[NV][3][H*W]  T, M1, M2 */
     size_t n_contrib;   /* int32[NV][2][H*W]  last contributor, median contributor */
-    size_t inst_off;    /* unused (0 bytes) */
     size_t inst_cnt;    /* uint32[max_instances]  (list_k > 0) contributions of every instance, counted by the forward */
     size_t n_list;      /* int32[NV][H*W]         (list_k > 0) contributions recorded per pixel */
     size_t tile_flag;   /* uint32[NV*T]           (list_k > 0) 1: a pixel of the tile had more than list_k */
-    size_t tile_rec_start; /* unused (0 bytes) */
     size_t lists;       /* uint4[NV*T][list_k][256] (list_k > 0) {list position, alpha bits, depth bits, 0} */
 } GaRasterLayout;
 
 /* Fills *layout for NV = batch*views images of H x W, P surfels per batch item
- * and room for max_instances (surfel,tile) pairs over all images.
- * Host-only, no CUDA call. */
-int ga_raster_layout(int batch, int P, int views, int H, int W,
-                     int64_t max_instances, GaRasterLayout *layout);
-
-/* As ga_raster_layout, with room for the per-pixel contribution lists the forward records when list_k > 0
- * (list_k * 4 KB per tile; 32 is the default the Python mirror uses for calls that need gradients). */
+ * and room for max_instances (surfel,tile) pairs over all images, plus room for
+ * the per-pixel contribution lists the forward records when list_k > 0
+ * (list_k * 4 KB per tile; 32 is the default the Python mirror uses for calls
+ * that need gradients, 0 records none).  Host-only, no CUDA call. */
 int ga_raster_layout_ex(int batch, int P, int views, int H, int W,
                         int64_t max_instances, int list_k, GaRasterLayout *layout);
 
@@ -77,19 +72,19 @@ int ga_raster_layout_ex(int batch, int P, int views, int H, int W,
  * If the instance count exceeds max_instances, status[1] is set and the
  * images are undefined (no out-of-bounds access happens); the caller re-runs
  * with a larger workspace.
+ *
+ * list_k > 0 makes the composite record, for every pixel, the (list position, alpha, depth) of each surfel that
+ * contributed (up to list_k per pixel; a tile with a longer pixel is flagged and its backward recomputes).
+ * ga_raster_backward_ex with the same list_k then walks those lists instead of re-culling and re-evaluating every
+ * (pixel, surfel) pair -- what upstream's backward.cu renderCUDA does.  The workspace must be laid out with the
+ * same list_k.
+ *
+ * Status read-back: status_host and status_event are both NULL, or both set.  When set, right after the tile scan
+ * (before the scatter, the sort and the composite) status[0..3] = {instance count, overflow flag, tiles sorted in
+ * global memory, 0} is copied to `status_host` (pinned host memory, 4 ints) and `status_event` (a cudaEvent_t) is
+ * recorded.  The caller synchronises on the event -- the GPU is still busy with the rest of the forward -- and, if
+ * the overflow flag is set, re-runs with a larger workspace (the kernels after the scan exit early in that case).
  */
-int ga_raster_forward(const float *gauss13, int batch, int P, int views,
-                      const float *viewmats, const float *projmats, const float *bg,
-                      int H, int W, float scale_modifier,
-                      float *out_color, float *out_allmap, int32_t *out_radii,
-                      void *workspace, size_t workspace_bytes, int64_t max_instances,
-                      void *stream);
-
-/* ga_raster_forward with per-pixel contribution lists: list_k > 0 makes the composite record, for every pixel, the
- * (list position, alpha, depth) of each surfel that contributed (up to list_k per pixel; a tile with a longer pixel
- * is flagged and its backward recomputes).  ga_raster_backward_ex with the same list_k then walks those lists instead
- * of re-culling and re-evaluating every (pixel, surfel) pair -- what upstream's backward.cu renderCUDA does.
- * status_host / status_event: both NULL, or as in ga_raster_forward_async. */
 int ga_raster_forward_ex(const float *gauss13, int batch, int P, int views,
                          const float *viewmats, const float *projmats, const float *bg,
                          int H, int W, float scale_modifier,
@@ -97,33 +92,16 @@ int ga_raster_forward_ex(const float *gauss13, int batch, int P, int views,
                          void *workspace, size_t workspace_bytes, int64_t max_instances, int list_k,
                          int32_t *status_host, void *status_event, void *stream);
 
-/* The same forward in two halves, for callers that want to look at status[0..1] (instance count, overflow) after
- * the binning -- the point where upstream reads `num_rendered` back (rasterizer_impl.cu) -- and only then enqueue
- * the composite: ga_raster_forward_bin = per-surfel stage + binning, ga_raster_forward_render = composite. */
-int ga_raster_forward_bin(const float *gauss13, int batch, int P, int views,
-                          const float *viewmats, const float *projmats, const float *bg,
-                          int H, int W, float scale_modifier,
-                          float *out_color, float *out_allmap, int32_t *out_radii,
-                          void *workspace, size_t workspace_bytes, int64_t max_instances, void *stream);
-int ga_raster_forward_render(const float *gauss13, int batch, int P, int views,
-                             const float *viewmats, const float *projmats, const float *bg,
-                             int H, int W, float scale_modifier,
-                             float *out_color, float *out_allmap, int32_t *out_radii,
-                             void *workspace, size_t workspace_bytes, int64_t max_instances, void *stream);
+/* Bytes of scratch the backward wants: the gradient accumulators [NV*P][18].  A larger buffer is accepted; the
+ * rest of it is not used. */
+size_t ga_raster_backward_scratch_bytes(int batch, int P, int views);
 
-/* The whole forward enqueued at once, with the status read-back overlapped: right after the tile scan (before the
- * scatter, the sort and the composite) status[0..3] = {instance count, overflow flag, tiles sorted in global memory,
- * 0} is copied to `status_host` (pinned host memory, 4 ints) and `status_event` (a cudaEvent_t) is recorded.  The
- * caller synchronises on the event -- the GPU is still busy with the rest of the forward -- and, if the overflow
- * flag is set, re-runs with a larger workspace (the kernels after the scan exit early in that case). */
-int ga_raster_forward_async(const float *gauss13, int batch, int P, int views,
-                            const float *viewmats, const float *projmats, const float *bg,
-                            int H, int W, float scale_modifier,
-                            float *out_color, float *out_allmap, int32_t *out_radii,
-                            void *workspace, size_t workspace_bytes, int64_t max_instances,
-                            int32_t *status_host, void *status_event, void *stream);
-
-/* ga_raster_backward for a workspace laid out and filled with list_k (ga_raster_layout_ex / ga_raster_forward_ex). */
+/*
+ * Backward.  dL_dcolor [NV][3][H][W], dL_dallmap [NV][7][H][W]; grad_gauss13
+ * [batch][P][13] is OVERWRITTEN with the gradient summed over the views of
+ * each batch item (same column order as gauss13).  workspace and list_k must
+ * be the ones the matching ga_raster_forward_ex filled and used.
+ */
 int ga_raster_backward_ex(const float *gauss13, int batch, int P, int views,
                           const float *viewmats, const float *projmats, const float *bg,
                           int H, int W, float scale_modifier,
@@ -154,33 +132,6 @@ int ga_render_post_backward(const float *color, const float *allmap, const float
  * has the same switch (so_set_variant).  Affects calls made after it returns.
  */
 int ga_raster_set_variant(int radius_formula, int quat_norm_grad);
-int ga_raster_get_variant(int *radius_formula, int *quat_norm_grad);
-
-/*
- * No longer selects anything: the forward composite evaluates its (pixel, surfel) pairs in parallel and has no
- * lane-group mapping left to choose.  Kept so that existing callers still link.  Returns 0 for the former group
- * sizes 32, 16 and 8 and -1 for any other value.
- */
-int ga_raster_set_tuning(int fwd_group);
-
-/* Bytes of scratch the backward wants: the gradient accumulators [NV*P][18].  A larger buffer is accepted; the
- * rest of it is not used. */
-size_t ga_raster_backward_scratch_bytes(int batch, int P, int views);
-
-/*
- * Backward.  dL_dcolor [NV][3][H][W], dL_dallmap [NV][7][H][W]; grad_gauss13
- * [batch][P][13] is OVERWRITTEN with the gradient summed over the views of
- * each batch item (same column order as gauss13).  workspace must be the one
- * the matching forward filled.
- */
-int ga_raster_backward(const float *gauss13, int batch, int P, int views,
-                       const float *viewmats, const float *projmats, const float *bg,
-                       int H, int W, float scale_modifier,
-                       const int32_t *radii,
-                       const float *dL_dcolor, const float *dL_dallmap,
-                       const void *workspace, size_t workspace_bytes, int64_t max_instances,
-                       void *scratch, size_t scratch_bytes,
-                       float *grad_gauss13, void *stream);
 
 /*
  * ---------------------------------------------------------------------------

@@ -441,11 +441,9 @@ def test_switchable_judgement_calls(radius_formula, quat_norm_grad):
     """The two unpinned choices of the restatement (radius formula; quaternion-normalisation gradient) are run-time
     switches in the CUDA path and in the oracle: every combination stays in parity (integers bit-exact), and the
     alternatives really differ from the default."""
-    import ctypes as C
     from gaussiananything_b200 import _lib, raster
     from oracle import surfel_oracle as so
     lib = _lib.lib()
-    lib.ga_raster_set_variant.argtypes = [C.c_int, C.c_int]
     P, H, W = 3000, 96, 112
     g = scene(P, 50, 6.0)
     g[:, 6:10] *= np.linspace(0.5, 2.0, P, dtype=np.float32)[:, None]        # non-unit quaternions

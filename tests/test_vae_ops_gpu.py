@@ -19,19 +19,8 @@ def _p(t):
 
 def _env():
     from gaussiananything_b200 import _lib
-    L = _lib.lib()
-    vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_int64, C.c_float
-    L.ga_layernorm_modulate.argtypes = [vp, vp, vp, vp, vp, i32, i32, vp, i32, i32, f32, vp]
-    L.ga_thin_linear.argtypes = [vp, vp, vp, i32, vp, vp, vp, i32, i32, i32, f32, vp]
-    L.ga_micro_attention_bf16.argtypes = [vp, vp, vp, vp, i32, i32, i32, f32, vp]
-    L.ga_micro_seq_build.argtypes = [vp, i32, vp, vp, i64, i32, i32, vp]
-    L.ga_surfel_cascade_pack.argtypes = [vp, i32, vp, vp, i32, i32, f32, f32, vp, vp, i64, vp]
-    L.ga_silu_to_bf16.argtypes = [vp, vp, i64, vp]
-    for n in ("ga_layernorm_modulate", "ga_thin_linear", "ga_micro_attention_bf16", "ga_micro_seq_build",
-              "ga_surfel_cascade_pack", "ga_silu_to_bf16"):
-        getattr(L, n).restype = i32
     dev = torch.device("cuda:0")
-    return L, dev, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    return _lib.lib(), dev, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 @pytest.mark.parametrize("R,D", [(77, 64), (300, 768), (33, 1024)])

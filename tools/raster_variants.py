@@ -22,9 +22,6 @@ def main():
     P, H, W, V = 100000, 512, 512, 6
     dev = torch.device("cuda:0")
     lib = _lib.lib()
-    lib.ga_profile_enable.argtypes = [C.c_int]
-    lib.ga_profile_read.argtypes = [C.POINTER(C.c_float), C.c_int]
-    lib.ga_profile_read.restype = C.c_int
     g = scene(P, 40)
     vs, ps, _, _ = cameras(V)
     g13 = torch.tensor(g, device=dev)[None].contiguous()
