@@ -45,8 +45,8 @@ struct RasterWs {
     float *depth;
     uint32_t *rect;
     uint32_t *tile_count;
-    uint32_t *big_tiles;       // tiles above the warp-sort limit, listed by the tile scan (status[3] entries); kept
-                               // in the tile_count region of the layout, after the counters
+    uint32_t *big_tiles;       // tiles above 512 instances, listed by the tile scan as a diagnostic (status[3]
+                               // entries); kept in the tile_count region of the layout, after the counters
     uint32_t *tile_start;
     unsigned long long *keys;
     uint32_t *ids;
@@ -68,11 +68,11 @@ cudaError_t ga_launch_preprocess(const RasterDims &d, const RasterWs &w, const f
                                  int32_t *out_radii, cudaStream_t s);
 // status_host / status_event (both NULL, or both set): after the tile scan -- the first point where the instance
 // count and the overflow flag are known -- status[0..3] is copied to pinned host memory and the event recorded, so
-// the host can look at them while the scatter / sort / composite kernels are still running.
+// the host can look at them while the scatter and composite kernels are still running.
 // Tile counters / scatter cursors are kept in GA_TILE_REPLICAS copies per tile (replica = warp index mod R): the
 // 1.05M atomics of the C2 scene otherwise queue up on 6144 addresses, ~170 deep, and L2 serialises same-address
 // atomics (scatter: 48 us for 1M atomics).  The scan sums the replicas of a tile and hands every replica its own
-// sub-range of the tile's slots; the order inside a tile is fixed afterwards by the sort, so results do not change.
+// sub-range of the tile's slots; the forward sorts each tile before it composites, so results do not change.
 #ifndef GA_TILE_REPLICAS
 #define GA_TILE_REPLICAS 8
 #endif

@@ -4,6 +4,9 @@
 // Restates upstream forward.cu / backward.cu renderCUDA
 // (github.com/hbb1/diff-surfel-rasterization; called from
 // /root/reference/nsr/gs_surfel.py:100-114).  Differences in HOW, not WHAT:
+//  * the binning leaves each tile's keys unordered; the forward's CTA for a
+//    tile sorts them by depth in shared memory before it composites, and
+//    writes the sorted keys and ids back for the backward.
 //  * the forward evaluates only the (pixel, surfel) pairs inside each surfel's
 //    conservative cull box (computed in K1), all of them in parallel, and then
 //    composites every pixel from shared memory.  The cull box contains every
@@ -114,13 +117,173 @@ __device__ __forceinline__ TileBox clip_box(const float4 bb, int ox, int oy, int
 
 struct FwdSmem {
     float4 rec[6][CHUNK];           // the chunk's staged records, see above
-    float2 pair[FWD_PAIRS];         // {alpha, depth} of the window's passing pairs, by pair index
+    float2 pair[FWD_PAIRS];         // {alpha, depth} of the window's passing pairs, by pair index; before the first
+                                    // window: the tile's keys, sorted (FWD_PAIRS keys of 8 bytes fit)
     uint32_t mask[CHUNK / 32][256]; // per pixel: the window's slots whose pair passed, slot t at bit t & 31 of word t >> 5
     int base[CHUNK + 1];            // pair base of every slot relative to the chunk; base[CHUNK] = the chunk's pairs
     uint32_t box[CHUNK];            // clipped box: x0 | y0 << 4 | w << 8 | (65536 / w + 1) << 13
     int cnt[CHUNK];                 // LISTS: contributions of each staged instance
     int wsum[8];
 };
+
+// Ascending-only bitonic network (flip + half-cleaners): every compare-exchange
+// moves the minimum to the lower index, so virtual +inf padding beyond n never
+// moves and n need not be a power of two.  Works on shared or global memory.
+__device__ __forceinline__ void block_bitonic_sort(unsigned long long *a, int n)
+{
+    int n2 = 1;
+    while (n2 < n) n2 <<= 1;
+    for (int k = 2; k <= n2; k <<= 1) {
+        // flip step: partner = mirror inside the k-block
+        for (int t = threadIdx.x; t < n2 / 2; t += blockDim.x) {
+            const int blk = t / (k / 2), off = t % (k / 2);
+            const int i = blk * k + off, p = blk * k + k - 1 - off;
+            if (p < n) {
+                unsigned long long x = a[i], y = a[p];
+                if (x > y) { a[i] = y; a[p] = x; }
+            }
+        }
+        __syncthreads();
+        for (int j = k / 4; j >= 1; j >>= 1) {
+            for (int t = threadIdx.x; t < n2 / 2; t += blockDim.x) {
+                const int i = (t / j) * 2 * j + (t % j), p = i + j;
+                if (p < n) {
+                    unsigned long long x = a[i], y = a[p];
+                    if (x > y) { a[i] = y; a[p] = x; }
+                }
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// Warp-level bitonic sort of 32*KPL keys held in registers, element i = r*32 + lane: partner distances < 32 are
+// shuffles, distances >= 32 stay inside the lane.  Fully unrolled (KPL <= 2 here): every stage is one 64-bit shuffle,
+// one 64-bit compare and a select, since the compiler can work out each stage's direction bits once per lane.
+template <int KPL>
+__device__ __forceinline__ void warp_shuffle_stages(unsigned long long (&v)[KPL], int lane, int k, int jstart)
+{
+#pragma unroll
+    for (int j = jstart; j >= 1; j >>= 1) {
+        const bool lower = (lane & j) == 0;
+#pragma unroll
+        for (int r = 0; r < KPL; r++) {
+            const bool asc = ((((r << 5) | lane) & k) == 0);
+            const unsigned long long mine = v[r];
+            const unsigned long long other = __shfl_xor_sync(0xffffffffu, mine, j);
+            const bool keep_min = (lower == asc);
+            v[r] = ((other < mine) == keep_min) ? other : mine;
+        }
+    }
+}
+
+template <int KPL>
+__device__ __forceinline__ void warp_bitonic_sort(unsigned long long (&v)[KPL], int lane)
+{
+    constexpr int N = 32 * KPL;
+#pragma unroll
+    for (int k = 2; k <= 32; k <<= 1) warp_shuffle_stages<KPL>(v, lane, k, k >> 1);
+#pragma unroll
+    for (int k = 64; k <= N; k <<= 1) {
+#pragma unroll
+        for (int j = k >> 1; j >= 32; j >>= 1) {
+            const int jr = j >> 5;
+#pragma unroll
+            for (int r = 0; r < KPL; r++) {
+                if ((r & jr) == 0) {
+                    const bool asc = (((r << 5) & k) == 0);              // k >= 64 here: decided by r alone
+                    unsigned long long a = v[r], b = v[r | jr];
+                    const bool sw = asc ? (a > b) : (a < b);
+                    v[r] = sw ? b : a;
+                    v[r | jr] = sw ? a : b;
+                }
+            }
+        }
+        warp_shuffle_stages<KPL>(v, lane, k, 16);
+    }
+}
+
+// Sorts n <= 256 * KPL keys from src into a: warp w sorts keys [w * 32 * KPL, (w + 1) * 32 * KPL) in registers and
+// stores that run to a (padded with ~0); then every key's rank is its position in its own run plus, for every other
+// run, a binary search for the keys below it.  Keys are unique, so the ranks are a permutation of [0, n).
+template <int KPL>
+__device__ __forceinline__ void block_merge_sort(const unsigned long long *src, unsigned long long *a, int n,
+                                                 const float *rec)
+{
+    constexpr int SEG = 32 * KPL;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int nseg = (n + SEG - 1) / SEG;
+    unsigned long long v[KPL];
+    int rank[KPL];
+    if (warp < nseg) {
+#pragma unroll
+        for (int r = 0; r < KPL; r++) {
+            const int i = warp * SEG + r * 32 + lane;
+            v[r] = i < n ? src[i] : ~0ull;
+            // the first chunk's staging loads these records right after the sort
+            if (i < n) asm volatile("prefetch.global.L2 [%0];" ::"l"(rec + (size_t)(uint32_t)v[r] * GA_REC_F));
+        }
+        warp_bitonic_sort<KPL>(v, lane);
+#pragma unroll
+        for (int r = 0; r < KPL; r++) a[warp * SEG + r * 32 + lane] = v[r];
+    }
+    __syncthreads();
+    if (warp < nseg) {
+#pragma unroll
+        for (int r = 0; r < KPL; r++) rank[r] = r * 32 + lane;
+        for (int sg = 0; sg < nseg; sg++) {
+            if (sg == warp) continue;
+            const unsigned long long *run = a + sg * SEG;
+#pragma unroll
+            for (int r = 0; r < KPL; r++) {
+                int lo = 0;                 // largest lo <= SEG - 1 with run[lo - 1] < v[r], then one more test
+#pragma unroll
+                for (int step = SEG / 2; step >= 1; step >>= 1)
+                    if (run[lo + step - 1] < v[r]) lo += step;
+                rank[r] += lo + (run[lo] < v[r] ? 1 : 0);
+            }
+        }
+    }
+    __syncthreads();
+    if (warp < nseg) {
+#pragma unroll
+        for (int r = 0; r < KPL; r++)
+            if (warp * SEG + r * 32 + lane < n) a[rank[r]] = v[r];
+    }
+    __syncthreads();
+}
+
+// Sorts the tile's n keys [start, start + n) ascending (the scatter wrote them unordered) and writes them back to
+// ws.keys, with their surfel ids to ws.ids.  The whole tile is sorted even when compositing stops early: the backward
+// reads the ids of every position up to the tile's deepest contributor.  Tiles up to FWD_PAIRS keys are sorted in s
+// (the pair buffer, idle until the first window), where they stay for the first chunk's staging; larger tiles are
+// sorted in place in global memory (L2 resident) by the bitonic network and counted in status[2].
+// The forward is bound by instruction issue, so the sort's cost is its instruction count.  On C2 (H100 80GB HBM3)
+// it made render_fwd 18 us longer per step with unrolled warp runs + binary-search ranks and the record prefetch (700 W
+// power limit); at 400 W: 25 us with the warp stages as a loop, 31 us without the prefetch, 56 us with a rank sort
+// (every key against every key) and 94 us with the bitonic network for every tile.
+__device__ __forceinline__ void sort_tile(const RasterWs &ws, uint32_t start, int n, unsigned long long *s, const float *rec)
+{
+    unsigned long long *gk = ws.keys + start;
+    if (n > FWD_PAIRS) {
+        if (threadIdx.x == 0) atomicAdd(&ws.status[2], 1);
+        block_bitonic_sort(gk, n);
+        for (int i = threadIdx.x; i < n; i += 256) ws.ids[start + i] = (uint32_t)(gk[i] & 0xffffffffull);
+        return;
+    }
+    if (n <= 256) block_merge_sort<1>(gk, s, n, rec);
+    else if (n <= 512) block_merge_sort<2>(gk, s, n, rec);
+    else {
+        for (int i = threadIdx.x; i < n; i += 256) s[i] = gk[i];
+        __syncthreads();
+        block_bitonic_sort(s, n);
+    }
+    for (int i = threadIdx.x; i < n; i += 256) {
+        const unsigned long long k = s[i];
+        gk[i] = k;
+        ws.ids[start + i] = (uint32_t)(k & 0xffffffffull);
+    }
+}
 
 template <bool LISTS>
 __global__ void __launch_bounds__(256, 3)
@@ -153,13 +316,18 @@ render_fwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg,
     uint4 *my_list = nullptr;
     if (LISTS) my_list = ws.lists + ((size_t)view * d.T + tile) * (size_t)d.list_k * 256 + pix_local;
 
+    const unsigned long long *skeys = reinterpret_cast<const unsigned long long *>(sm.pair);
+    sort_tile(ws, start, total, reinterpret_cast<unsigned long long *>(sm.pair), rec_base);
+
     for (int c0 = 0; c0 < total; c0 += CHUNK) {
         if (__syncthreads_count(done) == 256) break;
         const int cnt = min(CHUNK, total - c0);
         if (LISTS) sm.cnt[threadIdx.x] = 0;
         int npairs = 0;
         if ((int)threadIdx.x < cnt) {
-            const uint32_t id = ws.ids[start + c0 + threadIdx.x];
+            // the first window overwrites the sorted keys in sm.pair; later chunks read the ids back from global memory
+            const uint32_t id = (c0 == 0 && total <= FWD_PAIRS) ? (uint32_t)(skeys[threadIdx.x] & 0xffffffffull)
+                                                                : ws.ids[start + c0 + threadIdx.x];
             const float4 *src = reinterpret_cast<const float4 *>(rec_base + (size_t)id * GA_REC_F);
             const float4 a = __ldg(src), b = __ldg(src + 1), c = __ldg(src + 2);
             const float4 nr = __ldg(src + 3), bb = __ldg(src + 4), gb = __ldg(src + 5);

@@ -38,11 +38,11 @@ extern "C" {
  * equivalent of upstream's geomBuffer/binningBuffer/imgBuffer). */
 typedef struct GaRasterLayout {
     size_t total_bytes;
-    size_t status;      /* int32[16]: [0]=instances D, [1]=overflow flag, [2]=tiles sorted out of smem */
+    size_t status;      /* int32[16]: [0]=instances D, [1]=overflow flag, [2]=tiles above 4096 instances (sorted in global memory), [3]=tiles above 512 */
     size_t rec;         /* float[NV*P][24]  Tu3 Tv3 Tw3 | xy2 opacity | normal3 | r | bbox x0 x1 y0 y1 | g b - - */
     size_t depth;       /* float[NV*P]      view-space z (0 when culled) */
     size_t rect;        /* uint32[NV*P]     x0 | y0<<8 | x1<<16 | y1<<24 (tile units) */
-    size_t tile_count;  /* uint32[NV*T*9]   scratch: per-tile counters, then fill cursors (8 replicas per tile); then the list of tiles above the warp-sort limit */
+    size_t tile_count;  /* uint32[NV*T*9]   scratch: per-tile counters, then fill cursors (8 replicas per tile); then the list of tiles above 512 instances */
     size_t tile_start;  /* uint32[NV*T+1]   exclusive scan == tile ranges [start,end) */
     size_t keys;        /* uint64[max_instances]  (depth bits<<32 | surfel), sorted per tile */
     size_t ids;         /* uint32[max_instances]  sorted surfel index per instance */
@@ -80,8 +80,8 @@ int ga_raster_layout_ex(int batch, int P, int views, int H, int W,
  * same list_k.
  *
  * Status read-back: status_host and status_event are both NULL, or both set.  When set, right after the tile scan
- * (before the scatter, the sort and the composite) status[0..3] = {instance count, overflow flag, tiles sorted in
- * global memory, 0} is copied to `status_host` (pinned host memory, 4 ints) and `status_event` (a cudaEvent_t) is
+ * (before the scatter and the composite, which sorts each tile) status[0..3] = {instance count, overflow flag, 0,
+ * tiles above 512 instances} is copied to `status_host` (pinned host memory, 4 ints) and `status_event` (a cudaEvent_t) is
  * recorded.  The caller synchronises on the event -- the GPU is still busy with the rest of the forward -- and, if
  * the overflow flag is set, re-runs with a larger workspace (the kernels after the scan exit early in that case).
  */
