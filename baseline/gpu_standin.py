@@ -151,3 +151,69 @@ def time_torch_dit(dev, depth, D, H, N, Cin=3, M=1369, Dc=1024, nfe=20):
     del m
     torch.cuda.empty_cache()
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# TorchDino -- the DINOv2 ViT-L/14-reg4 image conditioner restated as plain PyTorch and run the way the reference runs
+# it: nn.Linear / Conv2d under bf16 autocast (cuBLAS / cuDNN), F.scaled_dot_product_attention, separate LayerNorm /
+# GELU / LayerScale / residual kernels.  Same state dict layout as gaussiananything_b200.dino (torch.hub layout);
+# the image is already 518^2, so the preprocess is the normalisation only.
+# ---------------------------------------------------------------------------------------------------------------------
+class TorchDino(nn.Module):
+    def __init__(self, sd, heads=16):
+        super().__init__()
+        self.sd = {k: v.float() for k, v in sd.items()}
+        self.heads = heads
+        self.depth = 1 + max(int(k.split(".")[1]) for k in sd if k.startswith("blocks."))
+        self.register_buffer("mean", torch.tensor((0.485, 0.456, 0.406)).view(1, 3, 1, 1))
+        self.register_buffer("std", torch.tensor((0.229, 0.224, 0.225)).view(1, 3, 1, 1))
+
+    def to(self, dev):
+        self.sd = {k: v.to(dev) for k, v in self.sd.items()}
+        return super().to(dev)
+
+    def forward(self, img):
+        sd, H = self.sd, self.heads
+        x = ((img.float() + 1.0) / 2.0 - self.mean) / self.std
+        x = F.conv2d(x, sd["patch_embed.proj.weight"], sd["patch_embed.proj.bias"], stride=14).flatten(2).transpose(1, 2)
+        B, _, D = x.shape
+        x = torch.cat([sd["cls_token"].expand(B, -1, -1), x], 1) + sd["pos_embed"]
+        x = torch.cat([x[:, :1], sd["register_tokens"].expand(B, -1, -1), x[:, 1:]], 1).float()
+        N = x.shape[1]
+        for i in range(self.depth):
+            p = "blocks.%d." % i
+            h = F.layer_norm(x, (D,), sd[p + "norm1.weight"], sd[p + "norm1.bias"], 1e-6)
+            qkv = F.linear(h, sd[p + "attn.qkv.weight"], sd[p + "attn.qkv.bias"]).view(B, N, 3, H, D // H).permute(2, 0, 3, 1, 4)
+            a = F.scaled_dot_product_attention(qkv[0], qkv[1], qkv[2]).transpose(1, 2).reshape(B, N, D)
+            x = x + sd[p + "ls1.gamma"] * F.linear(a, sd[p + "attn.proj.weight"], sd[p + "attn.proj.bias"])
+            h = F.layer_norm(x, (D,), sd[p + "norm2.weight"], sd[p + "norm2.bias"], 1e-6)
+            f = F.gelu(F.linear(h, sd[p + "mlp.fc1.weight"], sd[p + "mlp.fc1.bias"]))
+            x = x + sd[p + "ls2.gamma"] * F.linear(f, sd[p + "mlp.fc2.weight"], sd[p + "mlp.fc2.bias"])
+        xn = F.layer_norm(x.float(), (D,), sd["norm.weight"], sd["norm.bias"], 1e-6)
+        return {"x_norm_clstoken": xn[:, 0], "x_norm_patchtokens": xn[:, 5:]}
+
+
+def time_torch_dino(dev, sd, B, min_seconds=2.0):
+    """ms per image of TorchDino at batch B (eager, bf16 autocast), device events over >= min_seconds of work."""
+    m = TorchDino(sd).to(dev).eval()
+    img = torch.rand(B, 3, 518, 518, device=dev) * 2 - 1
+    with torch.no_grad(), torch.autocast("cuda", dtype=torch.bfloat16):
+        for _ in range(3):
+            y = m(img)
+        assert torch.isfinite(y["x_norm_patchtokens"]).all()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize(dev)
+        e0.record()
+        m(img)
+        e1.record()
+        e1.synchronize()
+        reps = max(3, math.ceil(min_seconds / max(e0.elapsed_time(e1) * 1e-3, 1e-6)))
+        e0.record()
+        for _ in range(reps):
+            m(img)
+        e1.record()
+        e1.synchronize()
+    ms = e0.elapsed_time(e1) / reps
+    del m
+    torch.cuda.empty_cache()
+    return {"batch": B, "reps": reps, "ms_per_batch": ms, "ms_per_image": ms / B}

@@ -25,3 +25,9 @@ def install_shims(replace_classes: bool = True):
         m = sys.modules.get("dit.dit_i23d")
         if m is not None and hasattr(m, "DiT_models"):
             m.DiT_models.update(_dit.DiT_models)
+        from . import dino as _dino
+        for name in ("sgm.modules.encoders.modules", "sgm.modules"):
+            m = sys.modules.get(name)
+            if m is not None:
+                for attr in ("FrozenDinov2ImageEmbedder", "PCD_Scaler", "GeneralConditioner"):
+                    setattr(m, attr, getattr(_dino, attr))

@@ -60,6 +60,9 @@ ABI = {
     "ga_micro_seq_build": (i32, [vp, i32, vp, vp, i64, i32, i32, vp]),
     "ga_surfel_cascade_pack": (i32, [vp, i32, vp, vp, i32, i32, f32, f32, vp, vp, i64, vp]),
     "ga_silu_to_bf16": (i32, [vp, vp, i64, vp]),
+    "ga_dino_frontend_scratch_bytes": (sz, [i32, i32, i32, i32]),
+    "ga_dino_frontend": (i32, [vp, i32, i32, i32, i32, i32, vp, i32, vp, sz, vp]),
+    "ga_dino_tokens": (i32, [vp, vp, vp, i32, vp, vp, i32, i32, i32, vp]),
     "ga_profile_enable": (i32, [i32]),
     "ga_profile_read": (i32, [C.POINTER(f32), i32]),
     "ga_b200_version": (C.c_char_p, []),

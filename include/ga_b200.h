@@ -241,6 +241,31 @@ int ga_surfel_cascade_pack(const float *res, int res_in_sequences, const float *
                            int64_t R, void *stream);
 int ga_silu_to_bf16(const float *x, void *y, int64_t n, void *stream);            /* y = bf16(silu(x)) */
 
+/*
+ * ---------------------------------------------------------------------------
+ * Part 3: image conditioner (DINOv2 ViT-L/14 with 4 registers, SURVEY 8f row N3).
+ * Replaces FrozenDinov2ImageEmbedder.preprocess (kornia resize + normalise,
+ * /root/reference/sgm/modules/encoders/modules.py:862-875) and the token
+ * preparation in front of the ViT blocks.  The blocks themselves run on the
+ * Part 2 entry points (ga_layernorm_modulate, ga_gemm_bf16_tn,
+ * ga_attention_bf16) and the final norm on ga_layernorm_rows.
+ * ---------------------------------------------------------------------------
+ */
+/* Bytes of fp32 scratch ga_dino_frontend needs: 0 unless the image is downscaled (H or W > out_size), when the
+ * antialias blur writes two [batch, 3, H, W] planes. */
+size_t ga_dino_frontend_scratch_bytes(int batch, int H, int W, int out_size);
+/* img fp32 [batch, 3, H, W] in [-1, 1] -> (blur if downscaling) -> bicubic align_corners=True resize to
+ * out_size^2 (skipped when H == W == out_size) -> (x + 1) / 2 -> (x - ImageNet mean) / std -> patches_bf16
+ * [batch * np * np, k_pitch], np = out_size / patch, column c*patch^2 + ky*patch + kx (conv weight
+ * reshape(D, 3*patch^2)), columns from 3*patch^2 on zero.  out_size % patch == 0, k_pitch >= 3*patch^2 and a
+ * multiple of 8; H, W, out_size <= 4096 (GA_ERR_SIZE above). */
+int ga_dino_frontend(const float *img, int batch, int H, int W, int out_size, int patch, void *patches_bf16,
+                     int k_pitch, void *scratch, size_t scratch_bytes, void *stream);
+/* x fp32 [batch, 1 + n_reg + n_patch, D] = cls_token + pos_embed[0] | reg_tokens [n_reg, D] (no pos_embed) |
+ * patch_out [batch * n_patch, D] + pos_embed[1 ..] ; pos_embed [1 + n_patch, D], D % 4 == 0 */
+int ga_dino_tokens(const float *patch_out, const float *cls_token, const float *reg_tokens, int n_reg,
+                   const float *pos_embed, float *x, int batch, int n_patch, int D, void *stream);
+
 /* Measurement aid: when enabled, cudaEvents are recorded around every kernel
  * stage of the next forward/backward; ga_profile_read synchronises on them and
  * returns per-stage milliseconds: [0] preprocess, [1] binning, [2] render fwd,
