@@ -31,3 +31,8 @@ def install_shims(replace_classes: bool = True):
             if m is not None:
                 for attr in ("FrozenDinov2ImageEmbedder", "PCD_Scaler", "GeneralConditioner"):
                     setattr(m, attr, getattr(_dino, attr))
+        m = sys.modules.get("nsr.lsgm.flow_matching_trainer")
+        if m is not None and hasattr(m, "FlowMatchingEngine"):
+            from . import mesh as _mesh
+            m.FlowMatchingEngine.extract_mesh_bounded = _mesh._engine_extract_mesh_bounded
+            m.FlowMatchingEngine.export_mesh_from_2dgs = _mesh._engine_export_mesh_from_2dgs

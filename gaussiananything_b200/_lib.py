@@ -63,6 +63,14 @@ ABI = {
     "ga_dino_frontend_scratch_bytes": (sz, [i32, i32, i32, i32]),
     "ga_dino_frontend": (i32, [vp, i32, i32, i32, i32, i32, vp, i32, vp, sz, vp]),
     "ga_dino_tokens": (i32, [vp, vp, vp, i32, vp, vp, i32, i32, i32, vp]),
+    "ga_mesh_work_bytes": (sz, [i64]),
+    "ga_mesh_prepare": (i32, [vp, vp, vp, i32, i32, i32, vp, f32, vp, vp]),
+    "ga_mesh_touch": (i32, [vp, i32, i32, i32, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "ga_mesh_integrate": (i32, [vp, i32, i32, i32, vp, vp, vp, vp, vp, i32, vp, vp]),
+    "ga_mesh_cubes_count": (i32, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "ga_mesh_cubes_emit": (i32, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "ga_mesh_clusters": (i32, [vp, i32, vp, i64, vp, vp, vp, vp, vp, vp, vp]),
+    "ga_mesh_filter": (i32, [vp, vp, i32, vp, i32, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]),
     "ga_profile_enable": (i32, [i32]),
     "ga_profile_read": (i32, [C.POINTER(f32), i32]),
     "ga_b200_version": (C.c_char_p, []),

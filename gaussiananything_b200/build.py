@@ -20,6 +20,9 @@ COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relax
 # rectangles / radii / depth keys are bit-exact with the C oracle.
 EXTRA = {
     "raster_preprocess.cu": ["--fmad=false"],
+    # TSDF weights / tsdf / colours and marching-cubes vertices: bit-exact with oracle/tsdf_oracle.py
+    "mesh_tsdf.cu": ["--fmad=false"],
+    "mesh_extract.cu": ["--fmad=false"],
 }
 
 

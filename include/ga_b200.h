@@ -266,6 +266,78 @@ int ga_dino_frontend(const float *img, int batch, int H, int W, int out_size, in
 int ga_dino_tokens(const float *patch_out, const float *cls_token, const float *reg_tokens, int n_reg,
                    const float *pos_embed, float *x, int batch, int n_patch, int D, void *stream);
 
+/*
+ * ---------------------------------------------------------------------------
+ * Part 4: mesh extraction (TSDF fusion of rendered RGB-D views, marching cubes, cluster filtering; SURVEY 8f row
+ * N4).  Replaces Open3D's ScalableTSDFVolume integrate / extract_triangle_mesh and TriangleMesh
+ * cluster_connected_triangles / remove_* as FlowMatchingEngine.extract_mesh_bounded and utils/mesh_util.post_process_mesh
+ * call them (nsr/lsgm/flow_matching_trainer.py:1244-1395, utils/mesh_util.py:22-44).
+ *
+ * The volume is made of units of 16^3 voxels.  Units are addressed inside a box of nx*ny*nz units whose first unit
+ * is (x0, y0, z0): box is int32[6] = {x0, y0, z0, nx, ny, nz} (device).  A unit's box index is
+ * (ux * ny + uy) * nz + uz; a voxel's index inside its unit is (x * 16 + y) * 16 + z.
+ * volume is double[2] = {voxel_length, sdf_trunc} (device).
+ * Counts come back in status int32[GA_MESH_STATUS_INTS] (device); each entry point below writes only its own
+ * words.  status_host (pinned, GA_MESH_STATUS_INTS ints) and status_event (a cudaEvent_t) are both NULL or both
+ * set; when set, the entry point copies all the status words there after its counts are final and records the
+ * event.  work: scratch of ga_mesh_work_bytes(n) bytes, n as stated at each entry point.
+ * ---------------------------------------------------------------------------
+ */
+#define GA_MESH_UNIT 16
+#define GA_MESH_CAM_FLOATS 20     /* per view, float and double: row-major 4x4 | fx fy cx cy */
+#define GA_MESH_STATUS_INTS 8     /* [0] units [1] point outside the box [2] vertices [3] triangles [4] clusters
+                                     [5] kept vertices [6] kept triangles */
+#define GA_MESH_TRI_ROW 16        /* int8 per marching-cubes case: edge triples, then -1 */
+
+/* Bytes of the `work` scratch for n items. Host-only. */
+size_t ga_mesh_work_bytes(int64_t n);
+/* rgb [V,3,H,W], depth [V,H,W], alpha [V,H,W] fp32 -> texels uint2 [V,H,W] = {depth bits, r | g << 8 | b << 16}:
+ * depth = 0 where alpha < alpha_thres or (double)depth >= depth_trunc[v] (double [V]); channel = uint8(clip(c,0,1)*255),
+ * truncated. */
+int ga_mesh_prepare(const float *rgb, const float *depth, const float *alpha, int views, int H, int W,
+                    const double *depth_trunc, float alpha_thres, void *texels, void *stream);
+/* Marks the units within sdf_trunc of every 4th pixel (rows and columns) with depth > 0, unprojected with
+ * cams_d[v] = {camera-to-world 4x4, fx fy cx cy} (double [V][20]): unit_table int32 [nx*ny*nz][(V+31)/32] gets bit v.
+ * A point whose units leave the box sets status[1] and marks nothing.  Then pool int32 [nx*ny*nz] lists the marked
+ * box indices in increasing order, unit_slot int32 [nx*ny*nz] maps a box index to its pool position or -1, and
+ * status[0] = number of marked units.  work: n = nx*ny*nz. */
+int ga_mesh_touch(const void *texels, int views, int H, int W, const double *cams_d, const double *volume,
+                  const int32_t *box, int box_units, int32_t *unit_table, int32_t *pool, int32_t *unit_slot,
+                  void *work, int32_t *status, int32_t *status_host, void *status_event, void *stream);
+/* TSDF integration of views 0..V-1, in order, into the n_units pooled units, each view only into the units it marked.
+ * cams_f[v] = {world-to-camera 4x4, fx fy cx cy} (float [V][20]); V <= 256.  voxels float [5][n_units * 4096]
+ * = tsdf | weight | r | g | b (r, g, b in 0..255) is overwritten. */
+int ga_mesh_integrate(const void *texels, int views, int H, int W, const float *cams_f, const double *volume,
+                      const int32_t *box, const int32_t *unit_table, const int32_t *pool, int n_units,
+                      float *voxels, void *stream);
+/* Marching cubes, counting pass.  cube uint8 [2][n_units * 4096]: case index of the cube at each voxel (0 when a
+ * corner's unit is missing or its weight is 0) | which of the voxel's +x, +y, +z edges carry a vertex (bits 0-2).
+ * vert_off / tri_off int32 [n_units * 4096]: exclusive offsets of each voxel's vertices / triangles; status[2],
+ * status[3] = totals.  tri_table int8 [256][GA_MESH_TRI_ROW].  work: n = n_units * 4096. */
+int ga_mesh_cubes_count(const float *voxels, int n_units, const int32_t *pool, const int32_t *unit_slot,
+                        const int32_t *box, const int8_t *tri_table, uint8_t *cube, int32_t *vert_off,
+                        int32_t *tri_off, void *work, int32_t *status, int32_t *status_host, void *status_event,
+                        void *stream);
+/* Marching cubes, emitting pass: vertices / colors double [status[2]][3] (colour in [0,1]), triangles int32
+ * [status[3]][3], in pool order, then voxel order, then x, y, z edge / table order. */
+int ga_mesh_cubes_emit(const float *voxels, int n_units, const int32_t *pool, const int32_t *unit_slot,
+                       const int32_t *box, const double *volume, const int8_t *tri_table, const uint8_t *cube,
+                       const int32_t *vert_off, const int32_t *tri_off, double *vertices, double *colors,
+                       int32_t *triangles, void *stream);
+/* Connected components of triangles that share an edge (vertex pair).  hash: hash_slots * 12 bytes, hash_slots a
+ * power of two >= 6 * n_tri.  label int32 [n_tri] = cluster of each triangle, clusters numbered by their smallest
+ * triangle; cluster_size int32 [n_tri], first status[4] entries valid.  work: n = n_tri. */
+int ga_mesh_clusters(const int32_t *triangles, int n_tri, void *hash, int64_t hash_slots, int32_t *label,
+                     int32_t *cluster_size, void *work, int32_t *status, int32_t *status_host, void *status_event,
+                     void *stream);
+/* Keeps the triangles whose cluster has >= min_size triangles, then the vertices they reference (in order), then
+ * drops the kept triangles with a repeated vertex.  out_* sized like the inputs; status[5], status[6] = kept
+ * vertices, kept triangles.  work: n = n_vert + n_tri. */
+int ga_mesh_filter(const double *vertices, const double *colors, int n_vert, const int32_t *triangles, int n_tri,
+                   const int32_t *label, const int32_t *cluster_size, int min_size, double *out_vertices,
+                   double *out_colors, int32_t *out_triangles, void *work, int32_t *status, int32_t *status_host,
+                   void *status_event, void *stream);
+
 /* Measurement aid: when enabled, cudaEvents are recorded around every kernel
  * stage of the next forward/backward; ga_profile_read synchronises on them and
  * returns per-stage milliseconds: [0] preprocess, [1] binning, [2] render fwd,
