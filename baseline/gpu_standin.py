@@ -217,3 +217,119 @@ def time_torch_dino(dev, sd, B, min_seconds=2.0):
     del m
     torch.cuda.empty_cache()
     return {"batch": B, "reps": reps, "ms_per_batch": ms, "ms_per_image": ms / B}
+
+
+class TorchVaeEncoder:
+    """Unfused bf16 PyTorch stand-in of the 3D VAE encoder (HybridEncoderPCDStructuredLatentSNoPCD + posterior) with
+    the reference's own op sequence: cuDNN convs and nn.Linear under bf16 autocast, F.group_norm / F.layer_norm,
+    F.scaled_dot_product_attention, a loop-per-point farthest-point sampling.  For timing beside
+    gaussiananything_b200.vae_encoder.SurfelEncoder (tools/vae_encoder_leg.py), not a checker."""
+
+    def __init__(self, sd, num_frames=8, latent_num=768, device="cuda:0"):
+        self.sd = {k: v.to(device).float() for k, v in sd.items()}
+        self.V, self.K = num_frames, latent_num
+
+    def _gn(self, x, p, silu=True):
+        y = F.group_norm(x.float(), 32, self.sd[p + "weight"], self.sd[p + "bias"], 1e-6)
+        return y * torch.sigmoid(y) if silu else y
+
+    def _conv(self, x, p, stride=1):
+        sd = self.sd
+        if stride == 2:
+            return F.conv2d(F.pad(x, (0, 1, 0, 1)), sd[p + "weight"], sd[p + "bias"], stride=2)
+        return F.conv2d(x, sd[p + "weight"], sd[p + "bias"], padding=sd[p + "weight"].shape[-1] // 2)
+
+    def _res(self, p, x):
+        h = self._conv(self._gn(x, p + "norm1."), p + "conv1.")
+        h = self._conv(self._gn(h, p + "norm2."), p + "conv2.")
+        if p + "nin_shortcut.weight" in self.sd:
+            x = self._conv(x, p + "nin_shortcut.")
+        return x + h
+
+    def _ln(self, x, p):
+        return F.layer_norm(x.float(), (x.shape[-1],), self.sd[p + "weight"], self.sd[p + "bias"], 1e-5)
+
+    def _mha(self, p, x, ctx, heads, qk_norm=False):
+        sd = self.sd
+        q, k, v = (F.linear(t, sd[p + n + ".weight"]) for t, n in ((x, "to_q"), (ctx, "to_k"), (ctx, "to_v")))
+        B, Nq, C = q.shape
+        q, k, v = (t.view(B, -1, heads, C // heads).transpose(1, 2) for t in (q, k, v))
+        if qk_norm:
+            rms = lambda t, w: (t.float() * torch.rsqrt(t.float().pow(2).mean(-1, keepdim=True) + 1e-5) * w).to(t.dtype)
+            q, k = rms(q, sd[p + "q_norm.weight"]), rms(k, sd[p + "k_norm.weight"])
+        o = F.scaled_dot_product_attention(q, k, v).transpose(1, 2).reshape(B, Nq, C)
+        return F.linear(o, sd[p + "to_out.0.weight"], sd[p + "to_out.0.bias"])
+
+    @staticmethod
+    def _fps(pcd, K, start):
+        B, N, _ = pcd.shape
+        idx = torch.empty(B, K, dtype=torch.long, device=pcd.device)
+        md = torch.full((B, N), float("inf"), device=pcd.device)
+        cur = start.to(pcd.device).long()
+        ar = torch.arange(B, device=pcd.device)
+        for k in range(K):
+            idx[:, k] = cur
+            d = ((pcd - pcd[ar, cur][:, None]) ** 2).sum(-1)
+            md = torch.minimum(md, d)
+            cur = md.argmax(1)
+        return torch.gather(pcd, 1, idx[..., None].expand(B, K, 3))
+
+    def _pe(self, xyz):
+        out = [xyz] + [f(xyz * 2.0 ** i) for i in range(10) for f in (torch.sin, torch.cos)]
+        p = "encoder.xyz_pos_embed.xyz_projection."
+        return F.linear(torch.cat(out, -1), self.sd[p + "weight"], self.sd[p + "bias"])
+
+    @torch.no_grad()
+    def encode(self, img, pcd, start):
+        sd, V, e = self.sd, self.V, "encoder."
+        with torch.autocast("cuda", dtype=torch.bfloat16):
+            h = self._conv(img, e + "conv_in.")
+            lvl = 0
+            while e + "down.%d.block.0.norm1.weight" % lvl in sd:
+                h = self._res(e + "down.%d.block.0." % lvl, h)
+                if e + "down.%d.downsample.conv.weight" % lvl in sd:
+                    h = self._conv(h, e + "down.%d.downsample.conv." % lvl, 2)
+                lvl += 1
+            h = self._res(e + "mid.block_1.", h)
+            a, b = e + "mid.attn_1.", e + "mid.attn_1.transformer_blocks.0."
+            n, C, Hf, Wf = h.shape
+            x_in = h
+            t = self._conv(self._gn(h, a + "norm.", False), a + "proj_in.").flatten(2).transpose(1, 2)
+            L = Hf * Wf
+            tm = t.reshape(n // V, V * L, -1)
+            tn = self._ln(tm, b + "norm1.")
+            tm = self._mha(b + "attn1.", tn, tn, 8) + tm
+            t = tm.reshape(n, L, -1)
+            tn = self._ln(t, b + "norm2.")
+            t = self._mha(b + "attn2.", tn, tn, 8) + t
+            xg, gate = F.linear(self._ln(t, b + "norm3."), sd[b + "ff.net.0.proj.weight"], sd[b + "ff.net.0.proj.bias"]).chunk(2, -1)
+            t = F.linear(xg * F.gelu(gate), sd[b + "ff.net.2.weight"], sd[b + "ff.net.2.bias"]) + t
+            h = self._conv(t.transpose(1, 2).reshape(n, -1, Hf, Wf), a + "proj_out.") + x_in
+            h = self._gn(self._res(e + "mid.block_2.", h), e + "norm_out.")
+            B = n // V
+            xyz = img[:, -3:, 4::8, 4::8].reshape(B, V, 3, -1).permute(0, 1, 3, 2).reshape(B, -1, 3)
+            tok = h.reshape(B, V, C, L).permute(0, 1, 3, 2).reshape(B, -1, C) + self._pe(xyz)
+            qxyz = self._fps(pcd.float(), self.K, start)
+            x = self._mha(e + "agg_ca.", self._pe(qxyz), tok, 8, qk_norm=True)
+            l = 0
+            while e + "srt.transformer.layers.%d.0.norm.weight" % l in sd:
+                p = e + "srt.transformer.layers.%d." % l
+                hn = self._ln(x, p + "0.norm.")
+                qkv = F.linear(hn, sd[p + "0.fn.qkv.weight"], sd[p + "0.fn.qkv.bias"]).view(B, self.K, 3, 8, C // 8)
+                q, k, v = qkv.permute(2, 0, 3, 1, 4)
+                rms = lambda t, w: (t.float() * torch.rsqrt(t.float().pow(2).mean(-1, keepdim=True) + 1e-5) * w).to(t.dtype)
+                q, k = rms(q, sd[p + "0.fn.q_norm.weight"]), rms(k, sd[p + "0.fn.k_norm.weight"])
+                o = F.scaled_dot_product_attention(q, k, v).transpose(1, 2).reshape(B, self.K, C)
+                x = x + F.linear(o, sd[p + "0.fn.proj.weight"], sd[p + "0.fn.proj.bias"])
+                f = F.gelu(F.linear(self._ln(x, p + "1.norm."), sd[p + "1.fn.mlp.0.weight"]) + sd[p + "1.fn.mlp.1.bias"])
+                x = x + F.linear(f, sd[p + "1.fn.mlp.2.weight"]) + sd[p + "1.fn.mlp.3.bias"]
+                l += 1
+            m = "encoder.Mlp_out."
+            hh = F.gelu(F.linear(self._ln(x, m + "norm."), sd[m + "fn.fc1.weight"], sd[m + "fn.fc1.bias"]), approximate="tanh")
+            hh = F.linear(hh, sd[m + "fn.fc2.weight"], sd[m + "fn.fc2.bias"]).float()
+        q = "decoder.superresolution.quant_conv."
+        mo = F.linear(F.gelu(F.linear(hh, sd[q + "fc1.weight"], sd[q + "fc1.bias"]), approximate="tanh"),
+                      sd[q + "fc2.weight"], sd[q + "fc2.bias"])
+        mean, logvar = mo.chunk(2, -1)
+        logvar = torch.tanh(logvar / 20.0) * 20.0
+        return {"h": hh, "query_pcd_xyz": qxyz, "mean": mean, "logvar": logvar, "std": torch.exp(0.5 * logvar)}

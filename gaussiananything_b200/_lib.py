@@ -28,6 +28,11 @@ class GaGemmEpilogue(C.Structure):
                 ("tok_pitch", C.c_int), ("eps", C.c_float)]
 
 
+class GaVaeEncHead(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("ln_w", "ln_b", "fc1_w", "fc1_b", "fc2_w", "fc2_b", "q1_w", "q1_b", "q2_w",
+                                          "q2_b")] + [("ln_eps", C.c_float)]
+
+
 vp, i32, i64, f32, sz = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_size_t
 _RASTER_IN = [vp, i32, i32, i32, vp, vp, vp, i32, i32, f32]   # gauss13, batch, P, views, viewmats, projmats, bg, H, W, scale
 
@@ -71,6 +76,14 @@ ABI = {
     "ga_mesh_cubes_emit": (i32, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "ga_mesh_clusters": (i32, [vp, i32, vp, i64, vp, vp, vp, vp, vp, vp, vp]),
     "ga_mesh_filter": (i32, [vp, vp, i32, vp, i32, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "ga_conv3x3_out_size": (i32, [i32, i32]),
+    "ga_conv3x3_bf16": (i32, [vp, i32, i32, i32, i32, vp, i32, vp, i32, i32, vp, vp, vp, vp]),
+    "ga_group_norm_scratch_bytes": (sz, [i32, i32]),
+    "ga_group_norm_nhwc": (i32, [vp, vp, vp, i32, i32, i32, f32, i32, vp, i32, vp, sz, vp]),
+    "ga_fps": (i32, [vp, i32, i32, i32, vp, vp, vp, vp]),
+    "ga_vae_enc_input": (i32, [vp, i32, i32, i32, i32, i32, vp, i32, i32, i32, vp, vp]),
+    "ga_heads32_split": (i32, [vp, vp, vp, i32, i32, i32, i32, f32, vp, vp, vp, vp]),
+    "ga_vae_enc_head": (i32, [C.POINTER(GaVaeEncHead), vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]),
     "ga_profile_enable": (i32, [i32]),
     "ga_profile_read": (i32, [C.POINTER(f32), i32]),
     "ga_b200_version": (C.c_char_p, []),

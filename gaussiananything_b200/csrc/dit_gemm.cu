@@ -160,6 +160,15 @@ __device__ __forceinline__ void epilogue_chunk(const GaGemmEpilogue &ep, uint32_
 #pragma unroll
                 for (int j = 0; j < 4; j++) if (nn + j < N) dst[j] = v[j];
             }
+        } else if (MODE == GA_EPI_GEGLU_BF16) {
+            // columns interleaved at pack time as (x_j, gate_j) pairs: out[m, j] = x_j * gelu_erf(gate_j)
+            __nv_bfloat16 *dst = reinterpret_cast<__nv_bfloat16 *>(ep.out) + (size_t)m * ep.ld_out + nn / 2;
+            if (vec) {
+                *reinterpret_cast<uint32_t *>(dst) = pack_bf16(v[0] * gelu_erf(v[1]), v[2] * gelu_erf(v[3]));
+            } else {
+#pragma unroll
+                for (int j = 0; j < 4; j += 2) if (nn + j + 1 < N) dst[j / 2] = __float2bfloat16(v[j] * gelu_erf(v[j + 1]));
+            }
         } else if (MODE == GA_EPI_RESID_GATE_F32) {
             // x[m, n] += gate[b, n] * (acc + bias)
             float *dst = reinterpret_cast<float *>(ep.out) + (size_t)m * ep.ld_out + nn;
@@ -466,6 +475,7 @@ static int launch_gemm(const void *A, int lda, const void *W, int ldw, const GaG
     case GA_EPI_GELU_BF16: return launch_gemm_mode<BN, GA_EPI_GELU_BF16>(ta, tb, ep, M, N, K, s);
     case GA_EPI_F32: return launch_gemm_mode<BN, GA_EPI_F32>(ta, tb, ep, M, N, K, s);
     case GA_EPI_RESID_GATE_F32: return launch_gemm_mode<BN, GA_EPI_RESID_GATE_F32>(ta, tb, ep, M, N, K, s);
+    case GA_EPI_GEGLU_BF16: return launch_gemm_mode<BN, GA_EPI_GEGLU_BF16>(ta, tb, ep, M, N, K, s);
     case GA_EPI_HEADS:
         if (BN == 128 || BN == 256)
             return launch_gemm_mode<((BN == 128 || BN == 256) ? BN : 128), GA_EPI_HEADS>(ta, tb, ep, M, N, K, s);
@@ -483,6 +493,7 @@ extern "C" int ga_gemm_bf16_tn(const void *A, int lda, const void *W, int ldw, i
     if (epi->mode == GA_EPI_HEADS && (N % 64 != 0 || epi->heads <= 0 || bn < 128)) return GA_ERR_BADARG;
     if (bn != 64 && bn != 128 && bn != 192 && bn != 256) return GA_ERR_BADARG;
     if (bn == 192 && epi->mode == GA_EPI_HEADS) return GA_ERR_BADARG;        // 192 is not a whole number of heads per half
+    if (epi->mode == GA_EPI_GEGLU_BF16 && N % 2) return GA_ERR_BADARG;        // (x, gate) column pairs
     cudaStream_t s = (cudaStream_t)stream;
     if (bn == 64) return launch_gemm<64>(A, lda, W, ldw, *epi, M, N, K, s);
     if (bn == 128) return launch_gemm<128>(A, lda, W, ldw, *epi, M, N, K, s);

@@ -301,14 +301,16 @@ class SurfelAE:
     gaussians_base 128^2, gaussians_upsampled 256^2, _2 384^2, _3 512^2 -- for all B x V cameras.  The reference
     issues 4 x B x V sequential launch sets from Python; here every level is ONE batched launch set and the four
     levels run on four CUDA streams, so the small levels (768 / 6 144 / 24 576 surfels: latency bound) overlap with
-    the 73 728-surfel one.  The encoder behaviours ('enc', 'enc_dec', ...) are out of scope (SURVEY.md 8) and raise."""
+    the 73 728-surfel one.  With `encoder=` (vae_encoder.SurfelEncoder) the encoder behaviours 'enc', 'encoder_vae' and
+    'enc_dec_wo_triplane' run too; without one, and for the other training behaviours, they raise."""
 
     OUTPUT_SIZE = {"gaussians_base": 128, "gaussians_upsampled": 256, "gaussians_upsampled_2": 384,
                    "gaussians_upsampled_3": 512}
 
-    def __init__(self, decoder, renderer=None, img_size=None, rand_base_render=True, rendering_kwargs=None):
+    def __init__(self, decoder, renderer=None, img_size=None, rand_base_render=True, rendering_kwargs=None, encoder=None):
         from .gs_surfel import GaussianRenderer2DGS
         self.decoder = decoder
+        self.encoder = encoder          # vae_encoder.SurfelEncoder: enables 'enc', 'encoder_vae', 'enc_dec_wo_triplane'
         self.img_size = img_size
         self.output_size = dict(self.OUTPUT_SIZE)
         self.rand_base_render = rand_base_render
@@ -373,7 +375,29 @@ class SurfelAE:
             return self.triplane_decode(latent, c, **kwargs)
         if behaviour == "get_rendering_kwargs":
             return self.rendering_kwargs
+        if self.encoder is not None and behaviour in ("enc", "encoder_vae", "enc_dec_wo_triplane"):
+            return self._encoder_behaviour(behaviour, img, kwargs)
         raise NotImplementedError("gaussiananything_b200.SurfelAE: behaviour %r is outside the decode / render path "
                                   "(encoder and training behaviours are not rebuilt: SURVEY.md section 8)" % (behaviour,))
 
     __call__ = forward
+
+    def _encoder_behaviour(self, behaviour, img, kwargs):
+        """nsr/script_util.py:320-359 with the point-cloud-structured encoder: img = img_to_encoder [B*V, 15, H, W],
+        pcd= [B, N, 3]; optional fps_start= [B] and generator= (posterior noise, FPS start)."""
+        enc = self.encoder
+        pcd, gen = kwargs.get("pcd"), kwargs.get("generator")
+        if pcd is None:
+            raise ValueError("SurfelAE(behaviour=%r) needs pcd= [B, N, 3]" % (behaviour,))
+        B = img.shape[0] // enc.V
+        if behaviour == "enc":
+            return enc.encode(img, pcd, kwargs.get("fps_start"), generator=gen)
+        if behaviour == "encoder_vae":
+            return enc.vae_reparameterization(enc.encode(img, pcd, kwargs.get("fps_start"), generator=gen), True, gen)
+        # enc_dec_wo_triplane: the posterior is sampled inside the encoder's launch sequence (mean + std * eps)
+        eps = torch.randn(B, enc.K, enc.zc, generator=gen)
+        lat = enc.encode(img, pcd, kwargs.get("fps_start"), noise=eps.to(img.device), generator=gen)
+        from .vae_encoder import Posterior
+        ret = {"latent_normalized": lat["latent_normalized"], "query_pcd_xyz": lat["query_pcd_xyz"],
+               "posterior": Posterior(lat["mean"], lat["logvar"], lat["std"]), "h": lat["h"]}
+        return self.decode_after_vae_no_render(ret, self.img_size)

@@ -155,6 +155,8 @@ int ga_raster_set_variant(int radius_formula, int quat_norm_grad);
 #define GA_EPI_RESID_GATE_F32  3   /* out fp32 [M, ld_out] += gate[m / rows_per_batch, n] * (acc + bias)   */
 #define GA_EPI_HEADS           4   /* split columns "(K H 64)" into heads: per-head RMSNorm on q/k, write
                                       Q,K [B,H,tok_pitch,64] and V transposed [B,H,64,tok_pitch] (bf16) */
+#define GA_EPI_GEGLU_BF16      5   /* W rows interleaved as (x_j, gate_j) pairs: out bf16 [M, ld_out] column j =
+                                      (acc + bias)[2j] * gelu_erf((acc + bias)[2j+1])  (GEGLU, N/2 columns) */
 
 typedef struct GaGemmEpilogue {
     int mode;
@@ -337,6 +339,64 @@ int ga_mesh_filter(const double *vertices, const double *colors, int n_vert, con
                    const int32_t *label, const int32_t *cluster_size, int min_size, double *out_vertices,
                    double *out_colors, int32_t *out_triangles, void *work, int32_t *status, int32_t *status_host,
                    void *status_event, void *stream);
+
+/*
+ * ---------------------------------------------------------------------------
+ * Part 5: 3D VAE encoder (HybridEncoderPCDStructuredLatentSNoPCD, /root/reference/nsr/srt/encoder.py:454-652, and the
+ * posterior of /root/reference/vit/vit_triplane.py:1347-1385).  Replaces the cuDNN 3x3 convolutions and GroupNorm
+ * of the SD conv encoder (ldm/modules/diffusionmodules/model.py:81-162,469-572), pytorch3d's
+ * sample_farthest_points + masked_gather, the per-head RMSNorm(32) of the SRT blocks and the readout MLPs.  The 1x1
+ * convolutions, linears and attentions of the encoder run on the Part 2 entry points (GEGLU via GA_EPI_GEGLU_BF16,
+ * the SRT's head_dim 32 zero-padded to 64 by ga_heads32_split).  Activations are NHWC.
+ * ---------------------------------------------------------------------------
+ */
+/* Output height (or width) of ga_conv3x3_bf16 for an input of H: H for stride 1, (H - 2) / 2 + 1 for stride 2.
+ * Host-only. */
+int ga_conv3x3_out_size(int H, int stride);
+/* 3x3 convolution as an implicit GEMM (wgmma, bf16 operands, fp32 accumulation).  x bf16 NHWC [n, H, W, Cin],
+ * Cin % 8 == 0; w_packed bf16 [Cout, k_pitch], column (ky * 3 + kx) * Cin + c, zero beyond 9 * Cin, k_pitch >=
+ * 9 * Cin rounded up to 64; Cout % 64 == 0.  stride 1: pad 1 on every side; stride 2: pad (0, 1, 0, 1) (the SD
+ * Downsample).  out[m, :] = bias + conv (+ residual[m, :], fp32), m = (image, oy, ox) over [n, Ho, Wo]; written to
+ * out_f32 and / or out_bf16 (either may be NULL, not both). */
+int ga_conv3x3_bf16(const void *x, int n, int H, int W, int Cin, const void *w_packed, int k_pitch,
+                    const float *bias, int Cout, int stride, const float *residual, float *out_f32,
+                    void *out_bf16, void *stream);
+/* Bytes of scratch ga_group_norm_nhwc needs for n images of HW pixels.  Host-only. */
+size_t ga_group_norm_scratch_bytes(int n, int HW);
+/* GroupNorm(32 groups) over x fp32 NHWC [n, HW, C] (statistics per image and group, fp32 partial sums folded in
+ * fp64), * gamma + beta, then SiLU if silu != 0; out bf16 (out_bf16 != 0) or fp32, same layout.  C % 32 == 0,
+ * C <= 1024.  Deterministic. */
+int ga_group_norm_nhwc(const float *x, const float *gamma, const float *beta, int n, int HW, int C, float eps,
+                       int silu, void *out, int out_bf16, void *scratch, size_t scratch_bytes, void *stream);
+/* Farthest-point sampling, one CTA per sample: pcd fp32 [batch, N, 3], N <= 16384, K <= min(N, 1024).  Point 0 is
+ * start_idx[b]; point k is the one with the largest distance to the points already chosen, distances fp32
+ * (dx*dx + dy*dy) + dz*dz with each operation rounded on its own, ties to the lowest index.  idx_out int32
+ * [batch, K], xyz_out fp32 [batch, K, 3] (the gathered points). */
+int ga_fps(const float *pcd, int batch, int N, int K, const int32_t *start_idx, int32_t *idx_out,
+           float *xyz_out, void *stream);
+/* img fp32 NCHW [n, C, H, W] -> x_bf16 NHWC [n, H, W, c_pad] (channels from C on zero; c_pad % 8 == 0), and, when
+ * token_xyz is not NULL, token_xyz fp32 ["(n ty tx)", 3] = img[:, xyz_c:xyz_c+3, off::step, off::step]. */
+int ga_vae_enc_input(const float *img, int n, int C, int H, int W, int c_pad, void *x_bf16, int xyz_c,
+                     int step, int off, float *token_xyz, void *stream);
+/* Head split for head_dim 32: qkv bf16 [R, 3 * heads * 32] ("(K H D)" columns, bias included) -> q, k per-head
+ * RMSNorm(32) (fp32, * qn_w / kn_w [32]; NULL = no norm), written zero-padded to 64 as Q, K [B, heads, tok_pitch, 64]
+ * and Vt [B, heads, 64, tok_pitch] (rows 32..63 zero), B = R / rows_per_batch: the ga_attention_bf16 layout. */
+int ga_heads32_split(const void *qkv, const float *qn_w, const float *kn_w, int R, int heads,
+                     int rows_per_batch, int tok_pitch, float eps, void *q, void *k, void *vt, void *stream);
+/* Weights of the readout head (all fp32, nn.Linear layout [out, in]). */
+typedef struct GaVaeEncHead {
+    const float *ln_w, *ln_b;       /* Mlp_out PreNorm LayerNorm [D] */
+    const float *fc1_w, *fc1_b;     /* [hid, D], [hid] */
+    const float *fc2_w, *fc2_b;     /* [2 zc, hid], [2 zc] */
+    const float *q1_w, *q1_b;       /* quant_conv fc1 [2 zc, 2 zc], [2 zc] */
+    const float *q2_w, *q2_b;       /* quant_conv fc2 [2 zc, 2 zc], [2 zc] */
+    float ln_eps;
+} GaVaeEncHead;
+/* Per token r of x fp32 [R, D]: h = fc2(gelu_tanh(fc1(LayerNorm(x)))) -> h_out [R, 2 zc]; moments =
+ * q2(gelu_tanh(q1(h))); mean = moments[:zc], logvar = 20 tanh(moments[zc:] / 20), std = exp(logvar / 2) (stdv may
+ * be NULL), latent = mean + std * noise (noise fp32 [R, zc]; NULL gives latent = mean; latent may be NULL). */
+int ga_vae_enc_head(const GaVaeEncHead *p, const float *x, const float *noise, int R, int D, int hid, int zc,
+                    float *h_out, float *mean, float *logvar, float *stdv, float *latent, void *stream);
 
 /* Measurement aid: when enabled, cudaEvents are recorded around every kernel
  * stage of the next forward/backward; ga_profile_read synchronises on them and
