@@ -28,6 +28,10 @@ class GaGemmEpilogue(C.Structure):
                 ("tok_pitch", C.c_int), ("eps", C.c_float)]
 
 
+# GaGemmEpilogue.mode: the header's GA_EPI_* (tests/test_abi.py checks them against it)
+EPI_BF16, EPI_GELU_BF16, EPI_F32, EPI_RESID_GATE_F32, EPI_HEADS, EPI_GEGLU_BF16 = 0, 1, 2, 3, 4, 5
+
+
 class GaVaeEncHead(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("ln_w", "ln_b", "fc1_w", "fc1_b", "fc2_w", "fc2_b", "q1_w", "q1_b", "q2_w",
                                           "q2_b")] + [("ln_eps", C.c_float)]

@@ -18,17 +18,15 @@ Scope: arch "vitl" at inp_size 518 only (the deployed configs); other sizes need
 gradients: the reference freezes the encoder.  Weights never come from the network: pass `state_dict=`, or place the
 upstream checkpoint file `dinov2_vitl14_reg4_pretrain.pth` under `torch.hub.get_dir()/checkpoints/`.
 """
-import ctypes as C
 import os
 import re
 
 import torch
 import torch.nn as nn
 
-from . import _lib
-from . import dit as _dit
-from ._lib import GaGemmEpilogue
-from .dit import EPI_F32, EPI_GELU_BF16, EPI_HEADS, EPI_RESID_GATE_F32, _p
+from . import _launch, _lib
+from ._launch import epilogue, gemm, ptr as _p
+from ._lib import EPI_F32, EPI_GELU_BF16, EPI_HEADS, EPI_RESID_GATE_F32
 
 D, HEADS, N_REG, PATCH, IMG_SIZE = 1024, 16, 4, 14, 518
 GRID = IMG_SIZE // PATCH                  # 37
@@ -125,7 +123,7 @@ class Dinov2Encoder:
     """DINOv2 ViT-L/14-reg4 forward at 518^2 on libga_b200.so.  `encode(img [B,3,H,W] in [-1,1])` returns
     {"x_norm_clstoken" [B,1024], "x_norm_patchtokens" [B,1369,1024]} (fp32), after the reference embedder's
     preprocess (kornia antialiased bicubic resize to 518, (x+1)/2, ImageNet normalisation)."""
-    MAX_GRAPHS = 4                 # captured (B, H, W) kept at a time (oldest dropped first)
+    use_graph = _launch.graph_switch()
 
     def __init__(self, state_dict, device="cuda:0"):
         self.L = _lib.lib()
@@ -155,22 +153,7 @@ class Dinov2Encoder:
                 ls1=f32(p + "ls1.gamma"), ls2=f32(p + "ls2.gamma"),
                 w1=b16(p + "mlp.fc1.weight"), b1=f32(p + "mlp.fc1.bias"),
                 w2=b16(p + "mlp.fc2.weight"), b2=f32(p + "mlp.fc2.bias")))
-        self.use_graph = os.environ.get("GA_B200_DINO_GRAPH", "1") != "0"
-        self._graphs = {}                  # (B, H, W) -> (graph, static image, static outputs)
-
-    # ---- launch helpers
-    def _gemm(self, A, W, M, N, K, epi, st):
-        _lib.check(self.L.ga_gemm_bf16_tn(_p(A), K, _p(W), K, M, N, K, C.byref(epi), _dit._gemm_config(M, N, epi.mode), st),
-                   "ga_gemm_bf16_tn")
-
-    @staticmethod
-    def _epi(mode, **kw):
-        e = GaGemmEpilogue()
-        e.mode = mode
-        e.eps = LN_EPS
-        for k, v in kw.items():
-            setattr(e, k, v.data_ptr() if isinstance(v, torch.Tensor) else v)
-        return e
+        self._graphs = _launch.GraphCache("GA_B200_DINO_GRAPH")          # (B, H, W) -> graph
 
     def encode(self, img, return_acts=False):
         """img [B, 3, H, W] (CUDA, any float dtype; H, W <= 4096).  The launch sequence is captured once per (B, H, W)
@@ -182,37 +165,21 @@ class Dinov2Encoder:
         if img.dim() != 4 or img.shape[1] != 3:
             raise ValueError("expected an image batch [B, 3, H, W], got %s" % (tuple(img.shape),))
         B, _, H, W = img.shape
-        dev = self.device
-        with torch.cuda.device(dev), torch.no_grad():
-            if return_acts or not self.use_graph or torch.cuda.is_current_stream_capturing():
-                x = img.to(device=dev, dtype=torch.float32).contiguous()
-                out = self._launches(x, [] if return_acts else None)
-                return {k: (v.contiguous() if isinstance(v, torch.Tensor) else v) for k, v in out.items()}
-            key = (B, H, W)
-            slot = self._graphs.get(key)
-            if slot is None:
-                while len(self._graphs) >= self.MAX_GRAPHS:
-                    self._graphs.pop(next(iter(self._graphs)))
-                with torch.inference_mode(False):
-                    s_img = torch.empty(B, 3, H, W, device=dev, dtype=torch.float32)
-                    s_img.copy_(img)
-                    self._launches(s_img)                          # warm-up: first-use kernel attributes are set here
-                    torch.cuda.synchronize(dev)
-                    g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g, capture_error_mode="thread_local"):
-                        outs = self._launches(s_img)
-                slot = self._graphs[key] = (g, s_img, outs)
-            g, s_img, outs = slot
-            s_img.copy_(img)
-            g.replay()
-            return {k: v.clone(memory_format=torch.contiguous_format) for k, v in outs.items()}
+        with torch.cuda.device(self.device), torch.no_grad():
+            x = img.to(device=self.device, dtype=torch.float32).contiguous()
+            if return_acts:
+                acts = []
+                out = {k: v.contiguous() for k, v in self._launches(x, acts).items()}
+                return dict(out, acts=acts)
+            return self._graphs.run((B, H, W), self._launches, (x,))
 
     def _launches(self, img, acts=None):
-        """The launch sequence of one encode on the current stream (eager, or under graph capture)."""
+        """The launch sequence of one encode on the current stream (eager, or under graph capture).  `acts`: a list
+        that receives the residual stream after every block."""
         L, w, dev = self.L, self.w, self.device
         B, _, H, W = img.shape
         R, H16 = B * N_TOK, HEADS
-        st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        st = _launch.stream(dev)
         z = lambda *s, dt=torch.float32: torch.empty(*s, device=dev, dtype=dt)
         bf = torch.bfloat16
         # ---- front end -> patch matrix -> patch-embed GEMM -> token assembly
@@ -222,7 +189,7 @@ class Dinov2Encoder:
         _lib.check(L.ga_dino_frontend(_p(img), B, H, W, IMG_SIZE, PATCH, _p(pm), K_PITCH, _p(scratch), nbytes, st),
                    "ga_dino_frontend")
         pe = z(B * N_PATCH, D)
-        self._gemm(pm, w["patch_w"], B * N_PATCH, D, K_PITCH, self._epi(EPI_F32, bias=w["patch_b"], out=pe, ld_out=D), st)
+        gemm(pm, w["patch_w"], B * N_PATCH, D, K_PITCH, epilogue(EPI_F32, bias=w["patch_b"], out=pe, ld_out=D), st)
         x = z(R, D)
         _lib.check(L.ga_dino_tokens(_p(pe), _p(w["cls"]), _p(w["reg"]), N_REG, _p(w["pos"]), _p(x), B, N_PATCH, D, st),
                    "ga_dino_tokens")
@@ -234,30 +201,27 @@ class Dinov2Encoder:
         for wb in self.blocks:
             _lib.check(L.ga_layernorm_modulate(_p(x), _p(wb["n1_w"]), _p(wb["n1_b"]), None, None, 0, 1, _p(h), R, D, LN_EPS,
                                                st), "norm1")
-            self._gemm(h, wb["qkv_w"], R, 3 * D, D,
-                       self._epi(EPI_HEADS, bias=wb["qkv_b"], q=qb, k=kb, vt=vtb, heads=H16, first_part=0,
-                                 tok_pitch=TOK_PITCH, rows_per_batch=N_TOK), st)
+            gemm(h, wb["qkv_w"], R, 3 * D, D,
+                 epilogue(EPI_HEADS, bias=wb["qkv_b"], q=qb, k=kb, vt=vtb, heads=H16, first_part=0,
+                          tok_pitch=TOK_PITCH, rows_per_batch=N_TOK), st)
             _lib.check(L.ga_attention_bf16(_p(qb), _p(kb), _p(vtb), _p(ao), B, H16, N_TOK, N_TOK, TOK_PITCH, TOK_PITCH,
                                            0.125, 0.0, st), "attention")
             # rows_per_batch = R: every row reads the one [D] LayerScale vector as its gate
-            self._gemm(ao, wb["proj_w"], R, D, D,
-                       self._epi(EPI_RESID_GATE_F32, bias=wb["proj_b"], out=x, ld_out=D, gate=wb["ls1"], gate_ld=D,
-                                 rows_per_batch=R), st)
+            gemm(ao, wb["proj_w"], R, D, D,
+                 epilogue(EPI_RESID_GATE_F32, bias=wb["proj_b"], out=x, ld_out=D, gate=wb["ls1"], gate_ld=D,
+                          rows_per_batch=R), st)
             _lib.check(L.ga_layernorm_modulate(_p(x), _p(wb["n2_w"]), _p(wb["n2_b"]), None, None, 0, 1, _p(h), R, D, LN_EPS,
                                                st), "norm2")
-            self._gemm(h, wb["w1"], R, 4 * D, D, self._epi(EPI_GELU_BF16, bias=wb["b1"], out=hid, ld_out=4 * D), st)
-            self._gemm(hid, wb["w2"], R, D, 4 * D,
-                       self._epi(EPI_RESID_GATE_F32, bias=wb["b2"], out=x, ld_out=D, gate=wb["ls2"], gate_ld=D,
-                                 rows_per_batch=R), st)
+            gemm(h, wb["w1"], R, 4 * D, D, epilogue(EPI_GELU_BF16, bias=wb["b1"], out=hid, ld_out=4 * D), st)
+            gemm(hid, wb["w2"], R, D, 4 * D,
+                 epilogue(EPI_RESID_GATE_F32, bias=wb["b2"], out=x, ld_out=D, gate=wb["ls2"], gate_ld=D,
+                          rows_per_batch=R), st)
             if acts is not None:
                 acts.append(x.view(B, N_TOK, D).clone())
         y = z(R, D)
         _lib.check(L.ga_layernorm_rows(_p(x), _p(w["norm_w"]), _p(w["norm_b"]), _p(y), R, D, LN_EPS, st), "final norm")
         y = y.view(B, N_TOK, D)
-        out = {"x_norm_clstoken": y[:, 0], "x_norm_patchtokens": y[:, 1 + N_REG:]}
-        if acts is not None:
-            out["acts"] = acts
-        return out
+        return {"x_norm_clstoken": y[:, 0], "x_norm_patchtokens": y[:, 1 + N_REG:]}
 
 
 def encode_flops(B=1, depth=24):

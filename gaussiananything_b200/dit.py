@@ -16,62 +16,19 @@ replayed from a CUDA graph.  There is no CPU / eager fallback.
 Precision: GEMM / attention operands bf16 (the reference runs them under bf16
 autocast), fp32 accumulation, fp32 residual stream, fp32 norms, fp32 output.
 """
-import ctypes as C
 import math
 
 import torch
 import torch.nn as nn
 
-from . import _lib
-from ._lib import GaGemmEpilogue
+from . import _launch, _lib
+from ._launch import epilogue, gemm, ptr as _p, round_up as _round_up
+from ._lib import EPI_F32, EPI_GELU_BF16, EPI_HEADS, EPI_RESID_GATE_F32
+# dit.EPI_*, dit.GaGemmEpilogue, dit._gemm_config and dit._p: earlier homes of these names, still read by tools and tests
+from ._launch import gemm_config as _gemm_config  # noqa: F401
+from ._lib import EPI_BF16, GaGemmEpilogue  # noqa: F401
 
-
-def _p(t):
-    return C.c_void_p(t.data_ptr() if t is not None else 0)
-
-
-EPI_BF16, EPI_GELU_BF16, EPI_F32, EPI_RESID_GATE_F32, EPI_HEADS = 0, 1, 2, 3, 4
 _bind = _lib.lib
-
-
-_GEMM_CFG_ENV = None
-_SMS = 132                # H100 SXM: one persistent GEMM CTA per SM
-
-
-def _gemm_config(M, N, mode=None):
-    """Tile width (ga_b200.h) from a two-term cost model checked against the H100 sweep
-    (tools/sweep_gemm.py, profiles/gemm_sweep_h100.txt):
-
-        cost(BN) = ceil(tiles(BN) / 132) * (BN + 64)
-
-    -- waves of the persistent grid times the per-tile work (the main loop scales with BN, the +64 is the fixed
-    TMA-fill / epilogue-drain share that makes wide tiles more efficient per byte).  It picks the measured winner on
-    all nine DiT shapes: 192 for 4096x768 (11.3 vs 13.1 us at 256), 4096x2304, 1536x3072 and 1536x4096, 256 for
-    4096x3072 and 2738x1536, 128 for the under-filled 1536x1024 GEMMs of the deployed size.
-    The HEADS epilogue (whole 64-wide heads per warpgroup: 128 or 256 only) stays at 128.  GA_B200_GEMM_CFG="big,small" overrides."""
-    global _GEMM_CFG_ENV
-    if _GEMM_CFG_ENV is None:
-        import os
-        _GEMM_CFG_ENV = os.environ.get("GA_B200_GEMM_CFG", "")
-    if _GEMM_CFG_ENV:
-        big, small = (int(v) for v in _GEMM_CFG_ENV.split(","))
-        return big if (M >= 1024 and N >= 512) else small
-    rows = -(-M // 128)
-    best, best_cost = 128, None
-    if mode == EPI_HEADS:
-        return 128                      # 256-wide HEADS tiles measured slower at M = 1536 (deployed qkv: +1.7 % per NFE)
-    for bn in (128, 192, 256):
-        if bn > 128 and N < bn:
-            continue
-        tiles = rows * -(-N // bn)
-        cost = -(-tiles // _SMS) * (bn + 64)
-        if best_cost is None or cost < best_cost:
-            best, best_cost = bn, cost
-    return best
-
-
-def _round_up(x, m):
-    return (x + m - 1) // m * m
 
 
 # --------------------------------------------------------------------------
@@ -398,27 +355,16 @@ class _DiTEngine:
         self._ctx_ref = None
 
     # ---- launches
-    def _gemm(self, A, W, M, N, K, epi, st, bn=None):
-        if bn is None:
-            bn = _gemm_config(M, N, epi.mode)
-        _lib.check(self.L.ga_gemm_bf16_tn(_p(A), K, _p(W), K, M, N, K, C.byref(epi), bn, st), "ga_gemm_bf16_tn")
-
-    def _epi(self, mode, **kw):
-        e = GaGemmEpilogue()
-        e.mode = mode
-        e.eps = 1e-5
-        for k, v in kw.items():
-            setattr(e, k, v.data_ptr() if isinstance(v, torch.Tensor) else v)
-        return e
+    _epi = staticmethod(epilogue)          # bench.py builds its isolated-GEMM epilogue through the engine
 
     def _context_kv(self, st):
         """Timestep-independent cross-attention K/V of every block: once per context (SURVEY.md F11)."""
         B, N, M = self._shape
         s, D, H = self.s, self.D, self.H
         for l, wb in enumerate(self.wb):
-            e = self._epi(EPI_HEADS, k=s["kc"][l], vt=s["vtc"][l], kn_w=wb["cak_n"], heads=H, first_part=1,
-                          tok_pitch=self.Mp, rows_per_batch=M)
-            self._gemm(s["ctx"], wb["cakv_w"], B * M, 2 * D, self.Dc, e, st)
+            e = epilogue(EPI_HEADS, k=s["kc"][l], vt=s["vtc"][l], kn_w=wb["cak_n"], heads=H, first_part=1,
+                         tok_pitch=self.Mp, rows_per_batch=M)
+            gemm(s["ctx"], wb["cakv_w"], B * M, 2 * D, self.Dc, e, st)
 
     def _forward_launches(self, st, cfg_scale):
         L, s, w = self.L, self.s, self.w
@@ -437,11 +383,11 @@ class _DiTEngine:
         concat = self.stage2 and not self.use_pe
         _lib.check(L.ga_embed_fc1(_p(s["x_in"]), self.Cin, _p(s["xyz_in"]) if concat else None, 3 if concat else 0,
                                   _p(w["fc1_w"]), _p(w["fc1_b"]), _p(s["e1"]), R, D, st), "embed_fc1")
-        self._gemm(s["e1"], w["fc2_w"], R, D, D, self._epi(EPI_F32, bias=w["fc2_b"], out=s["xres"], ld_out=D), st)
+        gemm(s["e1"], w["fc2_w"], R, D, D, epilogue(EPI_F32, bias=w["fc2_b"], out=s["xres"], ld_out=D), st)
         if self.use_pe:
             _lib.check(L.ga_xyz_posenc(_p(s["xyz_in"]), _p(s["pe"]), R, st), "xyz_pe")
-            self._gemm(s["pe"], w["xyz_w"], R, D, 64,
-                       self._epi(EPI_RESID_GATE_F32, bias=w["xyz_b"], out=s["xres"], ld_out=D, rows_per_batch=N), st)
+            gemm(s["pe"], w["xyz_w"], R, D, 64,
+                 epilogue(EPI_RESID_GATE_F32, bias=w["xyz_b"], out=s["xres"], ld_out=D, rows_per_batch=N), st)
         # ---- blocks
         scale = 1.0 / math.sqrt(64.0)
         for l, wb in enumerate(self.wb):
@@ -449,32 +395,31 @@ class _DiTEngine:
             ch = lambda j: mod[:, j * D:(j + 1) * D]
             # cross attention (pre-norm, residual)
             _lib.check(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["pre_w"]), None, None, 0, N, _p(s["h"]), R, D, 1e-5, st), "prenorm")
-            self._gemm(s["h"], wb["caq_w"], R, D, D,
-                       self._epi(EPI_HEADS, q=s["q"], qn_w=wb["caq_n"], heads=H, first_part=0, tok_pitch=self.Np,
-                                 rows_per_batch=N), st)
+            gemm(s["h"], wb["caq_w"], R, D, D,
+                 epilogue(EPI_HEADS, q=s["q"], qn_w=wb["caq_n"], heads=H, first_part=0, tok_pitch=self.Np,
+                          rows_per_batch=N), st)
             _lib.check(L.ga_attention_bf16(_p(s["q"]), _p(s["kc"][l]), _p(s["vtc"][l]), _p(s["ao"]), B, H, N, M, self.Np,
                                            self.Mp, scale, wb["ca_bound"], st), "cross attention")
-            self._gemm(s["ao"], wb["cao_w"], R, D, D,
-                       self._epi(EPI_RESID_GATE_F32, bias=wb["cao_b"], out=s["xres"], ld_out=D, rows_per_batch=N), st)
+            gemm(s["ao"], wb["cao_w"], R, D, D,
+                 epilogue(EPI_RESID_GATE_F32, bias=wb["cao_b"], out=s["xres"], ld_out=D, rows_per_batch=N), st)
             # gated self attention
             _lib.check(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["n1_w"]), _p(ch(0)), _p(ch(1)), 6 * D, N, _p(s["h"]), R, D,
                                              1e-5, st), "norm1")
-            self._gemm(s["h"], wb["qkv_w"], R, 3 * D, D,
-                       self._epi(EPI_HEADS, bias=wb["qkv_b"], q=s["q"], k=s["k"], vt=s["vt"], qn_w=wb["q_n"],
-                                 kn_w=wb["k_n"], heads=H, first_part=0, tok_pitch=self.Np, rows_per_batch=N), st)
+            gemm(s["h"], wb["qkv_w"], R, 3 * D, D,
+                 epilogue(EPI_HEADS, bias=wb["qkv_b"], q=s["q"], k=s["k"], vt=s["vt"], qn_w=wb["q_n"],
+                          kn_w=wb["k_n"], heads=H, first_part=0, tok_pitch=self.Np, rows_per_batch=N), st)
             _lib.check(L.ga_attention_bf16(_p(s["q"]), _p(s["k"]), _p(s["vt"]), _p(s["ao"]), B, H, N, N, self.Np, self.Np,
                                            scale, wb["sa_bound"], st), "self attention")
-            self._gemm(s["ao"], wb["proj_w"], R, D, D,
-                       self._epi(EPI_RESID_GATE_F32, bias=wb["proj_b"], out=s["xres"], ld_out=D, gate=ch(2),
-                                 gate_ld=6 * D, rows_per_batch=N), st)
+            gemm(s["ao"], wb["proj_w"], R, D, D,
+                 epilogue(EPI_RESID_GATE_F32, bias=wb["proj_b"], out=s["xres"], ld_out=D, gate=ch(2),
+                          gate_ld=6 * D, rows_per_batch=N), st)
             # gated FFN
             _lib.check(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["n2_w"]), _p(ch(3)), _p(ch(4)), 6 * D, N, _p(s["h"]), R, D,
                                              1e-5, st), "norm2")
-            self._gemm(s["h"], wb["w1"], R, 4 * D, D,
-                       self._epi(EPI_GELU_BF16, bias=wb["b1"], out=s["hid"], ld_out=4 * D), st)
-            self._gemm(s["hid"], wb["w2"], R, D, 4 * D,
-                       self._epi(EPI_RESID_GATE_F32, bias=wb["b2"], out=s["xres"], ld_out=D, gate=ch(5),
-                                 gate_ld=6 * D, rows_per_batch=N), st)
+            gemm(s["h"], wb["w1"], R, 4 * D, D, epilogue(EPI_GELU_BF16, bias=wb["b1"], out=s["hid"], ld_out=4 * D), st)
+            gemm(s["hid"], wb["w2"], R, D, 4 * D,
+                 epilogue(EPI_RESID_GATE_F32, bias=wb["b2"], out=s["xres"], ld_out=D, gate=ch(5),
+                          gate_ld=6 * D, rows_per_batch=N), st)
             if self.tap_blocks:
                 s["taps"][l].copy_(s["xres"])
         # ---- final layer (+ CFG combine)
@@ -541,9 +486,7 @@ class _DiTEngine:
         if self.tap_blocks and "taps" not in s:
             with torch.inference_mode(False):
                 s["taps"] = torch.zeros(self.depth, B * N, self.D, device=self.device)
-        dev = self.device
-        stream = torch.cuda.current_stream(dev)
-        st = C.c_void_p(stream.cuda_stream)
+        st = _launch.stream(self.device)
         s["x_in"].copy_(x.reshape(B, N, self.Cin).to(torch.float32))
         s["t_in"].copy_(t.reshape(-1).to(torch.float32).expand(B) if t.numel() == 1 else t.reshape(B).to(torch.float32))
         s["vec_in"].copy_(vec.reshape(B, self.Dc).to(torch.float32))
@@ -557,13 +500,7 @@ class _DiTEngine:
         gkey = (cfg_scale, self.tap_blocks)
         if self.use_graph:
             if self._graph is None or self._graph[0] != gkey:
-                # warm-up run (sets kernel attributes), then capture the same launch sequence
-                self._forward_launches(st, cfg_scale)
-                torch.cuda.synchronize(dev)
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    cst = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-                    self._forward_launches(cst, cfg_scale)
+                g, _ = _launch.capture(lambda: self._forward_launches(_launch.stream(self.device), cfg_scale), self.device)
                 self._graph = (gkey, g)
             self._graph[1].replay()
         else:

@@ -11,20 +11,16 @@ Mirrors what the reference's deployed decoder class does between DiT sampling an
 (wgmma GEMMs with fused epilogues, wgmma attention for the DiT2 blocks, one-warp-per-sequence attention for the
 up-samplers' micro-sequences, row kernels).  bf16 tensor-core operands, fp32 residual streams.  No CPU fallback.
 """
-import ctypes as C
-import os
-
 import torch
 
-from . import _lib
-from . import dit as _dit
-from ._lib import GaGemmEpilogue
-from .dit import EPI_BF16, EPI_F32, EPI_GELU_BF16, EPI_HEADS, EPI_RESID_GATE_F32, _p, _round_up
+from . import _launch, _lib
+from ._launch import epilogue, gemm, ptr as _p, round_up as _round_up
+from ._lib import EPI_BF16, EPI_F32, EPI_GELU_BF16, EPI_HEADS, EPI_RESID_GATE_F32
 
 
 class SurfelDecoder:
     CASCADE = (("ada_CA_f4_1", 8), ("ada_CA_f4_2", 4), ("ada_CA_f4_3", 3))
-    MAX_GRAPHS = 4                 # captured batch sizes kept at a time (oldest dropped first)
+    use_graph = _launch.graph_switch()
 
     def __init__(self, state_dict, num_heads, depth, scene_max=0.45, skip_weight=0.1, device="cuda:0"):
         self.L = _lib.lib()
@@ -78,8 +74,8 @@ class SurfelDecoder:
                                     h_w=f32(p + "gaussian_residual_pred.fn.weight"),
                                     h_b=f32(p + "gaussian_residual_pred.fn.bias")))
         self.w = w
-        self.use_graph = os.environ.get("GA_B200_VAE_GRAPH", "1") != "0"
-        self._graphs = {}                                  # batch size -> (graph, static latent, static xyz, static outputs)
+        # batch size -> graph; each graph owns its activations (GBs at the deployed size)
+        self._graphs = _launch.GraphCache("GA_B200_VAE_GRAPH")
 
     @staticmethod
     def _attn_mlp(pa, pm, f32, b16):
@@ -88,20 +84,6 @@ class SurfelDecoder:
                     proj_w=b16(pa + "proj.weight"), proj_b=f32(pa + "proj.bias"),
                     w1=b16(pm + "mlp.0.weight"), b1=f32(pm + "mlp.1.bias"), w2=b16(pm + "mlp.2.weight"), b2=f32(pm + "mlp.3.bias"),
                     bound=8.16 * float(qn.abs().max()) * float(kn.abs().max()))
-
-    # ---- launch helpers
-    def _gemm(self, A, W, M, N, K, epi, st):
-        _lib.check(self.L.ga_gemm_bf16_tn(_p(A), K, _p(W), K, M, N, K, C.byref(epi), _dit._gemm_config(M, N, epi.mode), st),
-                   "ga_gemm_bf16_tn")
-
-    @staticmethod
-    def _epi(mode, **kw):
-        e = GaGemmEpilogue()
-        e.mode = mode
-        e.eps = 1e-5
-        for k, v in kw.items():
-            setattr(e, k, v.data_ptr() if isinstance(v, torch.Tensor) else v)
-        return e
 
     def decode(self, latent_normalized, query_pcd_xyz):
         """latent_normalized [B, N, Cz], query_pcd_xyz [B, N, 3] (CUDA).  Returns the reference's ret_dict entries.
@@ -115,31 +97,9 @@ class SurfelDecoder:
         B, N, zc = latent_normalized.shape
         assert N == self.N and zc == self.zc and query_pcd_xyz.shape == (B, N, 3)
         with torch.cuda.device(dev):               # launches go to the decoder's device, not the process's current one
-            if not self.use_graph or torch.cuda.is_current_stream_capturing():
-                return self._aliases(self._decode_launches(latent_normalized, query_pcd_xyz))
-            slot = self._graphs.get(B)
-            if slot is None:
-                while len(self._graphs) >= self.MAX_GRAPHS:        # each graph owns its activations (GBs at the deployed size)
-                    self._graphs.pop(next(iter(self._graphs)))
-                # buffers and graph are created outside inference_mode so that later calls may come from either mode
-                with torch.inference_mode(False), torch.no_grad():
-                    s_lat = torch.empty(B, N, zc, device=dev, dtype=torch.float32)
-                    s_xyz = torch.empty(B, N, 3, device=dev, dtype=torch.float32)
-                    s_lat.copy_(latent_normalized)
-                    s_xyz.copy_(query_pcd_xyz)
-                    self._decode_launches(s_lat, s_xyz)            # warm-up: first-use kernel attributes are set here
-                    torch.cuda.synchronize(dev)
-                    g = torch.cuda.CUDAGraph()
-                    # thread_local: another thread of the process (NCCL's watchdog under torch.distributed) may issue
-                    # CUDA calls while this one captures
-                    with torch.cuda.graph(g, capture_error_mode="thread_local"):
-                        outs = self._decode_launches(s_lat, s_xyz)
-                slot = self._graphs[B] = (g, s_lat, s_xyz, outs)
-            g, s_lat, s_xyz, outs = slot
-            s_lat.copy_(latent_normalized)
-            s_xyz.copy_(query_pcd_xyz)
-            g.replay()
-            return self._aliases({k: v.clone() for k, v in outs.items()})
+            lat = latent_normalized.to(device=dev, dtype=torch.float32).contiguous()
+            xyz = query_pcd_xyz.to(device=dev, dtype=torch.float32).contiguous()
+            return self._aliases(self._graphs.run(B, self._decode_launches, (lat, xyz)))
 
     @staticmethod
     def _aliases(out):
@@ -153,22 +113,22 @@ class SurfelDecoder:
         L, w, dev = self.L, self.w, self.device
         B, N, zc = latent_normalized.shape
         D, H, R, dep = self.D, self.H, B * N, self.depth
-        st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        st = _launch.stream(dev)
         z = lambda *s, dt=torch.float32: torch.empty(*s, device=dev, dtype=dt)
         bf = torch.bfloat16
-        lat = latent_normalized.reshape(R, zc).contiguous().float()
-        xyz = query_pcd_xyz.reshape(R, 3).contiguous().float()
+        lat = latent_normalized.reshape(R, zc)
+        xyz = query_pcd_xyz.reshape(R, 3)
         # ---- post_quant_conv
         h0 = z(R, self.pq_k, dt=bf)
         _lib.check(L.ga_embed_fc1(_p(lat), zc, None, 0, _p(w["pq_w1"]), _p(w["pq_b1"]), _p(h0), R, self.pq_k, st), "post_quant fc1")
         c = z(R, D)
-        self._gemm(h0, w["pq_w2"], R, D, self.pq_k, self._epi(EPI_F32, bias=w["pq_b2"], out=c, ld_out=D), st)
+        gemm(h0, w["pq_w2"], R, D, self.pq_k, epilogue(EPI_F32, bias=w["pq_b2"], out=c, ld_out=D), st)
         # ---- DiT2: per-token adaLN tables of every block in one GEMM on silu(c)
         cs = z(R, D, dt=bf)
         _lib.check(L.ga_silu_to_bf16(_p(c), _p(cs), R * D, st), "silu")
         MW = dep * 6 * D
         mod = z(R, MW)
-        self._gemm(cs, w["ada_w"], R, MW, D, self._epi(EPI_F32, bias=w["ada_b"], out=mod, ld_out=MW), st)
+        gemm(cs, w["ada_w"], R, MW, D, epilogue(EPI_F32, bias=w["ada_b"], out=mod, ld_out=MW), st)
         x = w["pos"].repeat(B, 1).contiguous()                                           # [R, D] residual stream
         Np = _round_up(N, 128)
         h, ao, hid = z(R, D, dt=bf), z(R, D, dt=bf), z(R, 4 * D, dt=bf)
@@ -178,18 +138,18 @@ class SurfelDecoder:
         for l, wb in enumerate(self.blocks):
             ch = lambda j: mod[:, (l * 6 + j) * D:(l * 6 + j + 1) * D]
             _lib.check(L.ga_layernorm_modulate(_p(x), None, None, _p(ch(0)), _p(ch(1)), MW, 1, _p(h), R, D, 1e-6, st), "norm1")
-            self._gemm(h, wb["qkv_w"], R, 3 * D, D,
-                       self._epi(EPI_HEADS, bias=wb["qkv_b"], q=qb, k=kb, vt=vtb, qn_w=wb["q_n"], kn_w=wb["k_n"], heads=H,
-                                 first_part=0, tok_pitch=Np, rows_per_batch=N), st)
+            gemm(h, wb["qkv_w"], R, 3 * D, D,
+                 epilogue(EPI_HEADS, bias=wb["qkv_b"], q=qb, k=kb, vt=vtb, qn_w=wb["q_n"], kn_w=wb["k_n"], heads=H,
+                          first_part=0, tok_pitch=Np, rows_per_batch=N), st)
             _lib.check(L.ga_attention_bf16(_p(qb), _p(kb), _p(vtb), _p(ao), B, H, N, N, Np, Np, 0.125, wb["bound"], st), "attention")
-            self._gemm(ao, wb["proj_w"], R, D, D,
-                       self._epi(EPI_RESID_GATE_F32, bias=wb["proj_b"], out=x, ld_out=D, gate=ch(2), gate_ld=MW,
-                                 rows_per_batch=1), st)
+            gemm(ao, wb["proj_w"], R, D, D,
+                 epilogue(EPI_RESID_GATE_F32, bias=wb["proj_b"], out=x, ld_out=D, gate=ch(2), gate_ld=MW,
+                          rows_per_batch=1), st)
             _lib.check(L.ga_layernorm_modulate(_p(x), None, None, _p(ch(3)), _p(ch(4)), MW, 1, _p(h), R, D, 1e-6, st), "norm2")
-            self._gemm(h, wb["w1"], R, 4 * D, D, self._epi(EPI_GELU_BF16, bias=wb["b1"], out=hid, ld_out=4 * D), st)
-            self._gemm(hid, wb["w2"], R, D, 4 * D,
-                       self._epi(EPI_RESID_GATE_F32, bias=wb["b2"], out=x, ld_out=D, gate=ch(5), gate_ld=MW,
-                                 rows_per_batch=1), st)
+            gemm(h, wb["w1"], R, 4 * D, D, epilogue(EPI_GELU_BF16, bias=wb["b1"], out=hid, ld_out=4 * D), st)
+            gemm(hid, wb["w2"], R, D, 4 * D,
+                 epilogue(EPI_RESID_GATE_F32, bias=wb["b2"], out=x, ld_out=D, gate=ch(5), gate_ld=MW,
+                          rows_per_batch=1), st)
         # ---- base surfels
         base_pre = z(R, 13)
         _lib.check(L.ga_thin_linear(_p(x), None, None, 1, _p(w["sr_w"]), _p(w["sr_b"]), _p(base_pre), R, D, 13, 0.0, st), "conv_sr")
@@ -209,14 +169,14 @@ class SurfelDecoder:
             hs, qkv, aos, hids = z(Ms, D, dt=bf), z(Ms, 3 * D, dt=bf), z(Ms, D, dt=bf), z(Ms, 4 * D, dt=bf)
             for lw in stg["layers"]:
                 _lib.check(L.ga_layernorm_modulate(_p(seq), _p(lw["n1_w"]), _p(lw["n1_b"]), None, None, 0, 1, _p(hs), Ms, D, 1e-5, st), "sr norm1")
-                self._gemm(hs, lw["qkv_w"], Ms, 3 * D, D, self._epi(EPI_BF16, bias=lw["qkv_b"], out=qkv, ld_out=3 * D), st)
+                gemm(hs, lw["qkv_w"], Ms, 3 * D, D, epilogue(EPI_BF16, bias=lw["qkv_b"], out=qkv, ld_out=3 * D), st)
                 _lib.check(L.ga_micro_attention_bf16(_p(qkv), _p(lw["q_n"]), _p(lw["k_n"]), _p(aos), S, Lq, H, 1e-5, st), "micro attention")
-                self._gemm(aos, lw["proj_w"], Ms, D, D,
-                           self._epi(EPI_RESID_GATE_F32, bias=lw["proj_b"], out=seq, ld_out=D, rows_per_batch=1), st)
+                gemm(aos, lw["proj_w"], Ms, D, D,
+                     epilogue(EPI_RESID_GATE_F32, bias=lw["proj_b"], out=seq, ld_out=D, rows_per_batch=1), st)
                 _lib.check(L.ga_layernorm_modulate(_p(seq), _p(lw["n2_w"]), _p(lw["n2_b"]), None, None, 0, 1, _p(hs), Ms, D, 1e-5, st), "sr norm2")
-                self._gemm(hs, lw["w1"], Ms, 4 * D, D, self._epi(EPI_GELU_BF16, bias=lw["b1"], out=hids, ld_out=4 * D), st)
-                self._gemm(hids, lw["w2"], Ms, D, 4 * D,
-                           self._epi(EPI_RESID_GATE_F32, bias=lw["b2"], out=seq, ld_out=D, rows_per_batch=1), st)
+                gemm(hs, lw["w1"], Ms, 4 * D, D, epilogue(EPI_GELU_BF16, bias=lw["b1"], out=hids, ld_out=4 * D), st)
+                gemm(hids, lw["w2"], Ms, D, 4 * D,
+                     epilogue(EPI_RESID_GATE_F32, bias=lw["b2"], out=seq, ld_out=D, rows_per_batch=1), st)
             res = z(Ms, 13)
             _lib.check(L.ga_thin_linear(_p(seq), _p(stg["hn_w"]), _p(stg["hn_b"]), 0, _p(stg["h_w"]), _p(stg["h_b"]), _p(res), Ms, D, 13,
                                         1e-5, st), "residual head")

@@ -15,16 +15,12 @@ vit.vit_triplane...vae_reparameterization (/root/reference/vit/vit_triplane.py:1
 Activations are NHWC; bf16 tensor-core operands, fp32 accumulation, fp32 residual streams and norms.  No CPU fallback.
 """
 import ctypes as C
-import os
 
 import torch
 
-from . import _lib
-from . import dit as _dit
-from ._lib import GaGemmEpilogue, GaVaeEncHead
-from .dit import EPI_BF16, EPI_F32, EPI_GELU_BF16, EPI_HEADS, EPI_RESID_GATE_F32, _p, _round_up
-
-EPI_GEGLU_BF16 = 5
+from . import _launch, _lib
+from ._launch import epilogue, gemm, ptr as _p, round_up as _round_up
+from ._lib import EPI_BF16, EPI_F32, EPI_GEGLU_BF16, EPI_GELU_BF16, EPI_HEADS, EPI_RESID_GATE_F32, GaVaeEncHead
 
 
 def _expected_keys(ch=64, ch_mult=(1, 2, 4, 4), in_channels=15, z_channels=10, srt_depth=3, heads=8, d_head=64):
@@ -111,7 +107,7 @@ class Posterior:
 
 
 class SurfelEncoder:
-    MAX_GRAPHS = 4
+    use_graph = _launch.graph_switch()
 
     def __init__(self, state_dict, num_frames=8, latent_num=768, ch=64, ch_mult=(1, 2, 4, 4), in_channels=15,
                  z_channels=10, device="cuda:0"):
@@ -209,24 +205,9 @@ class SurfelEncoder:
                            q2_b=f32(q + "fc2.bias"))
         self.head = GaVaeEncHead(**{k: v.data_ptr() for k, v in self.head_t.items()}, ln_eps=1e-5)
         self.head_hid = self.head_t["fc1_w"].shape[0]
-        self.use_graph = os.environ.get("GA_B200_VAE_ENC_GRAPH", "1") != "0"
-        self._graphs = {}
+        self._graphs = _launch.GraphCache("GA_B200_VAE_ENC_GRAPH")          # (B, V, H, W, N) -> graph
 
     # ---- launch helpers
-    def _gemm(self, A, W, M, N, K, epi, st):
-        _lib.check(self.L.ga_gemm_bf16_tn(_p(A), K, _p(W), K, M, N, K, C.byref(epi), _dit._gemm_config(M, N, epi.mode), st),
-                   "ga_gemm_bf16_tn")
-
-    @staticmethod
-    def _epi(mode, **kw):
-        e = GaGemmEpilogue()
-        e.mode = mode
-        e.eps = 1e-5
-        e.rows_per_batch = 1
-        for k, v in kw.items():
-            setattr(e, k, v.data_ptr() if isinstance(v, torch.Tensor) else v)
-        return e
-
     def _conv(self, x, n, H, W, cin, cv, stride, st, residual=None, out_bf16=False, out_f32=True):
         Ho, Wo = self.L.ga_conv3x3_out_size(H, stride), self.L.ga_conv3x3_out_size(W, stride)
         M = n * Ho * Wo
@@ -236,10 +217,10 @@ class SurfelEncoder:
                                           _p(residual), _p(of), _p(ob), st), "ga_conv3x3_bf16")
         return of, ob, Ho, Wo
 
-    def _gn(self, x, w, b, n, HW, Cc, silu, st, bf16=True):
+    def _gn(self, x, w, b, n, HW, Cc, silu, scratch, st, bf16=True):
         out = torch.empty(n * HW, Cc, device=self.device, dtype=torch.bfloat16 if bf16 else torch.float32)
         _lib.check(self.L.ga_group_norm_nhwc(_p(x), _p(w), _p(b), n, HW, Cc, 1e-6, int(silu), _p(out), int(bf16),
-                                             _p(self._gn_scratch), self._gn_scratch.numel(), st), "ga_group_norm_nhwc")
+                                             _p(scratch), scratch.numel(), st), "ga_group_norm_nhwc")
         return out
 
     def _bf16(self, x, st):
@@ -247,17 +228,17 @@ class SurfelEncoder:
         _lib.check(self.L.ga_f32_to_bf16(_p(x), _p(y), x.numel(), st), "f32_to_bf16")
         return y
 
-    def _resblock(self, r, x, n, H, W, st):
+    def _resblock(self, r, x, n, H, W, gn_scratch, st):
         """x fp32 NHWC [n*H*W, Cin] -> (fp32, bf16) [n*H*W, Cout]"""
         cin, cout = x.shape[1], r["c1"]["cout"]
-        a = self._gn(x, r["n1w"], r["n1b"], n, H * W, cin, True, st)
+        a = self._gn(x, r["n1w"], r["n1b"], n, H * W, cin, True, gn_scratch, st)
         h, _, _, _ = self._conv(a, n, H, W, cin, r["c1"], 1, st)
-        a2 = self._gn(h, r["n2w"], r["n2b"], n, H * W, cout, True, st)
+        a2 = self._gn(h, r["n2w"], r["n2b"], n, H * W, cout, True, gn_scratch, st)
         res = x
         if "nin_w" in r:
             res = torch.empty(n * H * W, cout, device=self.device)
-            self._gemm(self._bf16(x, st), r["nin_w"], n * H * W, cout, cin,
-                       self._epi(EPI_F32, bias=r["nin_b"], out=res, ld_out=cout), st)
+            gemm(self._bf16(x, st), r["nin_w"], n * H * W, cout, cin,
+                 epilogue(EPI_F32, bias=r["nin_b"], out=res, ld_out=cout), st)
         of, ob, _, _ = self._conv(a2, n, H, W, cout, r["c2"], 1, st, residual=res, out_bf16=True)
         return of, ob
 
@@ -268,21 +249,21 @@ class SurfelEncoder:
         Np = _round_up(rows_per_batch, 128)
         z = lambda *s: torch.zeros(*s, device=self.device, dtype=torch.bfloat16)
         qb, kb, vt = z(nb * H, Np, 64), z(nb * H, Np, 64), z(nb * H, 64, Np)
-        self._gemm(hln, qkv_w, R, 3 * inner, inner,
-                   self._epi(EPI_HEADS, q=qb, k=kb, vt=vt, heads=H, first_part=0, tok_pitch=Np,
-                             rows_per_batch=rows_per_batch), st)
+        gemm(hln, qkv_w, R, 3 * inner, inner,
+             epilogue(EPI_HEADS, q=qb, k=kb, vt=vt, heads=H, first_part=0, tok_pitch=Np,
+                      rows_per_batch=rows_per_batch), st)
         ao = torch.empty(R, inner, device=self.device, dtype=torch.bfloat16)
         _lib.check(self.L.ga_attention_bf16(_p(qb), _p(kb), _p(vt), _p(ao), nb, H, rows_per_batch, rows_per_batch, Np, Np,
                                             0.125, 0.0, st), "attention")
-        self._gemm(ao, out_w, R, inner, inner, self._epi(EPI_RESID_GATE_F32, bias=out_b, out=resid, ld_out=inner), st)
+        gemm(ao, out_w, R, inner, inner, epilogue(EPI_RESID_GATE_F32, bias=out_b, out=resid, ld_out=inner), st)
 
-    def _attn_1(self, x, n, H, W, st):
+    def _attn_1(self, x, n, H, W, gn_scratch, st):
         """SpatialTransformer3D, in place on x (fp32 NHWC [n*H*W, D])"""
         m, D, inner = self.mv, self.D, self.inner
         R, HW = n * H * W, H * W
-        g = self._gn(x, m["gn_w"], m["gn_b"], n, HW, D, False, st)
+        g = self._gn(x, m["gn_w"], m["gn_b"], n, HW, D, False, gn_scratch, st)
         t = torch.empty(R, inner, device=self.device)
-        self._gemm(g, m["pin_w"], R, inner, D, self._epi(EPI_F32, bias=m["pin_b"], out=t, ld_out=inner), st)
+        gemm(g, m["pin_w"], R, inner, D, epilogue(EPI_F32, bias=m["pin_b"], out=t, ld_out=inner), st)
         hln = torch.empty(R, inner, device=self.device, dtype=torch.bfloat16)
         L = self.L
         for j, rpb in enumerate((self.V * HW, HW)):                 # attn1: all views' tokens; attn2: per view
@@ -293,10 +274,10 @@ class SurfelEncoder:
                                            st), "norm3")
         hid = m["ff_hid"]
         ff = torch.empty(R, hid, device=self.device, dtype=torch.bfloat16)
-        self._gemm(hln, m["ff1_w"], R, 2 * hid, inner, self._epi(EPI_GEGLU_BF16, bias=m["ff1_b"], out=ff, ld_out=hid), st)
-        self._gemm(ff, m["ff2_w"], R, inner, hid, self._epi(EPI_RESID_GATE_F32, bias=m["ff2_b"], out=t, ld_out=inner), st)
-        self._gemm(self._bf16(t, st), m["pout_w"], R, D, inner,
-                   self._epi(EPI_RESID_GATE_F32, bias=m["pout_b"], out=x, ld_out=D), st)
+        gemm(hln, m["ff1_w"], R, 2 * hid, inner, epilogue(EPI_GEGLU_BF16, bias=m["ff1_b"], out=ff, ld_out=hid), st)
+        gemm(ff, m["ff2_w"], R, inner, hid, epilogue(EPI_RESID_GATE_F32, bias=m["ff2_b"], out=t, ld_out=inner), st)
+        gemm(self._bf16(t, st), m["pout_w"], R, D, inner,
+             epilogue(EPI_RESID_GATE_F32, bias=m["pout_b"], out=x, ld_out=D), st)
         return x
 
     def _launches(self, img, pcd, start_idx, noise, acts=None):
@@ -304,31 +285,31 @@ class SurfelEncoder:
         n, cin, H, W = img.shape
         B = n // V
         Np = pcd.shape[1]
-        st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        self._gn_scratch = torch.empty(L.ga_group_norm_scratch_bytes(n, H * W), device=dev, dtype=torch.uint8)
+        st = _launch.stream(dev)
+        gn_scratch = torch.empty(L.ga_group_norm_scratch_bytes(n, H * W), device=dev, dtype=torch.uint8)
         Ht, Wt = (H - 4 + 7) // 8, (W - 4 + 7) // 8
         xin = torch.empty(n * H * W, self.cin_p, device=dev, dtype=torch.bfloat16)
         txyz = torch.empty(n * Ht * Wt, 3, device=dev)
         _lib.check(L.ga_vae_enc_input(_p(img), n, cin, H, W, self.cin_p, _p(xin), cin - 3, 8, 4, _p(txyz), st), "input")
         x, _, _, _ = self._conv(xin, n, H, W, self.cin_p, self.conv_in, 1, st)
         for i, lv in enumerate(self.levels):
-            x, xb = self._resblock(lv["block"], x, n, H, W, st)
+            x, xb = self._resblock(lv["block"], x, n, H, W, gn_scratch, st)
             if acts is not None:
                 acts["level%d" % i] = (x, H, W)
             if "down" in lv:
                 x, _, H, W = self._conv(xb, n, H, W, x.shape[1], lv["down"], 2, st)
         assert H * W == Ht * Wt, "token xyz grid %dx%d does not match the feature map %dx%d" % (Ht, Wt, H, W)
-        x, _ = self._resblock(self.mid1, x, n, H, W, st)
-        x = self._attn_1(x, n, H, W, st)
+        x, _ = self._resblock(self.mid1, x, n, H, W, gn_scratch, st)
+        x = self._attn_1(x, n, H, W, gn_scratch, st)
         if acts is not None:
             acts["attn_1"] = (x.clone(), H, W)
-        x, _ = self._resblock(self.mid2, x, n, H, W, st)
+        x, _ = self._resblock(self.mid2, x, n, H, W, gn_scratch, st)
         R = n * H * W
-        tok = self._gn(x, self.norm_out[0], self.norm_out[1], n, H * W, D, True, st, bf16=False)
+        tok = self._gn(x, self.norm_out[0], self.norm_out[1], n, H * W, D, True, gn_scratch, st, bf16=False)
         # ---- readout: tokens "(B V H W) C" are the NHWC rows as they stand
         pe = torch.empty(R, 64, device=dev, dtype=torch.bfloat16)
         _lib.check(L.ga_xyz_posenc(_p(txyz), _p(pe), R, st), "token posenc")
-        self._gemm(pe, self.xyz_w, R, D, 64, self._epi(EPI_RESID_GATE_F32, bias=self.xyz_b, out=tok, ld_out=D), st)
+        gemm(pe, self.xyz_w, R, D, 64, epilogue(EPI_RESID_GATE_F32, bias=self.xyz_b, out=tok, ld_out=D), st)
         qidx = torch.empty(B, K, device=dev, dtype=torch.int32)
         qxyz = torch.empty(B, K, 3, device=dev)
         _lib.check(L.ga_fps(_p(pcd), B, Np, K, _p(start_idx), _p(qidx), _p(qxyz), st), "fps")
@@ -336,21 +317,20 @@ class SurfelEncoder:
         qpe = torch.empty(RQ, 64, device=dev, dtype=torch.bfloat16)
         _lib.check(L.ga_xyz_posenc(_p(qxyz), _p(qpe), RQ, st), "query posenc")
         qh = torch.empty(RQ, D, device=dev, dtype=torch.bfloat16)
-        self._gemm(qpe, self.xyz_w, RQ, D, 64, self._epi(EPI_BF16, bias=self.xyz_b, out=qh, ld_out=D), st)
+        gemm(qpe, self.xyz_w, RQ, D, 64, epilogue(EPI_BF16, bias=self.xyz_b, out=qh, ld_out=D), st)
         a, inner, Hh = self.agg, self.inner, self.inner // 64
         Lk = V * H * W
         PQ, PK = _round_up(K, 128), _round_up(Lk, 128)
         zb = lambda *s: torch.zeros(*s, device=dev, dtype=torch.bfloat16)
         qb, kb, vt = zb(B * Hh, PQ, 64), zb(B * Hh, PK, 64), zb(B * Hh, 64, PK)
-        self._gemm(qh, a["q_w"], RQ, inner, D, self._epi(EPI_HEADS, q=qb, qn_w=a["q_n"], heads=Hh, first_part=0,
-                                                         tok_pitch=PQ, rows_per_batch=K), st)
-        self._gemm(self._bf16(tok, st), a["kv_w"], R, 2 * inner, D,
-                   self._epi(EPI_HEADS, k=kb, vt=vt, kn_w=a["k_n"], heads=Hh, first_part=1, tok_pitch=PK, rows_per_batch=Lk),
-                   st)
+        gemm(qh, a["q_w"], RQ, inner, D, epilogue(EPI_HEADS, q=qb, qn_w=a["q_n"], heads=Hh, first_part=0,
+                                                   tok_pitch=PQ, rows_per_batch=K), st)
+        gemm(self._bf16(tok, st), a["kv_w"], R, 2 * inner, D,
+             epilogue(EPI_HEADS, k=kb, vt=vt, kn_w=a["k_n"], heads=Hh, first_part=1, tok_pitch=PK, rows_per_batch=Lk), st)
         ao = torch.empty(RQ, inner, device=dev, dtype=torch.bfloat16)
         _lib.check(L.ga_attention_bf16(_p(qb), _p(kb), _p(vt), _p(ao), B, Hh, K, Lk, PQ, PK, 0.125, a["bound"], st), "agg_ca")
         xs = torch.empty(RQ, D, device=dev)
-        self._gemm(ao, a["out_w"], RQ, D, inner, self._epi(EPI_F32, bias=a["out_b"], out=xs, ld_out=D), st)
+        gemm(ao, a["out_w"], RQ, D, inner, epilogue(EPI_F32, bias=a["out_b"], out=xs, ld_out=D), st)
         if acts is not None:
             acts["agg_ca"] = xs.clone()
         # ---- SRT blocks (heads of 32, padded to 64 for the attention kernel)
@@ -360,21 +340,19 @@ class SurfelEncoder:
             qkv = torch.empty(RQ, 3 * D, device=dev, dtype=torch.bfloat16)
             _lib.check(L.ga_layernorm_modulate(_p(xs), _p(blk["n1w"]), _p(blk["n1b"]), None, None, 0, 1, _p(hs), RQ, D, 1e-5,
                                                st), "srt norm1")
-            self._gemm(hs, blk["qkv_w"], RQ, 3 * D, D, self._epi(EPI_BF16, bias=blk["qkv_b"], out=qkv, ld_out=3 * D), st)
+            gemm(hs, blk["qkv_w"], RQ, 3 * D, D, epilogue(EPI_BF16, bias=blk["qkv_b"], out=qkv, ld_out=3 * D), st)
             sq, sk, sv = zb(B * nh, PQ, 64), zb(B * nh, PQ, 64), zb(B * nh, 64, PQ)
             _lib.check(L.ga_heads32_split(_p(qkv), _p(blk["q_n"]), _p(blk["k_n"]), RQ, nh, K, PQ, 1e-5, _p(sq), _p(sk),
                                           _p(sv), st), "heads32")
             so = torch.empty(RQ, nh * 64, device=dev, dtype=torch.bfloat16)
             _lib.check(L.ga_attention_bf16(_p(sq), _p(sk), _p(sv), _p(so), B, nh, K, K, PQ, PQ, 32 ** -0.5, 0.0, st),
                        "srt attention")
-            self._gemm(so, blk["proj_w"], RQ, D, nh * 64, self._epi(EPI_RESID_GATE_F32, bias=blk["proj_b"], out=xs, ld_out=D),
-                       st)
+            gemm(so, blk["proj_w"], RQ, D, nh * 64, epilogue(EPI_RESID_GATE_F32, bias=blk["proj_b"], out=xs, ld_out=D), st)
             _lib.check(L.ga_layernorm_modulate(_p(xs), _p(blk["n2w"]), _p(blk["n2b"]), None, None, 0, 1, _p(hs), RQ, D, 1e-5,
                                                st), "srt norm2")
             hid = torch.empty(RQ, blk["w1"].shape[0], device=dev, dtype=torch.bfloat16)
-            self._gemm(hs, blk["w1"], RQ, hid.shape[1], D, self._epi(EPI_GELU_BF16, bias=blk["b1"], out=hid, ld_out=hid.shape[1]),
-                       st)
-            self._gemm(hid, blk["w2"], RQ, D, hid.shape[1], self._epi(EPI_RESID_GATE_F32, bias=blk["b2"], out=xs, ld_out=D), st)
+            gemm(hs, blk["w1"], RQ, hid.shape[1], D, epilogue(EPI_GELU_BF16, bias=blk["b1"], out=hid, ld_out=hid.shape[1]), st)
+            gemm(hid, blk["w2"], RQ, D, hid.shape[1], epilogue(EPI_RESID_GATE_F32, bias=blk["b2"], out=xs, ld_out=D), st)
         if acts is not None:
             acts["srt"] = xs.clone()
         zc = self.zc
@@ -409,26 +387,7 @@ class SurfelEncoder:
         pc = pcd.float().contiguous()
         noise = noise.to(dev).float().contiguous()
         with torch.cuda.device(dev):
-            if not self.use_graph or torch.cuda.is_current_stream_capturing():
-                return self._launches(img, pc, start_idx, noise)
-            key = (B, self.V, H, W, pc.shape[1])
-            slot = self._graphs.get(key)
-            if slot is None:
-                while len(self._graphs) >= self.MAX_GRAPHS:
-                    self._graphs.pop(next(iter(self._graphs)))
-                with torch.inference_mode(False), torch.no_grad():
-                    s_in = [t.clone() for t in (img, pc, start_idx, noise)]
-                    self._launches(*s_in)
-                    torch.cuda.synchronize(dev)
-                    g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g, capture_error_mode="thread_local"):
-                        outs = self._launches(*s_in)
-                slot = self._graphs[key] = (g, s_in, outs)
-            g, s_in, outs = slot
-            for s, t in zip(s_in, (img, pc, start_idx, noise)):
-                s.copy_(t)
-            g.replay()
-            return {k: v.clone() for k, v in outs.items()}
+            return self._graphs.run((B, self.V, H, W, pc.shape[1]), self._launches, (img, pc, start_idx, noise))
 
     def vae_reparameterization(self, latent, sample_posterior=True, generator=None):
         """latent: encode()'s dict.  Returns latent_normalized [B, K, zc], query_pcd_xyz and the posterior."""

@@ -58,8 +58,9 @@ def test_library_exports_every_declared_symbol():
 
 def test_ctypes_table_matches_header():
     """_lib.lib() declares restype and argtypes for every function of the header, parameter by parameter as the
-    header states them, and the ctypes structures have the header's fields in the header's order.  ctypes does not
-    check a call against the C prototype: a wrong width or a missing argument would pass a wrong value silently."""
+    header states them, the ctypes structures have the header's fields in the header's order, and the EPI_* mode
+    constants are the header's GA_EPI_*.  ctypes does not check a call against the C prototype: a wrong width, a
+    missing argument or a wrong mode would pass a wrong value silently."""
     from gaussiananything_b200 import _lib
     L = _lib.lib()
     decls = _declared_functions()
@@ -71,11 +72,14 @@ def test_ctypes_table_matches_header():
         assert fn.argtypes is not None and len(fn.argtypes) == len(params), (name, params, fn.argtypes)
         for decl, ct in zip(params, fn.argtypes):
             assert _ctype_matches(decl, ct), (name, decl, ct)
-    for cls in (_lib.GaRasterLayout, _lib.GaGemmEpilogue):
+    for cls in (_lib.GaRasterLayout, _lib.GaGemmEpilogue, _lib.GaVaeEncHead):
         fields = _declared_fields(cls.__name__)
         assert [n for n, _ in cls._fields_] == [re.search(r"(\w+)\s*$", f).group(1) for f in fields], cls.__name__
         for f, (n, ct) in zip(fields, cls._fields_):
             assert _ctype_matches(f, ct), (cls.__name__, f, ct)
+    header = open(os.path.join(ROOT, "include", "ga_b200.h")).read()
+    modes = {"EPI_" + n: int(v) for n, v in re.findall(r"^#define GA_EPI_(\w+)\s+(\d+)", header, flags=re.M)}
+    assert len(modes) == 6 and modes == {n: getattr(_lib, n) for n in dir(_lib) if n.startswith("EPI_")}, modes
 
 
 def test_layout_ex_is_host_only_and_monotonic():

@@ -119,11 +119,11 @@ def test_scene_builders_do_not_need_the_oracle():
 
 
 def test_gemm_tile_width_rule_matches_the_committed_sweep():
-    """dit._gemm_config (host logic, no GPU needed) against profiles/gemm_sweep_h100.txt: on every swept DiT shape the width it
+    """_launch.gemm_config (host logic, no GPU needed) against profiles/gemm_sweep_h100.txt: on every swept DiT shape the width it
     picks is within 3 % of the fastest single-CTA configuration that was measured, and HEADS epilogues stay 128 wide."""
     import os
     import re
-    from gaussiananything_b200 import dit
+    from gaussiananything_b200 import _launch, _lib
     path = os.path.join(os.path.dirname(__file__), "..", "profiles", "gemm_sweep_h100.txt")
     rows = [l for l in open(path) if l.startswith("M=")]
     assert len(rows) == 9
@@ -131,7 +131,7 @@ def test_gemm_tile_width_rule_matches_the_committed_sweep():
         M, N, K = (int(v) for v in re.match(r"M=(\d+) N=(\d+) K=(\d+)", line).groups())
         us = {int(c): float(t) for c, t in re.findall(r"(\d+):\s+([\d.]+)us", line.split("|", 1)[1])}
         single = {c: t for c, t in us.items() if c in (128, 192, 256)}
-        pick = dit._gemm_config(M, N, dit.EPI_BF16)
+        pick = _launch.gemm_config(M, N, _lib.EPI_BF16)
         assert pick in single, (M, N, pick)
         assert single[pick] <= 1.03 * min(single.values()), (M, N, K, pick, single)
-        assert dit._gemm_config(M, N, dit.EPI_HEADS) == 128
+        assert _launch.gemm_config(M, N, _lib.EPI_HEADS) == 128

@@ -6,9 +6,10 @@ import sys
 import torch
 
 sys.path.insert(0, ".")
-from gaussiananything_b200 import dit  # noqa: E402
+from gaussiananything_b200 import _lib  # noqa: E402
+from gaussiananything_b200._launch import ptr  # noqa: E402
 
-L = dit._bind()
+L = _lib.lib()
 dev = torch.device("cuda:0")
 st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
@@ -22,8 +23,8 @@ def gemm_case(M, N, K, bn, tag=""):
     A = torch.randn(M, K, device=dev).bfloat16()
     W = (torch.randn(N, K, device=dev) / math.sqrt(K)).bfloat16()
     out = torch.full((M, N), 7.0, device=dev, dtype=torch.float32)
-    e = dit.GaGemmEpilogue(mode=dit.EPI_F32, out=out.data_ptr(), ld_out=N)
-    rc = L.ga_gemm_bf16_tn(dit._p(A), K, dit._p(W), K, M, N, K, C.byref(e), bn, st)
+    e = _lib.GaGemmEpilogue(mode=_lib.EPI_F32, out=out.data_ptr(), ld_out=N)
+    rc = L.ga_gemm_bf16_tn(ptr(A), K, ptr(W), K, M, N, K, C.byref(e), bn, st)
     torch.cuda.synchronize()
     ref = A.float() @ W.float().T
     r = rel(out, ref)
@@ -53,7 +54,7 @@ def attn_case(B, H, Nq, Nk):
     k[:, :Nk] = torch.randn(B * H, Nk, 64, device=dev)
     vt[:, :, :Nk] = torch.randn(B * H, 64, Nk, device=dev)
     out = torch.zeros(B, Nq, H * 64, device=dev, dtype=torch.bfloat16)
-    rc = L.ga_attention_bf16(dit._p(q), dit._p(k), dit._p(vt), dit._p(out), B, H, Nq, Nk, pq, pk, 0.125, 0.0, st)
+    rc = L.ga_attention_bf16(ptr(q), ptr(k), ptr(vt), ptr(out), B, H, Nq, Nk, pq, pk, 0.125, 0.0, st)
     torch.cuda.synchronize()
     ref = torch.nn.functional.scaled_dot_product_attention(
         q[:, :Nq].float().view(B, H, Nq, 64), k[:, :Nk].float().view(B, H, Nk, 64),
