@@ -51,8 +51,10 @@ ABI = {
     "ga_render_post_backward": (i32, [vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]),
     "ga_raster_set_variant": (i32, [i32, i32]),
     "ga_gemm_bf16_tn": (i32, [vp, i32, vp, i32, i32, i32, i32, C.POINTER(GaGemmEpilogue), i32, vp]),
+    "ga_gemm_validate": (i32, [vp, i32, vp, i32, i32, i32, i32, C.POINTER(GaGemmEpilogue), i32]),
     "ga_attention_bf16": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, f32, vp]),
     "ga_attention_causal_bf16": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, f32, vp]),
+    "ga_attention_validate": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32]),
     "ga_rmsnorm_modulate": (i32, [vp, vp, vp, vp, i32, i32, vp, i32, i32, f32, vp]),
     "ga_linear_small": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
     "ga_timestep_sinusoid": (i32, [vp, vp, i32, i32, vp]),

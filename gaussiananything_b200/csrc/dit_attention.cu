@@ -228,13 +228,29 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant
     }
 }
 
+}  // namespace
+
+extern "C" int ga_attention_validate(const void *Q, const void *K, const void *Vt, const void *out, int batch,
+                                     int heads, int Nq, int Nk, int pitch_q, int pitch_k, int causal)
+{
+    if (!Q || !K || !Vt || !out || batch <= 0 || heads <= 0 || Nq <= 0 || Nk <= 0) return GA_ERR_BADARG;
+    if (pitch_q < Nq || pitch_k < Nk || pitch_k % 128 != 0) return GA_ERR_BADARG;
+    if (causal && Nq != Nk) return GA_ERR_BADARG;
+    // TMA sources need 16-byte bases; the output is written as bf16 pairs
+    const auto misaligned = [](const void *p, uintptr_t b) { return (reinterpret_cast<uintptr_t>(p) & (b - 1)) != 0; };
+    if (misaligned(Q, 16) || misaligned(K, 16) || misaligned(Vt, 16) || misaligned(out, 4)) return GA_ERR_BADARG;
+    if ((int64_t)batch * heads > 65535) return GA_ERR_SIZE;                  // one (batch, head) per grid.y
+    return 0;
+}
+
+namespace {
+
 template <bool kCausal>
 int launch_attention(const void *Q, const void *K, const void *Vt, void *out, int batch, int heads, int Nq, int Nk,
                      int pitch_q, int pitch_k, float softmax_scale, float score_bound, void *stream)
 {
-    if (!Q || !K || !Vt || !out || batch <= 0 || heads <= 0 || Nq <= 0 || Nk <= 0) return GA_ERR_BADARG;
-    if (pitch_q < Nq || pitch_k < Nk || pitch_k % 128 != 0) return GA_ERR_BADARG;
-    if (kCausal && Nq != Nk) return GA_ERR_BADARG;
+    const int rc0 = ga_attention_validate(Q, K, Vt, out, batch, heads, Nq, Nk, pitch_q, pitch_k, kCausal ? 1 : 0);
+    if (rc0) return rc0;
     const uint64_t BH = (uint64_t)batch * heads;
     static GaPerDevice attr_set;
     if (ga_first_use_on_device(attr_set)) {

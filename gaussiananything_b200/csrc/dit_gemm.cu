@@ -484,16 +484,52 @@ static int launch_gemm(const void *A, int lda, const void *W, int ldw, const GaG
     }
 }
 
+static bool misaligned(const void *p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) != 0; }
+
+// The rules of ga_b200.h, host only: every address and size the kernel derives from the arguments stays inside the
+// buffers they describe and is aligned for the vector loads and stores it is used with.
+extern "C" int ga_gemm_validate(const void *A, int lda, const void *W, int ldw, int M, int N, int K,
+                                const GaGemmEpilogue *epi, int block_n)
+{
+    if (!A || !W || !epi || M <= 0 || N <= 0 || K <= 0) return GA_ERR_BADARG;
+    // TMA operands: 16-byte base and row pitch; the pitch covers the K columns the tensor map describes
+    if (misaligned(A, 16) || misaligned(W, 16) || lda % 8 || ldw % 8 || lda < K || ldw < K) return GA_ERR_BADARG;
+    const int bn = block_n, mode = epi->mode;
+    if (bn != 64 && bn != 128 && bn != 192 && bn != 256) return GA_ERR_BADARG;
+    if (mode < GA_EPI_BF16 || mode > GA_EPI_GEGLU_BF16) return GA_ERR_BADARG;
+    if (mode == GA_EPI_HEADS) {
+        if (bn != 128 && bn != 256) return GA_ERR_BADARG;                   // the widths HEADS is instantiated for
+        if (epi->heads <= 0 || epi->heads > N / 64 || N % (64 * epi->heads)) return GA_ERR_BADARG;
+        if (epi->first_part != 0 && epi->first_part != 1) return GA_ERR_BADARG;
+        const int parts = N / (64 * epi->heads);
+        if (epi->first_part + parts > 3) return GA_ERR_BADARG;              // a fourth part would be written as V again
+        void *const dst[3] = {epi->q, epi->k, epi->vt};
+        for (int p = epi->first_part; p < epi->first_part + parts; p++)
+            if (!dst[p] || misaligned(dst[p], 16)) return GA_ERR_BADARG;     // 16-byte token rows / Vt pieces
+        if (epi->rows_per_batch < 1 || epi->tok_pitch < epi->rows_per_batch) return GA_ERR_BADARG;
+        return 0;
+    }
+    if (!epi->out) return GA_ERR_BADARG;
+    const bool f32 = mode == GA_EPI_F32 || mode == GA_EPI_RESID_GATE_F32;
+    // float4 (fp32), 4 x bf16 (BF16, GELU) and 2 x bf16 (GEGLU) stores at row starts when ld_out % 4 == 0
+    if (misaligned(epi->out, f32 ? 16 : (mode == GA_EPI_GEGLU_BF16 ? 4 : 8))) return GA_ERR_BADARG;
+    if (mode == GA_EPI_GEGLU_BF16) {
+        if (N % 2 || epi->ld_out < N / 2) return GA_ERR_BADARG;             // (x, gate) column pairs
+    } else if (epi->ld_out < N) {
+        return GA_ERR_BADARG;
+    }
+    if (mode == GA_EPI_RESID_GATE_F32 && epi->gate && (epi->rows_per_batch < 1 || epi->gate_ld < N))
+        return GA_ERR_BADARG;
+    return 0;
+}
+
 extern "C" int ga_gemm_bf16_tn(const void *A, int lda, const void *W, int ldw, int M, int N, int K,
                                const GaGemmEpilogue *epi, int block_n, void *stream)
 {
-    if (!A || !W || !epi || M <= 0 || N <= 0 || K <= 0) return GA_ERR_BADARG;
+    const int rc = ga_gemm_validate(A, lda, W, ldw, M, N, K, epi, block_n);
+    if (rc) return rc;
     // block_n = tile width {64, 128, 192, 256}
     const int bn = block_n;
-    if (epi->mode == GA_EPI_HEADS && (N % 64 != 0 || epi->heads <= 0 || bn < 128)) return GA_ERR_BADARG;
-    if (bn != 64 && bn != 128 && bn != 192 && bn != 256) return GA_ERR_BADARG;
-    if (bn == 192 && epi->mode == GA_EPI_HEADS) return GA_ERR_BADARG;        // 192 is not a whole number of heads per half
-    if (epi->mode == GA_EPI_GEGLU_BF16 && N % 2) return GA_ERR_BADARG;        // (x, gate) column pairs
     cudaStream_t s = (cudaStream_t)stream;
     if (bn == 64) return launch_gemm<64>(A, lda, W, ldw, *epi, M, N, K, s);
     if (bn == 128) return launch_gemm<128>(A, lda, W, ldw, *epi, M, N, K, s);

@@ -161,7 +161,7 @@ int ga_raster_set_variant(int radius_formula, int quat_norm_grad);
 typedef struct GaGemmEpilogue {
     int mode;
     const float *bias;        /* [N] or NULL */
-    void *out;                /* modes 0-3 */
+    void *out;                /* modes 0-3, 5 */
     int ld_out;
     const float *gate;        /* mode 3: [batch, gate_ld] (already offset to the gate chunk) or NULL (= 1) */
     int gate_ld;
@@ -176,9 +176,20 @@ typedef struct GaGemmEpilogue {
 
 /* A [M, lda] bf16 row-major, W [N, ldw] bf16 row-major (nn.Linear weight), K contiguous in both.
  * block_n = tile width {64, 128, 192, 256} of the 128 x width output tile (192: not for GA_EPI_HEADS).
- * lda, ldw multiples of 8. */
+ * lda, ldw multiples of 8.  Arguments are checked by ga_gemm_validate before anything is launched. */
 int ga_gemm_bf16_tn(const void *A, int lda, const void *W, int ldw, int M, int N, int K,
                     const GaGemmEpilogue *epi, int block_n, void *stream);
+/* Host only, no CUDA call: 0 when ga_gemm_bf16_tn accepts the arguments, else GA_ERR_BADARG.  The rules:
+ *   A, W, epi non-NULL; M, N, K > 0; A and W 16-byte aligned; lda, ldw multiples of 8 and >= K;
+ *   block_n in {64, 128, 192, 256}; mode in 0..5;
+ *   modes 0-3, 5: out non-NULL; ld_out >= N (N / 2 for GEGLU, where N is even); out aligned to 16 bytes (modes 2, 3),
+ *     8 bytes (modes 0, 1) or 4 bytes (mode 5);
+ *   mode 3 with a gate: rows_per_batch >= 1 and gate_ld >= N (a NULL gate reads neither);
+ *   mode 4: block_n 128 or 256; heads >= 1; N a multiple of 64 * heads; first_part 0 or 1 and first_part +
+ *     N / (64 * heads) <= 3; q, k, vt non-NULL and 16-byte aligned for each part the columns reach (q for part 0,
+ *     k for 1, vt for 2); rows_per_batch >= 1 and tok_pitch >= rows_per_batch. */
+int ga_gemm_validate(const void *A, int lda, const void *W, int ldw, int M, int N, int K,
+                     const GaGemmEpilogue *epi, int block_n);
 
 /* softmax(Q K^T * softmax_scale) V, head_dim 64.  Q [B*H, pitch_q, 64], K [B*H, pitch_k, 64],
  * Vt [B*H, 64, pitch_k] (bf16, padding beyond Nk must be finite); out [B, Nq, H*64] bf16.
@@ -194,6 +205,12 @@ int ga_attention_bf16(const void *Q, const void *K, const void *Vt, void *out, i
 int ga_attention_causal_bf16(const void *Q, const void *K, const void *Vt, void *out, int batch, int heads,
                              int Nq, int Nk, int pitch_q, int pitch_k, float softmax_scale, float score_bound,
                              void *stream);
+/* Host only, no CUDA call: the argument check both attention entry points make first (causal != 0 for the causal
+ * one).  GA_ERR_BADARG unless Q, K, Vt, out are non-NULL; batch, heads, Nq, Nk > 0; pitch_q >= Nq; pitch_k >= Nk and
+ * a multiple of 128; Nq == Nk when causal; Q, K, Vt 16-byte and out 4-byte aligned.  GA_ERR_SIZE when
+ * batch * heads > 65535 (one grid row per (batch, head)).  0 otherwise. */
+int ga_attention_validate(const void *Q, const void *K, const void *Vt, const void *out, int batch, int heads,
+                          int Nq, int Nk, int pitch_q, int pitch_k, int causal);
 
 /* out_bf16[r,:] = RMSNorm(x[r,:]; eps) * w [* (1 + scale[b,:]) + shift[b,:]], b = r / rows_per_batch;
  * shift/scale both NULL or both set, rows mod_ld apart. */

@@ -121,6 +121,91 @@ def test_forward_ex_rejects_null_small_workspace_and_one_status_pointer():
     assert fwd(256, 256, None) == -1 and fwd(256, None, 256) == -1
 
 
+def test_gemm_validate_rules():
+    """ga_gemm_validate is host-only: fake, never dereferenced addresses.  Each rule of the header, one at a time,
+    from an accepted call of every mode."""
+    from gaussiananything_b200 import _lib
+    L = _lib.lib()
+    A, W, OUT = 0x100000, 0x200000, 0x300000
+    base = dict(M=300, N=512, K=256, lda=264, ldw=256, bn=128)
+
+    def rc(mode, bn=None, M=None, N=None, K=None, lda=None, ldw=None, A_=A, W_=W, **fields):
+        f = dict({0: dict(out=OUT, ld_out=512), 1: dict(out=OUT, ld_out=512), 2: dict(out=OUT, ld_out=515),
+                  3: dict(out=OUT, ld_out=512), 5: dict(out=OUT, ld_out=256),
+                  4: dict(q=OUT, k=OUT + 0x10000, vt=OUT + 0x20000, heads=4, first_part=1, rows_per_batch=150,
+                          tok_pitch=256)}.get(mode, dict(out=OUT, ld_out=512)), **fields)
+        e = _lib.GaGemmEpilogue(mode=mode, eps=1e-5, **f)
+        g = lambda v, k: base[k] if v is None else v
+        return L.ga_gemm_validate(A_, g(lda, "lda"), W_, g(ldw, "ldw"), g(M, "M"), g(N, "N"), g(K, "K"), C.byref(e),
+                                  g(bn, "bn"))
+
+    for mode in range(6):
+        assert rc(mode) == 0, mode
+        for bn in (64, 192, 256):
+            assert rc(mode, bn=bn) == (-1 if mode == 4 and bn != 256 else 0), (mode, bn)
+    assert rc(3, gate=0x400000, gate_ld=512, rows_per_batch=1) == 0
+    assert L.ga_gemm_validate(A, 264, W, 256, 300, 512, 256, None, 128) == -1           # epi NULL
+    bad = [
+        dict(A_=0), dict(W_=0), dict(M=0), dict(N=0), dict(K=0), dict(bn=96), dict(bn=0),
+        dict(A_=A + 8), dict(W_=W + 2),                                              # TMA bases: 16 bytes
+        dict(lda=260), dict(ldw=252), dict(lda=248), dict(K=272),                    # pitch % 8, pitch >= K
+        dict(out=0), dict(ld_out=511),
+        dict(out=OUT + 8), dict(out=OUT + 4),                                         # fp32: 16-byte out
+        dict(gate=0x400000, gate_ld=512, rows_per_batch=0), dict(gate=0x400000, gate_ld=511, rows_per_batch=1),
+    ]
+    for kw in bad[:15]:
+        for mode in (0, 1, 2, 3, 5):
+            if "ld_out" in kw and mode == 5:
+                continue
+            assert rc(mode, **kw) == -1, (mode, kw)
+    for mode in (2, 3):
+        assert rc(mode, out=OUT + 8) == -1 and rc(mode, out=OUT + 4) == -1
+    for mode in (0, 1):
+        assert rc(mode, out=OUT + 8) == 0 and rc(mode, out=OUT + 4) == -1 and rc(mode, out=OUT + 2) == -1
+    assert rc(5, out=OUT + 4) == 0 and rc(5, out=OUT + 2) == -1
+    assert rc(5, ld_out=255) == -1 and rc(5, N=511, ld_out=256) == -1              # GEGLU: ld_out >= N / 2, N even
+    for kw in bad[17:]:
+        assert rc(3, **kw) == -1, kw
+    assert rc(3, gate=0, gate_ld=0, rows_per_batch=0) == 0                          # no gate: neither is read
+    assert rc(6) == -1 and rc(-1) == -1
+    # HEADS: N = 512 = 2 parts of 4 heads x 64, starting at k
+    assert rc(4, bn=256) == 0 and rc(4, first_part=0) == 0
+    heads_bad = [dict(heads=0), dict(heads=3), dict(first_part=2), dict(first_part=-1), dict(heads=2),
+                 dict(k=0), dict(vt=0), dict(k=OUT + 8), dict(vt=OUT + 0x20008),
+                 dict(rows_per_batch=0), dict(tok_pitch=149)]
+    for kw in heads_bad:
+        assert rc(4, **kw) == -1, kw
+    assert rc(4, N=448) == -1                                                        # not whole heads
+    assert rc(4, N=768, first_part=0) == 0 and rc(4, N=768, first_part=1) == -1    # a 4th part
+    assert rc(4, N=1024, first_part=0) == -1
+    assert rc(4, q=0) == 0 and rc(4, q=0, first_part=0) == -1                       # q only when part 0 is reached
+    assert rc(4, N=256, first_part=0, k=0, vt=0) == 0                              # q only
+    assert rc(4, N=256, first_part=0, q=0) == -1
+
+
+def test_attention_validate_rules():
+    from gaussiananything_b200 import _lib
+    L = _lib.lib()
+    Q, K, V, O = 0x100000, 0x200000, 0x300000, 0x400000
+
+    def rc(causal=0, **kw):
+        a = dict(Q=Q, K=K, V=V, O=O, B=2, H=16, Nq=768, Nk=1369, pq=768, pk=1408)
+        a.update(kw)
+        if causal and "Nk" not in kw:
+            a.update(Nk=a["Nq"], pk=_ru(a["Nq"]))
+        return L.ga_attention_validate(a["Q"], a["K"], a["V"], a["O"], a["B"], a["H"], a["Nq"], a["Nk"], a["pq"],
+                                       a["pk"], causal)
+
+    _ru = lambda n: (n + 127) // 128 * 128
+    assert rc() == 0 and rc(causal=1) == 0 and rc(Nq=17, pq=17) == 0 and rc(O=O + 4) == 0
+    for kw in (dict(Q=0), dict(K=0), dict(V=0), dict(O=0), dict(B=0), dict(H=0), dict(Nq=0), dict(Nk=0),
+               dict(pq=767), dict(pk=1280), dict(pk=1409), dict(Q=Q + 8), dict(K=K + 8), dict(V=V + 2),
+               dict(O=O + 2)):
+        assert rc(**kw) == -1, kw
+    assert rc(causal=1, Nk=767, pk=768) == -1 and rc(causal=0, Nk=767, pk=768) == 0
+    assert rc(B=1, H=65535) == 0 and rc(B=2, H=32768) == -3 and rc(B=65536, H=1) == -3
+
+
 def test_product_never_touches_the_oracle():
     pkg = os.path.join(ROOT, "gaussiananything_b200")
     for dp, _, fs in os.walk(pkg):
