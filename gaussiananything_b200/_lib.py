@@ -94,6 +94,8 @@ ABI = {
     "ga_clip_text_embed": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp]),
     "ga_clip_text_eot_gather": (i32, [vp, vp, vp, i32, i32, i32, vp]),
     "ga_quick_gelu_bf16": (i32, [vp, i64, vp]),
+    "ga_gbuffer_pack": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, vp, i32, vp, vp, vp, vp, vp, vp]),
+    "ga_recon_metrics": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, vp, vp, vp]),
     "ga_profile_enable": (i32, [i32]),
     "ga_profile_read": (i32, [C.POINTER(f32), i32]),
     "ga_b200_version": (C.c_char_p, []),

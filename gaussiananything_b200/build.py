@@ -23,6 +23,8 @@ EXTRA = {
     # TSDF weights / tsdf / colours and marching-cubes vertices: bit-exact with oracle/tsdf_oracle.py
     "mesh_tsdf.cu": ["--fmad=false"],
     "mesh_extract.cu": ["--fmad=false"],
+    # encoder input and metric sums: every operation rounded on its own, as include/ga_b200.h Part 7 states them
+    "gbuffer_ops.cu": ["--fmad=false"],
 }
 
 

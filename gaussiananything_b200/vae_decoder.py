@@ -262,7 +262,9 @@ class SurfelAE:
     issues 4 x B x V sequential launch sets from Python; here every level is ONE batched launch set and the four
     levels run on four CUDA streams, so the small levels (768 / 6 144 / 24 576 surfels: latency bound) overlap with
     the 73 728-surfel one.  With `encoder=` (vae_encoder.SurfelEncoder) the encoder behaviours 'enc', 'encoder_vae' and
-    'enc_dec_wo_triplane' run too; without one, and for the other training behaviours, they raise."""
+    'enc_dec_wo_triplane' run too, and 'reconstruct_chunk' (gbuffer.reconstruct_chunk: a G-buffer chunk folder in,
+    Gaussians, renders at the chunk's cameras and per-view metrics out); without one, and for the other training
+    behaviours, they raise."""
 
     OUTPUT_SIZE = {"gaussians_base": 128, "gaussians_upsampled": 256, "gaussians_upsampled_2": 384,
                    "gaussians_upsampled_3": 512}
@@ -337,6 +339,10 @@ class SurfelAE:
             return self.rendering_kwargs
         if self.encoder is not None and behaviour in ("enc", "encoder_vae", "enc_dec_wo_triplane"):
             return self._encoder_behaviour(behaviour, img, kwargs)
+        if behaviour == "reconstruct_chunk":
+            # chunk=, pcd=, optional input_views=, eval_views=, fps_start=, generator=, bg_color= (gbuffer.py)
+            from .gbuffer import reconstruct_chunk
+            return reconstruct_chunk(self, **kwargs)
         raise NotImplementedError("gaussiananything_b200.SurfelAE: behaviour %r is outside the decode / render path "
                                   "(encoder and training behaviours are not rebuilt: SURVEY.md section 8)" % (behaviour,))
 

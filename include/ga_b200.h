@@ -440,6 +440,52 @@ int ga_clip_text_eot_gather(const int32_t *ids, const float *x, float *out, int 
 /* In place on bf16 x [n]: x = x * sigmoid(1.702 x) (QuickGELU, computed in fp32). */
 int ga_quick_gelu_bf16(void *x, int64_t n, void *stream);
 
+/*
+ * ---------------------------------------------------------------------------
+ * Part 7: 3D VAE reconstruction from G-buffer chunk folders (the reference's vae-3d.sh input:
+ * datasets/g_buffer_objaverse.py read_chunk :3225-3302 and PostProcess._post_process_sample_batch :481-702, at
+ * reso == reso_encoder == the files' size, frame_0_as_canonical=False, append_xyz, plucker_embedding, read_normal).
+ * Both kernels are compiled without FMA contraction: every operation below is rounded to fp32 on its own, in the
+ * order written.
+ * ---------------------------------------------------------------------------
+ */
+/* One launch, one thread per four pixels of a row (16-byte stores).  Inputs as the chunk's files decode, the n_chunk
+ * views side by side: raw_img, normal uint8 [H, n_chunk * W, 3], alpha uint8 [H, n_chunk * W] (may be NULL without
+ * targets), depth fp32 [n_chunk, H, W], cams fp32 [n_chunk, 25] (c2w row-major 16 | K 9, normalised by the image
+ * size), views int32 [n_views] in [0, n_chunk) (the caller checks the range).  W % 4 == 0, W <= 1024.
+ * img_to_encoder fp32 [n_views, 15, H, W], row s from view views[s]:
+ *   0-2   (rgb / 255 - mean) / std, mean = (0.485, 0.456, 0.406), std = (0.229, 0.224, 0.225): the ImageNet
+ *         Normalize of PostProcess.__init__ (:156-160); load_eval_data's chunk branch leaves imgnet_normalize=True
+ *   3-5   n = (u8 / 255) * 2 - 1, then (-n.x, -n.z, n.y) (unity2blender_fix)
+ *   6-11  cross(o, d), d: o = c2w[:3, 3]; d = c2w[:3, :3] g, g = (gx, gy, 1) / sqrt(gx gx + gy gy + 1),
+ *         gx = ((x + 0.5) / W - cx) / fx, gy = ((y + 0.5) / H - cy) / fy  (gen_rays; sums left to right)
+ *   12-14 p = o + depth * r, r = q / max(|q|, 1e-12), q = (c2w (lx, ly, 1, 1))[:3] - o,
+ *         lx = (u - cx + cy sk / fy - sk v / fy) / fx, ly = (v - cy) / fy, u = (x + 0.5) / W, v = (y + 0.5) / H
+ *         (RaySampler); p clipped to [-0.45, 0.45], then 0 where |p| == 0.45.  A background pixel (depth 0) gives
+ *         p = o: removed only where the camera origin's coordinate is outside the clip, as in the reference.
+ * Targets, all four or none: t_img fp32 [n_views, 3, H, W] = (rgb / 255) * 2 - 1; t_alpha [n_views, 1, H, W] =
+ * alpha / 255; t_depth [n_views, 1, H, W] = depth; t_mask [n_views, 1, H, W] = depth > 0 as 1.0 / 0.0. */
+int ga_gbuffer_pack(const uint8_t *raw_img, const uint8_t *normal, const uint8_t *alpha, const float *depth,
+                    const float *cams, int n_chunk, int H, int W, const int32_t *views, int n_views,
+                    float *img_to_encoder, float *t_img, float *t_alpha, float *t_depth, float *t_mask,
+                    void *stream);
+/* Blocks per view of the first stage of ga_recon_metrics: partial is fp32 [n_views, GA_RECON_METRICS_BLOCKS, 8]. */
+#define GA_RECON_METRICS_BLOCKS 64
+/* Per-view sums over the H * W pixels of rendered maps against targets, table fp32 [n_views, 8]:
+ *   [0] sum over 3 channels of (image - (t_img + 1) / 2)^2      image in [0, 1], t_img in [-1, 1]
+ *   [1] sum of t_mask * |depth - t_depth|                        [2] sum of t_mask
+ *   [3] sum of t_mask * (1 - <rend_normal, t_normal>)            (nsr/train_nv_util.py:2162 on the foreground)
+ *   [4] sum of |alpha - t_alpha|
+ *   [5], [6] pixels where alpha > 0.5 and / or t_alpha > 0.5     [7] H * W
+ * image, rend_normal, t_img fp32 [n_views, 3, H, W]; depth, alpha, t_depth, t_alpha, t_mask [n_views, 1, H, W];
+ * t_normal fp32, view v at t_normal + v * t_normal_stride, [3, H, W] (channels 3-5 of img_to_encoder with stride
+ * 15 H W).  H * W <= 2^24, so the counts are exact.  Two stages in a fixed order (per-block partial sums, then one
+ * block per view adds them in block order), no atomics: the same inputs give the same bits. */
+int ga_recon_metrics(const float *image, const float *depth, const float *alpha, const float *rend_normal,
+                     const float *t_img, const float *t_depth, const float *t_alpha, const float *t_mask,
+                     const float *t_normal, int64_t t_normal_stride, int n_views, int H, int W, float *partial,
+                     float *table, void *stream);
+
 /* Measurement aid: when enabled, cudaEvents are recorded around every kernel
  * stage of the next forward/backward; ga_profile_read synchronises on them and
  * returns per-stage milliseconds: [0] preprocess, [1] binning, [2] render fwd,
