@@ -96,6 +96,13 @@ ABI = {
     "ga_quick_gelu_bf16": (i32, [vp, i64, vp]),
     "ga_gbuffer_pack": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, vp, i32, vp, vp, vp, vp, vp, vp]),
     "ga_recon_metrics": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, vp, vp, vp]),
+    "ga_conv3x3_relu_bf16": (i32, [vp, i32, i32, i32, i32, vp, i32, vp, i32, vp, vp]),
+    "ga_lpips_pack": (i32, [vp, vp, i32, i32, i32, i32, vp, vp, vp, vp]),
+    "ga_maxpool2x2_bf16": (i32, [vp, i32, i32, i32, i32, vp, vp]),
+    "ga_lpips_head": (i32, [vp, i32, i32, i32, i32, vp, vp, vp]),
+    "ga_lpips_reduce": (i32, [vp, i32, i32, i32, vp, vp]),
+    "ga_ssim_scratch_bytes": (sz, [i32, i32, i32]),
+    "ga_ssim": (i32, [vp, vp, i32, i32, i32, vp, vp, sz, vp, vp]),
     "ga_profile_enable": (i32, [i32]),
     "ga_profile_read": (i32, [C.POINTER(f32), i32]),
     "ga_b200_version": (C.c_char_p, []),

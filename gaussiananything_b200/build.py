@@ -25,6 +25,8 @@ EXTRA = {
     "mesh_extract.cu": ["--fmad=false"],
     # encoder input and metric sums: every operation rounded on its own, as include/ga_b200.h Part 7 states them
     "gbuffer_ops.cu": ["--fmad=false"],
+    # LPIPS pack / head and SSIM: every operation rounded on its own, as include/ga_b200.h Part 8 states them
+    "lpips_ops.cu": ["--fmad=false"],
 }
 
 

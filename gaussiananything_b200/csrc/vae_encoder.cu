@@ -11,7 +11,8 @@ using namespace sm90;
 namespace {
 
 // ---------------------------------------------------------------------------------------------------------------
-// 3x3 convolution, implicit GEMM: out[m, n] = bias[n] + sum_k A[m, k] W[n, k] (+ residual[m, n]),
+// 3x3 convolution, implicit GEMM: out[m, n] = bias[n] + sum_k A[m, k] W[n, k] (+ residual[m, n]), then max(., 0)
+// when RELU,
 // m = (image, oy, ox), k = (ky * 3 + kx) * Cin + c.  A is never materialised: every 16-byte piece (8 channels of one
 // tap of one output pixel) is gathered with cp.async straight from the NHWC input, zero-filled where the tap falls
 // into the padding or k runs past 9 * Cin.  The pieces land in the 128-byte-swizzled K-major layout that
@@ -48,7 +49,7 @@ template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile(
 // cp.async writes through the generic proxy, wgmma reads through the async proxy
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 
-template <int BN>
+template <int BN, bool RELU>
 __global__ void __launch_bounds__(kConvThreads, 1) conv3x3_kernel(const ConvArgs a)
 {
     using Cfg = ConvCfg<BN>;
@@ -150,6 +151,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv3x3_kernel(const ConvArgs
                 const float2 rr = *reinterpret_cast<const float2 *>(a.residual + o);
                 v0 += rr.x; v1 += rr.y;
             }
+            if (RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
             if (a.out_f32) *reinterpret_cast<float2 *>(a.out_f32 + o) = make_float2(v0, v1);
             if (a.out_bf16) *reinterpret_cast<__nv_bfloat162 *>(a.out_bf16 + o) = __floats2bfloat162_rn(v0, v1);
         }
@@ -461,17 +463,39 @@ __global__ void __launch_bounds__(kHeadThreads) readout_head_kernel(const GaVaeE
 }  // namespace
 
 // ---- host side ----------------------------------------------------------------------------------------------------
-template <int BN>
+template <int BN, bool RELU>
 static int launch_conv(const ConvArgs &a, cudaStream_t s)
 {
     using Cfg = ConvCfg<BN>;
     static GaPerDevice attr_set;
     if (ga_first_use_on_device(attr_set)) {
-        cudaError_t e = cudaFuncSetAttribute(conv3x3_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem);
+        cudaError_t e = cudaFuncSetAttribute(conv3x3_kernel<BN, RELU>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             Cfg::kSmem);
         if (e != cudaSuccess) return (int)e;
     }
     dim3 grid((a.M + CBM - 1) / CBM, a.Cout / BN);
-    return (int)ga_launch_pdl(conv3x3_kernel<BN>, grid, dim3(kConvThreads), (size_t)Cfg::kSmem, s, a);
+    return (int)ga_launch_pdl(conv3x3_kernel<BN, RELU>, grid, dim3(kConvThreads), (size_t)Cfg::kSmem, s, a);
+}
+
+// the argument checks of both conv entry points; fills `a` and returns 0, or the error code
+static int conv_args(ConvArgs &a, const void *x, int n, int H, int W, int Cin, const void *w_packed, int k_pitch,
+                     const float *bias, int Cout, int stride, const float *residual, float *out_f32, void *out_bf16)
+{
+    if (!x || !w_packed || n <= 0 || Cin <= 0 || Cin % 8 || Cout <= 0 || Cout % 64) return GA_ERR_BADARG;
+    if (!out_f32 && !out_bf16) return GA_ERR_BADARG;
+    const int Ho = ga_conv3x3_out_size(H, stride), Wo = ga_conv3x3_out_size(W, stride);
+    if (Ho <= 0 || Wo <= 0) return GA_ERR_BADARG;
+    if (k_pitch < ((9 * Cin + CBK - 1) / CBK) * CBK || (reinterpret_cast<uintptr_t>(w_packed) & 15) ||
+        (reinterpret_cast<uintptr_t>(x) & 15))
+        return GA_ERR_BADARG;
+    if ((int64_t)n * Ho * Wo >= (int64_t)1 << 31) return GA_ERR_SIZE;
+    a.x = reinterpret_cast<const __nv_bfloat16 *>(x);
+    a.w = reinterpret_cast<const __nv_bfloat16 *>(w_packed);
+    a.bias = bias; a.residual = residual; a.out_f32 = out_f32;
+    a.out_bf16 = reinterpret_cast<__nv_bfloat16 *>(out_bf16);
+    a.H = H; a.W = W; a.Cin = Cin; a.Ho = Ho; a.Wo = Wo; a.Cout = Cout; a.k_pitch = k_pitch; a.stride = stride;
+    a.M = n * Ho * Wo; a.K = 9 * Cin;
+    return 0;
 }
 
 extern "C" int ga_conv3x3_out_size(int H, int stride)
@@ -486,23 +510,21 @@ extern "C" int ga_conv3x3_bf16(const void *x, int n, int H, int W, int Cin, cons
                                const float *bias, int Cout, int stride, const float *residual, float *out_f32,
                                void *out_bf16, void *stream)
 {
-    if (!x || !w_packed || n <= 0 || Cin <= 0 || Cin % 8 || Cout <= 0 || Cout % 64) return GA_ERR_BADARG;
-    if (!out_f32 && !out_bf16) return GA_ERR_BADARG;
-    const int Ho = ga_conv3x3_out_size(H, stride), Wo = ga_conv3x3_out_size(W, stride);
-    if (Ho <= 0 || Wo <= 0) return GA_ERR_BADARG;
-    if (k_pitch < ((9 * Cin + CBK - 1) / CBK) * CBK || (reinterpret_cast<uintptr_t>(w_packed) & 15) ||
-        (reinterpret_cast<uintptr_t>(x) & 15))
-        return GA_ERR_BADARG;
-    if ((int64_t)n * Ho * Wo >= (int64_t)1 << 31) return GA_ERR_SIZE;
     ConvArgs a;
-    a.x = reinterpret_cast<const __nv_bfloat16 *>(x);
-    a.w = reinterpret_cast<const __nv_bfloat16 *>(w_packed);
-    a.bias = bias; a.residual = residual; a.out_f32 = out_f32;
-    a.out_bf16 = reinterpret_cast<__nv_bfloat16 *>(out_bf16);
-    a.H = H; a.W = W; a.Cin = Cin; a.Ho = Ho; a.Wo = Wo; a.Cout = Cout; a.k_pitch = k_pitch; a.stride = stride;
-    a.M = n * Ho * Wo; a.K = 9 * Cin;
+    const int rc = conv_args(a, x, n, H, W, Cin, w_packed, k_pitch, bias, Cout, stride, residual, out_f32, out_bf16);
+    if (rc) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    return Cout % 128 == 0 ? launch_conv<128>(a, s) : launch_conv<64>(a, s);
+    return Cout % 128 == 0 ? launch_conv<128, false>(a, s) : launch_conv<64, false>(a, s);
+}
+
+extern "C" int ga_conv3x3_relu_bf16(const void *x, int n, int H, int W, int Cin, const void *w_packed, int k_pitch,
+                                    const float *bias, int Cout, void *out_bf16, void *stream)
+{
+    ConvArgs a;
+    const int rc = conv_args(a, x, n, H, W, Cin, w_packed, k_pitch, bias, Cout, 1, nullptr, nullptr, out_bf16);
+    if (rc) return rc;
+    cudaStream_t s = (cudaStream_t)stream;
+    return Cout % 128 == 0 ? launch_conv<128, true>(a, s) : launch_conv<64, true>(a, s);
 }
 
 extern "C" size_t ga_group_norm_scratch_bytes(int n, int HW)

@@ -10,6 +10,7 @@ caption.txt, ins.txt; the object's surface samples are a separate fps-4096.ply.
   pack                        one launch of ga_gbuffer_pack: img_to_encoder [V, 15, H, W] and the render targets
   cameras                     the chunk's c rows in the renderer's camera format (mesh.orbit_cameras)
   metrics                     ga_recon_metrics on rendered maps against the targets -> per-view numbers
+  perceptual_metrics          per-view LPIPS (VGG) and SSIM of the rendered images against the targets (lpips.py)
   reconstruct_chunk           pack -> encode -> decode -> render at the chunk's own cameras -> metrics
                               (SurfelAE behaviour 'reconstruct_chunk')
 
@@ -219,15 +220,30 @@ def metrics(render_out, targets):
     return derive(metric_table(render_out, targets))
 
 
+def perceptual_metrics(render_out, targets, lpips_model):
+    """Per-view {'lpips' [V], 'ssim' [V]} (fp32, on the device) of the rendered images against the targets, over
+    the whole frame (no mask): LPIPS compares render_out['image'] * 2 - 1 with targets['img'], both in [-1, 1];
+    SSIM compares render_out['image'] with (targets['img'] + 1) / 2, both in [0, 1].  render_out: [1, V, ...] or
+    [V, ...]; lpips_model: an lpips.LPIPS."""
+    from .lpips import ssim
+    img = render_out["image"]
+    img = (img[0] if img.dim() == 5 else img).float()
+    t = targets["img"].float()
+    if tuple(img.shape) != tuple(t.shape):
+        raise ValueError("gbuffer.perceptual_metrics: render %s and targets %s differ in shape"
+                         % (tuple(img.shape), tuple(t.shape)))
+    return {"lpips": lpips_model(img * 2 - 1, t).reshape(-1), "ssim": ssim(img, (t + 1) / 2)}
+
+
 def reconstruct_chunk(ae, chunk, pcd, input_views=range(8), eval_views=range(8, 16), fps_start=None, generator=None,
-                      bg_color=None):
+                      bg_color=None, lpips=None):
     """The VAE round trip on one chunk: the encoder sees `input_views`, the finest level of detail (73 728 surfels
     at the deployed sizes) is rendered at the chunk's own cameras for `input_views` and `eval_views`, and each render
     is scored against the chunk's files.  chunk: a folder or read_chunk's dict; pcd: a PLY path or [N, 3].
 
     Returns the 'enc_dec_wo_triplane' dict (latent, the four gaussians_* levels) plus 'input' and 'eval', each
     {'views', 'c', 'render' (GaussianRenderer2DGS.render's dict, [1, V, ...]), 'targets', 'table' [V, 8],
-    'metrics'}."""
+    'metrics'}; with `lpips` (an lpips.LPIPS) each also holds 'perceptual' (perceptual_metrics)."""
     if ae.encoder is None:
         raise NotImplementedError("SurfelAE(behaviour='reconstruct_chunk') needs encoder= (vae_encoder.SurfelEncoder)")
     if isinstance(chunk, (str, os.PathLike)):
@@ -248,9 +264,12 @@ def reconstruct_chunk(ae, chunk, pcd, input_views=range(8), eval_views=range(8, 
         r = ae.gs.render(out["gaussians_upsampled_3"], cam["cam_view"], cam["cam_view_proj"], cam["cam_pos"],
                          tanfov=cam["tanfov"], bg_color=bg, output_size=enc_in.shape[-1])
     table = metric_table(r, t_all)
+    perc = perceptual_metrics(r, t_all, lpips) if lpips is not None else None
     for name, lo, hi, views in (("input", 0, nin, input_views), ("eval", nin, len(c_all), eval_views)):
         if hi > lo:
             out[name] = {"views": views, "c": c_all[lo:hi], "render": {k: v[:, lo:hi] for k, v in r.items()},
                          "targets": {k: v[lo:hi] for k, v in t_all.items()}, "table": table[lo:hi],
                          "metrics": derive(table[lo:hi])}
+            if perc is not None:
+                out[name]["perceptual"] = {k: v[lo:hi] for k, v in perc.items()}
     return out

@@ -486,6 +486,67 @@ int ga_recon_metrics(const float *image, const float *depth, const float *alpha,
                      const float *t_normal, int64_t t_normal_stride, int n_views, int H, int W, float *partial,
                      float *table, void *stream);
 
+/*
+ * ---------------------------------------------------------------------------
+ * Part 8: image-quality metrics.  LPIPS with the VGG16 backbone (the network and formulas of the reference's
+ * sgm/modules/autoencoding/lpips/loss/lpips.py, i.e. lpips.LPIPS(net="vgg", version="0.1") as nsr/losses/builder.py
+ * uses it) and SSIM (_ssim of nsr/losses/builder.py:23-55, size_average=False).  Inference only.
+ * LPIPS: ga_lpips_pack, then VGG16's 13 convolutions on ga_conv3x3_relu_bf16 (bf16 operands and activations, fp32
+ * accumulation) with ga_maxpool2x2_bf16 between the stages, ga_lpips_head on each of the five taps (relu1_2,
+ * relu2_2, relu3_3, relu4_3, relu5_3), then ga_lpips_reduce.  The head and the reduction run in fp32, SSIM's
+ * window sums in fp64.
+ * This file's kernels (lpips_ops.cu) are compiled without FMA contraction: every operation below is rounded to fp32 on
+ * its own, in the order written.
+ * ---------------------------------------------------------------------------
+ */
+/* ga_conv3x3_bf16 at stride 1 with no residual and a ReLU epilogue: out_bf16[m, :] = bf16(max(bias + conv, 0)),
+ * fp32 up to the final rounding.  Same arguments and checks as ga_conv3x3_bf16 (bias may be NULL). */
+int ga_conv3x3_relu_bf16(const void *x, int n, int H, int W, int Cin, const void *w_packed, int k_pitch,
+                         const float *bias, int Cout, void *out_bf16, void *stream);
+/* The two images of n pairs, in0 and in1 fp32 NCHW [n, 3, H, W] each -> out bf16 NHWC [2n, H, W, 8] (16-byte
+ * aligned): images 0..n-1 from in0, n..2n-1 from in1.  Per value x: x = 2 x - 1 when normalize != 0 (the package's
+ * normalize=True for [0, 1] input), then bf16((x - shift[c]) / scale[c]) (one fp32 subtraction and one fp32 division;
+ * shift, scale fp32 [3], device); channels 3-7 are 0.  The first VGG convolution then runs with Cin 8 (K 72,
+ * k_pitch 128) and zero weights for channels 3-7. */
+int ga_lpips_pack(const float *in0, const float *in1, int n, int H, int W, int normalize, const float *shift,
+                  const float *scale, void *out, void *stream);
+/* nn.MaxPool2d(2, 2) on bf16 NHWC: x [n, H, W, C] -> out [n, H / 2, W / 2, C] (floor), the max of each 2x2 window.
+ * Bit-exact for finite input.  C % 8 == 0, H, W >= 2, x and out 16-byte aligned. */
+int ga_maxpool2x2_bf16(const void *x, int n, int H, int W, int C, void *out, void *stream);
+#define GA_LPIPS_TAPS 5
+/* Blocks per pair of ga_lpips_head: its partial is fp32 [n, GA_LPIPS_HEAD_BLOCKS] per tap. */
+#define GA_LPIPS_HEAD_BLOCKS 128
+/* One LPIPS tap: feat bf16 NHWC [2n, H, W, C] (a ReLU output, 16-byte aligned), C in {64, 128, 256, 512};
+ * lin_w fp32 [C] (the tap's bias-free 1x1 NetLinLayer).  For pair i at each pixel, f0 = feat[i], f1 = feat[i + n]:
+ *   n0 = sqrt(sum_c f0_c * f0_c) + 1e-10,  n1 likewise          (NormalizeTensor, eps 1e-10)
+ *   d  = sum_c w_c * (t_c * t_c),  t_c = f0_c / n0 - f1_c / n1
+ * Channel sums: each of G = min(32, C / 8) lanes adds its channels in increasing order, then an xor butterfly
+ * over the G lanes.  partial[i * GA_LPIPS_HEAD_BLOCKS + b] = sum of d over pixels [b * per, (b + 1) * per) (per =
+ * ceil(H W / GA_LPIPS_HEAD_BLOCKS)) in a fixed order that depends on H and W only, so a pair's partials are the
+ * same bits whatever n is.  Swapping the two images gives the same bits; equal images give exactly 0.  No atomics. */
+int ga_lpips_head(const void *feat, int n, int H, int W, int C, const float *lin_w, float *partial, void *stream);
+/* partial fp32 [GA_LPIPS_TAPS, n, GA_LPIPS_HEAD_BLOCKS] (ga_lpips_head's output for tap k at partial + k n
+ * GA_LPIPS_HEAD_BLOCKS) -> out fp32 [n, GA_LPIPS_TAPS + 1]: out[i, k] = fp32(the fp64 sum of the tap's partials in
+ * block order / ((H >> k) (W >> k))), the tap's spatial mean (H, W: the input size; tap k is (H >> k) x (W >> k));
+ * out[i, 5] = (((out[i,0] + out[i,1]) + out[i,2]) + out[i,3]) + out[i,4] in fp32.  H >> 4 and W >> 4 >= 1. */
+int ga_lpips_reduce(const float *partial, int n, int H, int W, float *out, void *stream);
+#define GA_SSIM_WINDOW 11
+/* Bytes of scratch ga_ssim needs.  Host-only. */
+size_t ga_ssim_scratch_bytes(int n, int H, int W);
+/* SSIM of n image pairs, img1 and img2 fp32 [n, 3, H, W] -> out fp32 [n], the mean of the SSIM map over C, H and W.
+ * window fp32 [11, 11] (device): create_window(11, .)'s values, g g^T of the normalised fp32 Gaussian (sigma 1.5),
+ * computed by the caller.  The kernel uses this 2D window (not the separable form).  With zero padding of 5, in fp64
+ * (the fp32 window and pixels widened; E[x^2] - mu^2 in fp32 would cancel to SSIM errors of ~2e-5):
+ *   mu1 = sum w x, mu2 = sum w y, e11 = sum w (x x), e22 = sum w (y y), e12 = sum w (x y)
+ *        taps in row-major order, each step one fp64 fma (x x, y y, x y are exact in fp64)
+ *   mu1_sq = mu1 mu1, mu2_sq = mu2 mu2, mu1_mu2 = mu1 mu2
+ *   s1 = e11 - mu1_sq, s2 = e22 - mu2_sq, s12 = e12 - mu1_mu2
+ *   map = fp32(((2 mu1_mu2 + C1) (2 s12 + C2)) / ((mu1_sq + mu2_sq + C1) (s1 + s2 + C2))), C1 = 0.01^2, C2 = 0.03^2
+ * The map is summed per 16 x 16 block in fp32 (fixed order), the block sums of an image in fp64, and out =
+ * fp32(sum / (3 H W)).  Equal images give exactly 1; the same inputs give the same bits.  n <= 21845. */
+int ga_ssim(const float *img1, const float *img2, int n, int H, int W, const float *window, void *scratch,
+            size_t scratch_bytes, float *out, void *stream);
+
 /* Measurement aid: when enabled, cudaEvents are recorded around every kernel
  * stage of the next forward/backward; ga_profile_read synchronises on them and
  * returns per-stage milliseconds: [0] preprocess, [1] binning, [2] render fwd,
