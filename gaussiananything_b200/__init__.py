@@ -42,3 +42,7 @@ def install_shims(replace_classes: bool = True):
             from . import mesh as _mesh
             m.FlowMatchingEngine.extract_mesh_bounded = _mesh._engine_extract_mesh_bounded
             m.FlowMatchingEngine.export_mesh_from_2dgs = _mesh._engine_export_mesh_from_2dgs
+        m = sys.modules.get("nsr.losses.builder")
+        if m is not None:
+            from . import lpips as _lpips
+            m.LPIPSLoss = _lpips.LPIPSLoss

@@ -103,6 +103,9 @@ ABI = {
     "ga_lpips_reduce": (i32, [vp, i32, i32, i32, vp, vp]),
     "ga_ssim_scratch_bytes": (sz, [i32, i32, i32]),
     "ga_ssim": (i32, [vp, vp, i32, i32, i32, vp, vp, sz, vp, vp]),
+    "ga_conv3x3_mask_bf16": (i32, [vp, i32, i32, i32, i32, vp, i32, i32, vp, vp, vp]),
+    "ga_lpips_tap_backward": (i32, [vp, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp]),
+    "ga_lpips_input_backward": (i32, [vp, i32, i32, i32, vp, vp, i32, vp, vp]),
     "ga_profile_enable": (i32, [i32]),
     "ga_profile_read": (i32, [C.POINTER(f32), i32]),
     "ga_b200_version": (C.c_char_p, []),

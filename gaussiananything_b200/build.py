@@ -27,6 +27,8 @@ EXTRA = {
     "gbuffer_ops.cu": ["--fmad=false"],
     # LPIPS pack / head and SSIM: every operation rounded on its own, as include/ga_b200.h Part 8 states them
     "lpips_ops.cu": ["--fmad=false"],
+    # LPIPS tap and input backward: every operation rounded on its own, as include/ga_b200.h Part 9 states them
+    "lpips_grad.cu": ["--fmad=false"],
 }
 
 

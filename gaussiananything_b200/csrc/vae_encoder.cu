@@ -11,8 +11,9 @@ using namespace sm90;
 namespace {
 
 // ---------------------------------------------------------------------------------------------------------------
-// 3x3 convolution, implicit GEMM: out[m, n] = bias[n] + sum_k A[m, k] W[n, k] (+ residual[m, n]), then max(., 0)
-// when RELU,
+// 3x3 convolution, implicit GEMM: out[m, n] = bias[n] + sum_k A[m, k] W[n, k] (+ residual[m, n]), then the epilogue
+// EPI: kEpiNone as is, kEpiRelu max(., 0), kEpiMask mask[m, n] > 0 ? . : 0 (a select: the ReLU backward, where mask is
+// the forward's ReLU output, so a non-finite value never leaks through a masked zero),
 // m = (image, oy, ox), k = (ky * 3 + kx) * Cin + c.  A is never materialised: every 16-byte piece (8 channels of one
 // tap of one output pixel) is gathered with cp.async straight from the NHWC input, zero-filled where the tap falls
 // into the padding or k runs past 9 * Cin.  The pieces land in the 128-byte-swizzled K-major layout that
@@ -38,7 +39,10 @@ struct ConvArgs {
     float *out_f32;             // [M, Cout] or NULL
     __nv_bfloat16 *out_bf16;    // [M, Cout] or NULL
     int H, W, Cin, Ho, Wo, Cout, k_pitch, stride, M, K;
+    const __nv_bfloat16 *mask;  // [M, Cout] for kEpiMask
 };
+
+constexpr int kEpiNone = 0, kEpiRelu = 1, kEpiMask = 2;
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid)
 {
@@ -49,7 +53,7 @@ template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile(
 // cp.async writes through the generic proxy, wgmma reads through the async proxy
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 
-template <int BN, bool RELU>
+template <int BN, int EPI>
 __global__ void __launch_bounds__(kConvThreads, 1) conv3x3_kernel(const ConvArgs a)
 {
     using Cfg = ConvCfg<BN>;
@@ -151,7 +155,12 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv3x3_kernel(const ConvArgs
                 const float2 rr = *reinterpret_cast<const float2 *>(a.residual + o);
                 v0 += rr.x; v1 += rr.y;
             }
-            if (RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            if (EPI == kEpiRelu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            if (EPI == kEpiMask) {
+                const float2 mk = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(a.mask + o));
+                v0 = mk.x > 0.f ? v0 : 0.f;
+                v1 = mk.y > 0.f ? v1 : 0.f;
+            }
             if (a.out_f32) *reinterpret_cast<float2 *>(a.out_f32 + o) = make_float2(v0, v1);
             if (a.out_bf16) *reinterpret_cast<__nv_bfloat162 *>(a.out_bf16 + o) = __floats2bfloat162_rn(v0, v1);
         }
@@ -463,18 +472,18 @@ __global__ void __launch_bounds__(kHeadThreads) readout_head_kernel(const GaVaeE
 }  // namespace
 
 // ---- host side ----------------------------------------------------------------------------------------------------
-template <int BN, bool RELU>
+template <int BN, int EPI>
 static int launch_conv(const ConvArgs &a, cudaStream_t s)
 {
     using Cfg = ConvCfg<BN>;
     static GaPerDevice attr_set;
     if (ga_first_use_on_device(attr_set)) {
-        cudaError_t e = cudaFuncSetAttribute(conv3x3_kernel<BN, RELU>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        cudaError_t e = cudaFuncSetAttribute(conv3x3_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                              Cfg::kSmem);
         if (e != cudaSuccess) return (int)e;
     }
     dim3 grid((a.M + CBM - 1) / CBM, a.Cout / BN);
-    return (int)ga_launch_pdl(conv3x3_kernel<BN, RELU>, grid, dim3(kConvThreads), (size_t)Cfg::kSmem, s, a);
+    return (int)ga_launch_pdl(conv3x3_kernel<BN, EPI>, grid, dim3(kConvThreads), (size_t)Cfg::kSmem, s, a);
 }
 
 // the argument checks of both conv entry points; fills `a` and returns 0, or the error code
@@ -495,6 +504,7 @@ static int conv_args(ConvArgs &a, const void *x, int n, int H, int W, int Cin, c
     a.out_bf16 = reinterpret_cast<__nv_bfloat16 *>(out_bf16);
     a.H = H; a.W = W; a.Cin = Cin; a.Ho = Ho; a.Wo = Wo; a.Cout = Cout; a.k_pitch = k_pitch; a.stride = stride;
     a.M = n * Ho * Wo; a.K = 9 * Cin;
+    a.mask = nullptr;
     return 0;
 }
 
@@ -514,7 +524,7 @@ extern "C" int ga_conv3x3_bf16(const void *x, int n, int H, int W, int Cin, cons
     const int rc = conv_args(a, x, n, H, W, Cin, w_packed, k_pitch, bias, Cout, stride, residual, out_f32, out_bf16);
     if (rc) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    return Cout % 128 == 0 ? launch_conv<128, false>(a, s) : launch_conv<64, false>(a, s);
+    return Cout % 128 == 0 ? launch_conv<128, kEpiNone>(a, s) : launch_conv<64, kEpiNone>(a, s);
 }
 
 extern "C" int ga_conv3x3_relu_bf16(const void *x, int n, int H, int W, int Cin, const void *w_packed, int k_pitch,
@@ -524,7 +534,19 @@ extern "C" int ga_conv3x3_relu_bf16(const void *x, int n, int H, int W, int Cin,
     const int rc = conv_args(a, x, n, H, W, Cin, w_packed, k_pitch, bias, Cout, 1, nullptr, nullptr, out_bf16);
     if (rc) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    return Cout % 128 == 0 ? launch_conv<128, true>(a, s) : launch_conv<64, true>(a, s);
+    return Cout % 128 == 0 ? launch_conv<128, kEpiRelu>(a, s) : launch_conv<64, kEpiRelu>(a, s);
+}
+
+extern "C" int ga_conv3x3_mask_bf16(const void *x, int n, int H, int W, int Cin, const void *w_packed, int k_pitch,
+                                    int Cout, const void *mask, void *out_bf16, void *stream)
+{
+    ConvArgs a;
+    if (!mask || (reinterpret_cast<uintptr_t>(mask) & 3)) return GA_ERR_BADARG;
+    const int rc = conv_args(a, x, n, H, W, Cin, w_packed, k_pitch, nullptr, Cout, 1, nullptr, nullptr, out_bf16);
+    if (rc) return rc;
+    a.mask = reinterpret_cast<const __nv_bfloat16 *>(mask);
+    cudaStream_t s = (cudaStream_t)stream;
+    return Cout % 128 == 0 ? launch_conv<128, kEpiMask>(a, s) : launch_conv<64, kEpiMask>(a, s);
 }
 
 extern "C" size_t ga_group_norm_scratch_bytes(int n, int HW)

@@ -4,12 +4,15 @@
           objective (nsr/losses/builder.py LPIPSLoss; the same network and formulas as
           sgm/modules/autoencoding/lpips/loss/lpips.py): ScalingLayer, VGG16 `features` cut at relu1_2 .. relu5_3,
           unit-normalised features (eps 1e-10), squared difference, a bias-free 1x1 NetLinLayer per tap, spatial mean,
-          sum over the five taps.  Inference only.
+          sum over the five taps.
+  LPIPSLoss  mirrors LPIPSLoss of nsr/losses/builder.py: loss_weight * LPIPS(target, pred).mean(), differentiable
+          in pred and / or target through the Part 9 backward (input gradients only; the network is frozen).
   ssim    _ssim of nsr/losses/builder.py with create_window(11, 3) and size_average=False: per-image SSIM.
 
 Precision: the 13 convolutions take bf16 operands and keep bf16 ReLU outputs (fp32 accumulation), as every network
 here; the head and the reductions run in fp32.  Rounding noise enters LPIPS squared, so the bf16 error is a small
-positive bias (INTEGRATION.md section 3g).
+positive bias (INTEGRATION.md section 3g).  The backward keeps bf16 gradients between the convolutions, fp32 at the
+pooled maps, the head and the input (INTEGRATION.md section 3h).
 
 Weights are never downloaded: state_dict= (the LPIPS module layout), or vgg_path= / lin_path=, or the default local
 files torch.hub.get_dir()/checkpoints/vgg16-397923af.pth (torchvision's VGG16) and .../checkpoints/vgg.pth (the
@@ -119,7 +122,7 @@ def gaussian_window(window_size=SSIM_WINDOW, sigma=1.5):
     return g.mm(g.t()).float()
 
 
-def _check_pair(in0, in1, what, min_size=1):
+def _check_pair(in0, in1, what, min_size=1, allow_grad=False):
     if in0.dim() != 4 or in0.shape[1] != 3:
         raise ValueError("%s: expected images [N, 3, H, W], got %s" % (what, tuple(in0.shape)))
     if tuple(in0.shape) != tuple(in1.shape):
@@ -128,7 +131,7 @@ def _check_pair(in0, in1, what, min_size=1):
         raise ValueError("%s: N must be positive and H, W at least %d, got %s" % (what, min_size, tuple(in0.shape)))
     if not (in0.is_cuda and in1.is_cuda):
         raise RuntimeError("%s runs on CUDA tensors (there is no CPU fallback)" % what)
-    if torch.is_grad_enabled() and (in0.requires_grad or in1.requires_grad):
+    if not allow_grad and torch.is_grad_enabled() and (in0.requires_grad or in1.requires_grad):
         raise RuntimeError("%s is inference-only (no autograd through the CUDA kernels): call it under torch.no_grad() "
                            "or on detached inputs" % what)
 
@@ -196,6 +199,12 @@ class LPIPS:
             self.convs.append(dict(tap=k, cin=cp, cout=cout, kp=kp, w=packed.to(device=dev, dtype=torch.bfloat16),
                                    b=f32(sd["net.slice%d.%d.bias" % (k + 1, i)]),
                                    last=j + 1 == len(CONVS) or CONVS[j + 1][0] != k))    # its ReLU is tap k
+            if j:                                            # the dgrad's weights (include/ga_b200.h Part 9)
+                wf, self.convs[-1]["kpf"] = flip_pack(w)
+                self.convs[-1]["wf"] = wf.to(dev)
+        # features.0's dgrad in ga_lpips_input_backward: w_flip [9, 64, 3] = W0[co, c, 2 - ky, 2 - kx]
+        w0 = sd["net.slice1.0.weight"].detach().float().cpu().to(torch.bfloat16).float()
+        self.w0_flip = w0.flip(2, 3).permute(2, 3, 0, 1).reshape(9, CHNS[0], 3).contiguous().to(dev)
         self.lin = [f32(sd["lin%d.model.1.weight" % k].reshape(-1)) for k in range(TAPS)]
         self._graphs = _launch.GraphCache("GA_B200_LPIPS_GRAPH")          # (chunk, H, W) -> graph
 
@@ -265,3 +274,141 @@ class LPIPS:
         return val
 
     __call__ = forward
+
+    # ---- differentiable values (LPIPSLoss): Part 9
+    def values(self, in0, in1, normalize=False):
+        """Per-pair LPIPS [N, 1, 1, 1], differentiable in whichever input requires grad (with grad mode on).
+        Otherwise it is forward(): the graphs run and nothing is saved."""
+        if not (torch.is_grad_enabled() and (in0.requires_grad or in1.requires_grad)):
+            return self.forward(in0, in1, normalize=normalize)
+        _check_pair(in0, in1, "LPIPS", MIN_SIZE, allow_grad=True)
+        sides = tuple(s for s, t in enumerate((in0, in1)) if t.requires_grad)
+        f = lambda t: t.to(device=self.device, dtype=torch.float32).contiguous()
+        return _LPIPSGrad.apply(self, bool(normalize), sides, f(in0), f(in1)).reshape(-1, 1, 1, 1)
+
+    def _forward_saving(self, in0, in1, normalize, sides):
+        """One chunk of n pairs, launched eagerly into fresh tensors that belong to the caller: the [n, 6] table, the
+        five taps [2n, h, w, C], and for each side in `sides` its 13 ReLU outputs [n, h, w, C] (the taps as views).
+        The two sides run their convolutions apart, so the other side's inner activations are freed as they go; a
+        convolution's pixels do not depend on the batch, so the values are forward()'s bits."""
+        n, _, H, W = in0.shape
+        dev, L = self.device, self.L
+        st = _launch.stream(dev)
+        x = torch.empty(2 * n, H, W, 8, device=dev, dtype=torch.bfloat16)
+        _lib.check(L.ga_lpips_pack(_p(in0), _p(in1), n, H, W, int(bool(normalize)), _p(self.shift), _p(self.scale),
+                                   _p(x), st), "ga_lpips_pack")
+        partial = torch.empty(TAPS, n, HEAD_BLOCKS, device=dev)
+        xs, taps, acts = [x[:n], x[n:]], [], {s: [] for s in sides}
+        h, w, tap = H, W, 0
+        for cv in self.convs:
+            if cv["tap"] != tap:
+                y = torch.empty(2 * n, h // 2, w // 2, cv["cin"], device=dev, dtype=torch.bfloat16)
+                _lib.check(L.ga_maxpool2x2_bf16(_p(taps[-1]), 2 * n, h, w, cv["cin"], _p(y), st), "ga_maxpool2x2_bf16")
+                xs, h, w, tap = [y[:n], y[n:]], h // 2, w // 2, cv["tap"]
+            if cv["last"]:
+                y = torch.empty(2 * n, h, w, cv["cout"], device=dev, dtype=torch.bfloat16)
+                ys = [y[:n], y[n:]]
+            else:
+                ys = [torch.empty(n, h, w, cv["cout"], device=dev, dtype=torch.bfloat16) for _ in range(2)]
+            for s in range(2):
+                _lib.check(L.ga_conv3x3_relu_bf16(_p(xs[s]), n, h, w, cv["cin"], _p(cv["w"]), cv["kp"], _p(cv["b"]),
+                                                  cv["cout"], _p(ys[s]), st), "ga_conv3x3_relu_bf16")
+                if s in acts:
+                    acts[s].append(ys[s])
+            xs = ys
+            if cv["last"]:
+                _lib.check(L.ga_lpips_head(_p(y), n, h, w, cv["cout"], _p(self.lin[tap]), _p(partial[tap]), st),
+                           "ga_lpips_head")
+                taps.append(y)
+        out = torch.empty(n, TAPS + 1, device=dev)
+        _lib.check(L.ga_lpips_reduce(_p(partial), n, H, W, _p(out), st), "ga_lpips_reduce")
+        return {"out": out, "taps": taps, "acts": acts, "n": n, "H": H, "W": W}
+
+    def _backward_side(self, saved, side, g, normalize, dx):
+        """d(sum_i g_i LPIPS_i) / d(images of `side`) of one chunk into dx fp32 [n, 3, H, W] (contiguous)."""
+        n, H, W = saved["n"], saved["H"], saved["W"]
+        acts, taps = saved["acts"][side], saved["taps"]
+        dev, L = self.device, self.L
+        st = _launch.stream(dev)
+        grad, dpool = None, None                 # bf16 at the current conv's pre-activation; fp32 at a pooled map
+        for j in range(len(self.convs) - 1, -1, -1):
+            cv = self.convs[j]
+            k = cv["tap"]
+            h, w = H >> k, W >> k
+            if cv["last"]:
+                grad = torch.empty(n, h, w, cv["cout"], device=dev, dtype=torch.bfloat16)
+                _lib.check(L.ga_lpips_tap_backward(_p(taps[k]), n, h, w, cv["cout"], side, _p(self.lin[k]), _p(g),
+                                                   _p(dpool), _p(grad), st), "ga_lpips_tap_backward")
+            if j == 0:
+                _lib.check(L.ga_lpips_input_backward(_p(grad), n, H, W, _p(self.w0_flip), _p(self.scale),
+                                                     int(bool(normalize)), _p(dx), st), "ga_lpips_input_backward")
+                break
+            if self.convs[j - 1]["tap"] == k:    # inside the slice: through the lower conv's ReLU
+                out = torch.empty(n, h, w, cv["cin"], device=dev, dtype=torch.bfloat16)
+                _lib.check(L.ga_conv3x3_mask_bf16(_p(grad), n, h, w, cv["cout"], _p(cv["wf"]), cv["kpf"], cv["cin"],
+                                                  _p(acts[j - 1]), _p(out), st), "ga_conv3x3_mask_bf16")
+                grad = out
+            else:                                # the slice's first conv: to the pooled map of tap k - 1, fp32
+                dpool = torch.empty(n, h, w, cv["cin"], device=dev)
+                _lib.check(L.ga_conv3x3_bf16(_p(grad), n, h, w, cv["cout"], _p(cv["wf"]), cv["kpf"], None, cv["cin"],
+                                             1, None, _p(dpool), None, st), "ga_conv3x3_bf16")
+                grad = None
+
+
+def flip_pack(w):
+    """The dgrad weights of a 3x3 convolution W [Co, Ci, 3, 3] (fp32, CPU): bf16 [Ci, kp] in the packed layout with
+    Cout = Ci, Cin = Co, column (ky * 3 + kx) * Co + co = W[co, ci, 2 - ky, 2 - kx]; and kp = 9 Co rounded up to 64."""
+    co, ci = w.shape[:2]
+    kp = _launch.round_up(9 * co, 64)
+    packed = torch.zeros(ci, kp)
+    packed[:, :9 * co] = w.flip(2, 3).permute(1, 2, 3, 0).reshape(ci, 9 * co)
+    return packed.to(torch.bfloat16), kp
+
+
+class _LPIPSGrad(torch.autograd.Function):
+    """Per-pair LPIPS [N] of fp32 contiguous in0, in1 with the activations saved for `sides`, pairs `chunk` at a
+    time; backward runs the Part 9 chain per chunk and side.  The saved tensors belong to this context (allocated per
+    call, never a graph's buffers) and are freed with the autograd graph."""
+
+    @staticmethod
+    def forward(ctx, model, normalize, sides, in0, in1):
+        N = in0.shape[0]
+        with torch.cuda.device(model.device):
+            chunks = [model._forward_saving(in0[s:s + model.chunk], in1[s:s + model.chunk], normalize, sides)
+                      for s in range(0, N, model.chunk)]
+        ctx.model, ctx.normalize, ctx.sides, ctx.chunks, ctx.shape = model, normalize, sides, chunks, tuple(in0.shape)
+        return torch.cat([c["out"][:, TAPS] for c in chunks])
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gval):
+        model, chunks = ctx.model, ctx.chunks
+        g = gval.to(device=model.device, dtype=torch.float32).contiguous()
+        dx = [torch.empty(ctx.shape, device=model.device) if s in ctx.sides else None for s in range(2)]
+        with torch.cuda.device(model.device):
+            s0 = 0
+            for c in chunks:
+                n = c["n"]
+                for s in ctx.sides:
+                    model._backward_side(c, s, g[s0:s0 + n], ctx.normalize, dx[s][s0:s0 + n])
+                s0 += n
+        return None, None, None, dx[0], dx[1]
+
+
+class LPIPSLoss(torch.nn.Module):
+    """LPIPSLoss of nsr/losses/builder.py on the library's LPIPS: forward(pred, target) = loss_weight *
+    LPIPS(target, pred).mean(), a 0-dim fp32 tensor, differentiable in whichever of pred and target requires grad.
+    Inputs may be non-contiguous views (the reference's centre crops) of any float dtype; gradients come back in the
+    input's dtype and shape.  `lpips=` takes an existing LPIPS; otherwise one is built from the local weight files
+    (raising as LPIPS does when they are absent).  use_input_norm and range_norm are accepted and unused, as in the
+    reference; so is conf_sigma_percl."""
+
+    def __init__(self, loss_weight=1.0, use_input_norm=True, range_norm=True, lpips=None):
+        super().__init__()
+        self.perceptual = lpips if lpips is not None else LPIPS(net="vgg", spatial=False)
+        self.loss_weight = loss_weight
+        self.use_input_norm = use_input_norm
+        self.range_norm = range_norm
+
+    def forward(self, pred, target, conf_sigma_percl=None):
+        return self.loss_weight * self.perceptual.values(target, pred).mean()

@@ -547,6 +547,57 @@ size_t ga_ssim_scratch_bytes(int n, int H, int W);
 int ga_ssim(const float *img1, const float *img2, int n, int H, int W, const float *window, void *scratch,
             size_t scratch_bytes, float *out, void *stream);
 
+/*
+ * ---------------------------------------------------------------------------
+ * Part 9: LPIPS backward, the input gradients of Part 8's LPIPS (the network is frozen: no weight gradients).  For
+ * the per-pair values v_i of the forward and upstream weights g_i (fp32, device; autograd's incoming gradient), the
+ * gradient of sum_i g_i v_i with respect to the images of one side: side 0 is in0 (images 0..n-1 of the packed
+ * batch), side 1 is in1 (images n..2n-1), each computed only when asked for.  Per side, from the last layer down:
+ *   tap 4:  ga_lpips_tap_backward without dpool -> the gradient at conv 12's pre-activation (bf16)
+ *   inside a slice: ga_conv3x3_mask_bf16 with the flipped weights of the conv above and the ReLU output of the conv
+ *           below as mask -> the gradient at the lower conv's pre-activation (bf16)
+ *   the first conv of slices 1-4: ga_conv3x3_bf16 (stride 1, no bias, out_f32) with its flipped weights -> the
+ *           gradient at the pooled map (fp32), then ga_lpips_tap_backward of the tap below with that dpool
+ *   conv 0: ga_lpips_input_backward -> fp32 NCHW gradients of the images.
+ * Flipped weights of a conv with weight W [Co, Ci, 3, 3]: the Part 5 packed layout with Cout = Ci and Cin = Co,
+ * W'[ci, (ky * 3 + kx) * Co + co] = bf16(W[co, ci, 2 - ky, 2 - kx]): the dgrad of a stride-1 pad-1 3x3 convolution is
+ * the stride-1 pad-1 3x3 convolution with these weights.  Accumulation in fp32; no atomics and no loss scaling (bf16
+ * has fp32's exponent range), so the same inputs give the same bits whatever n and the chunking.
+ * lpips_grad.cu is compiled without FMA contraction: every operation below is rounded to fp32 on its own, in the
+ * order written.  The convolutions follow Part 5 (fp32 accumulation in the wgmma's order).
+ * ---------------------------------------------------------------------------
+ */
+/* ga_conv3x3_bf16 at stride 1 with no bias or residual and a ReLU-mask epilogue: out_bf16[m, c] =
+ * bf16(mask[m, c] > 0 ? conv : 0), a select (a non-finite conv value never leaks through a masked zero).  mask bf16
+ * [n, H, W, Cout] (4-byte aligned).  Other arguments and checks as ga_conv3x3_bf16. */
+int ga_conv3x3_mask_bf16(const void *x, int n, int H, int W, int Cin, const void *w_packed, int k_pitch, int Cout,
+                         const void *mask, void *out_bf16, void *stream);
+/* One tap's backward for one side.  feat: the tap, bf16 NHWC [2n, H, W, C] as ga_lpips_head reads it (16-byte
+ * aligned), C in {64, 128, 256, 512}; lin_w fp32 [C]; g fp32 [n] (device).  For pair i at each pixel, f = feat[side n
+ * + i] (this side), f' = feat[(1 - side) n + i] (the other), with the head's channel sums (G lanes, each in increasing
+ * channel order, then an xor butterfly):
+ *   r = sqrt(sum_c f_c f_c), nf = r + 1e-10, nf' = sqrt(sum_c f'_c f'_c) + 1e-10
+ *   t_c = f_c / nf - f'_c / nf',  u_c = 2 (w_c t_c),  S = sum_c u_c f_c,  s = g_i / fp32(H W),  q = (S / nf) / nf
+ *   head_c = s (u_c / nf - (f_c / r) q)  where r > 0, else 0 (the reference's normalize_tensor gives NaN at an all-zero
+ *            vector, and its ReLU backward, a select, turns that into 0)
+ * The same code serves both sides, so swapping the two images swaps the sides' gradients with the same bits.
+ * dpool: NULL, or the fp32 gradient at this tap's 2x2 max pool, NHWC [n, H / 2, W / 2, C] (16-byte aligned): the
+ * pooled gradient goes to the window's first maximum of f in row-major order (torch's max_pool2d rule); the row and
+ * column the floor drops (odd H or W) get none.  Out: grad bf16 NHWC [n, H, W, C] (16-byte aligned) =
+ *   bf16(f_c > 0 ? routed_c + head_c : 0),
+ * the gradient at the pre-activation of the conv whose ReLU output the tap is.  H W <= 2^24. */
+int ga_lpips_tap_backward(const void *feat, int n, int H, int W, int C, int side, const float *lin_w, const float *g,
+                          const float *dpool, void *grad, void *stream);
+/* The dgrad of VGG's first convolution (3 -> 64) fused with the backward of ga_lpips_pack.  g0 bf16 NHWC
+ * [n, H, W, 64] (16-byte aligned): the gradient at conv 0's pre-activation; w_flip fp32 [9, 64, 3] (device),
+ * w_flip[ky * 3 + kx, co, c] = bf16(W0[co, c, 2 - ky, 2 - kx]) as fp32.  Per pixel and c < 3:
+ *   acc_c = sum over taps (ky, kx) in row-major order, inside the image, of sum over co in increasing order of
+ *           w_flip[ky * 3 + kx, co, c] * g0[y + ky - 1, x + kx - 1, co]
+ *   dx[i, c, y, x] = acc_c / scale[c], then * 2 when normalize != 0        (fp32 NCHW [n, 3, H, W])
+ * (the straight-through gradient of the pack's bf16 rounding).  n <= 65535. */
+int ga_lpips_input_backward(const void *g0, int n, int H, int W, const float *w_flip, const float *scale,
+                            int normalize, float *dx, void *stream);
+
 /* Measurement aid: when enabled, cudaEvents are recorded around every kernel
  * stage of the next forward/backward; ga_profile_read synchronises on them and
  * returns per-stage milliseconds: [0] preprocess, [1] binning, [2] render fwd,
