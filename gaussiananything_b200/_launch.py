@@ -1,6 +1,8 @@
 """Host-side launch policy shared by the networks that run on the transformer kernels (dit, dino, vae_decoder,
 vae_encoder): argument formats of the GEMM entry point, its tile width, and CUDA-graph capture and replay."""
+import contextlib
 import ctypes as C
+import gc
 import os
 
 import torch
@@ -73,17 +75,32 @@ def gemm(A, W, M, N, K, epi, stream, block_n=None):
     _lib.check(_lib.lib().ga_gemm_bf16_tn(ptr(A), K, ptr(W), K, M, N, K, C.byref(epi), bn, stream), "ga_gemm_bf16_tn")
 
 
+@contextlib.contextmanager
+def no_cyclic_gc():
+    """Python's cyclic garbage collector off for the block (restored after).  A network that is no longer referenced
+    but sits in a reference cycle (its graph cache's closures point back at it) is freed by the collector, at whatever
+    allocation triggers it; if that happens inside a capture, its CUDA graph's memory pool is released with cudaFree on
+    the capturing thread, which invalidates the capture."""
+    was = gc.isenabled()
+    gc.disable()
+    try:
+        yield
+    finally:
+        if was:
+            gc.enable()
+
+
 def capture(launches, device):
     """Runs `launches()` once eagerly (first-use kernel attributes are set there), then captures it into a new CUDA
-    graph.  Returns (graph, what launches() returned inside the capture).  Tensors made here are not inference tensors,
-    so the graph may be replayed from either mode."""
+    graph, with the cyclic garbage collector off (no_cyclic_gc).  Returns (graph, what launches() returned inside the
+    capture).  Tensors made here are not inference tensors, so the graph may be replayed from either mode."""
     with torch.inference_mode(False), torch.no_grad():
         launches()
         torch.cuda.synchronize(device)
         g = torch.cuda.CUDAGraph()
         # thread_local: another thread of the process (NCCL's watchdog under torch.distributed) may issue CUDA calls
         # while this one captures
-        with torch.cuda.graph(g, capture_error_mode="thread_local"):
+        with no_cyclic_gc(), torch.cuda.graph(g, capture_error_mode="thread_local"):
             out = launches()
     return g, out
 

@@ -106,6 +106,10 @@ ABI = {
     "ga_conv3x3_mask_bf16": (i32, [vp, i32, i32, i32, i32, vp, i32, i32, vp, vp, vp]),
     "ga_lpips_tap_backward": (i32, [vp, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp]),
     "ga_lpips_input_backward": (i32, [vp, i32, i32, i32, vp, vp, i32, vp, vp]),
+    "ga_fps_ex_workspace_bytes": (sz, [i32, i32, i32]),
+    "ga_fps_ex": (i32, [vp, vp, i32, i32, i32, vp, vp, vp, vp, sz, vp]),
+    "ga_chunk_surface_points_scratch_bytes": (sz, [i32, i32, i32]),
+    "ga_chunk_surface_points": (i32, [vp, vp, vp, i32, i32, i32, vp, i32, i32, f32, vp, vp, vp, sz, vp]),
     "ga_profile_enable": (i32, [i32]),
     "ga_profile_read": (i32, [C.POINTER(f32), i32]),
     "ga_b200_version": (C.c_char_p, []),

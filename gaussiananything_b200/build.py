@@ -29,6 +29,8 @@ EXTRA = {
     "lpips_ops.cu": ["--fmad=false"],
     # LPIPS tap and input backward: every operation rounded on its own, as include/ga_b200.h Part 9 states them
     "lpips_grad.cu": ["--fmad=false"],
+    # chunk surface points (gbuffer_pack_kernel's unprojection to the bit) and FPS distances, include/ga_b200.h Part 10
+    "pcd_ops.cu": ["--fmad=false"],
 }
 
 

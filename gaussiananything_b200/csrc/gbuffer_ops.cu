@@ -6,13 +6,13 @@
 // deployed configuration; the rounding of every step is stated in include/ga_b200.h and restated by
 // oracle/gbuffer_oracle.py.  This file is compiled without FMA contraction so that the stated roundings hold.
 #include "../../include/ga_b200.h"
+#include "gbuffer_common.cuh"
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
 
 namespace {
 
-constexpr float XYZ_CLIP = 0.45f;
 // torchvision Normalize with the ImageNet statistics (PostProcess.__init__ with imgnet_normalize=True, which is what
 // load_eval_data's chunk branch passes)
 __constant__ float RGB_MEAN[3] = {0.485f, 0.456f, 0.406f};
@@ -77,7 +77,7 @@ gbuffer_pack_kernel(PackArgs a)
     }
 
     const float ox = cam[3], oy = cam[7], oz = cam[11];
-    const float fx = cam[16], sk = cam[17], cx = cam[18], fy = cam[20], cy = cam[21];
+    const float fx = cam[16], cx = cam[18], fy = cam[20], cy = cam[21];
     const float v_cam = ((float)y + 0.5f) / (float)H;
     float pl[6][4], xyz[3][4];
 #pragma unroll
@@ -98,21 +98,10 @@ gbuffer_pack_kernel(PackArgs a)
         pl[3][i] = dx;
         pl[4][i] = dy;
         pl[5][i] = dz;
-        // RaySampler: lift with the skew term, transform the point by the whole c2w, subtract the origin, normalise
-        const float lx = (u_cam - cx + cy * sk / fy - sk * v_cam / fy) / fx, ly = (v_cam - cy) / fy;
-        float rx = cam[0] * lx + cam[1] * ly + cam[2] + cam[3] - ox;
-        float ry = cam[4] * lx + cam[5] * ly + cam[6] + cam[7] - oy;
-        float rz = cam[8] * lx + cam[9] * ly + cam[10] + cam[11] - oz;
-        const float rn = fmaxf(sqrtf(rx * rx + ry * ry + rz * rz), 1e-12f);
-        rx = rx / rn;
-        ry = ry / rn;
-        rz = rz / rn;
-        const float p[3] = {ox + d4[i] * rx, oy + d4[i] * ry, oz + d4[i] * rz};
+        float p[3];
+        gbuf::unproject(cam, u_cam, v_cam, d4[i], p);
 #pragma unroll
-        for (int c = 0; c < 3; c++) {
-            const float q = fminf(fmaxf(p[c], -XYZ_CLIP), XYZ_CLIP);
-            xyz[c][i] = fabsf(q) == XYZ_CLIP ? 0.0f : q;
-        }
+        for (int c = 0; c < 3; c++) xyz[c][i] = p[c];
     }
 #pragma unroll
     for (int c = 0; c < 6; c++) store4(enc + (6 + c) * HW, pl[c][0], pl[c][1], pl[c][2], pl[c][3]);

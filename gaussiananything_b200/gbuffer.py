@@ -4,14 +4,15 @@
 A chunk folder holds 16 posed views of one object as the reference's dataset stores them
 (datasets/g_buffer_objaverse.py read_chunk :3225-3302): raw_img.jpg and normal.png with the views side by side,
 alpha.jpg likewise, depth.npz ['depth'] fp32 [16, h, w], c.npy fp32 [16, 25] (c2w 16 | normalised K 9), bbox.npy,
-caption.txt, ins.txt; the object's surface samples are a separate fps-4096.ply.
+caption.txt, ins.txt; the object's surface samples are a separate fps-4096.ply, or are made from the depth maps by
+pcd.chunk_surface_pcd.
 
   read_chunk / read_fps_pcd   decode the files on the host (PIL and numpy; the PLY is parsed here)
   pack                        one launch of ga_gbuffer_pack: img_to_encoder [V, 15, H, W] and the render targets
   cameras                     the chunk's c rows in the renderer's camera format (mesh.orbit_cameras)
   metrics                     ga_recon_metrics on rendered maps against the targets -> per-view numbers
   perceptual_metrics          per-view LPIPS (VGG) and SSIM of the rendered images against the targets (lpips.py)
-  reconstruct_chunk           pack -> encode -> decode -> render at the chunk's own cameras -> metrics
+  reconstruct_chunk           (surface cloud, pcd.py, when none is given) -> pack -> encode -> decode -> render at the chunk's own cameras -> metrics
                               (SurfelAE behaviour 'reconstruct_chunk')
 
 Deployed configuration only: the files' size == reso_encoder == reso == 512, cameras used as stored
@@ -235,11 +236,12 @@ def perceptual_metrics(render_out, targets, lpips_model):
     return {"lpips": lpips_model(img * 2 - 1, t).reshape(-1), "ssim": ssim(img, (t + 1) / 2)}
 
 
-def reconstruct_chunk(ae, chunk, pcd, input_views=range(8), eval_views=range(8, 16), fps_start=None, generator=None,
+def reconstruct_chunk(ae, chunk, pcd=None, input_views=range(8), eval_views=range(8, 16), fps_start=None, generator=None,
                       bg_color=None, lpips=None):
     """The VAE round trip on one chunk: the encoder sees `input_views`, the finest level of detail (73 728 surfels
     at the deployed sizes) is rendered at the chunk's own cameras for `input_views` and `eval_views`, and each render
-    is scored against the chunk's files.  chunk: a folder or read_chunk's dict; pcd: a PLY path or [N, 3].
+    is scored against the chunk's files.  chunk: a folder or read_chunk's dict; pcd: a PLY path or [N, 3], or None:
+    the chunk's own surface cloud, pcd.chunk_surface_pcd of all its views (what the reference's save_pcd.py writes).
 
     Returns the 'enc_dec_wo_triplane' dict (latent, the four gaussians_* levels) plus 'input' and 'eval', each
     {'views', 'c', 'render' (GaussianRenderer2DGS.render's dict, [1, V, ...]), 'targets', 'table' [V, 8],
@@ -254,6 +256,9 @@ def reconstruct_chunk(ae, chunk, pcd, input_views=range(8), eval_views=range(8, 
     if len(input_views) != ae.encoder.V:
         raise ValueError("reconstruct_chunk: %d input views, the encoder was built for %d" % (len(input_views), ae.encoder.V))
     dev = torch.device("cuda", torch.cuda.current_device())
+    if pcd is None:
+        from .pcd import chunk_surface_pcd
+        pcd = chunk_surface_pcd(chunk, device=dev)
     pcd = torch.as_tensor(pcd, dtype=torch.float32).to(dev).reshape(1, -1, 3)
     enc_in, t_all, c_all = pack(chunk, input_views + eval_views, dev)
     nin = len(input_views)

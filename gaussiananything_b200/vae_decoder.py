@@ -340,7 +340,7 @@ class SurfelAE:
         if self.encoder is not None and behaviour in ("enc", "encoder_vae", "enc_dec_wo_triplane"):
             return self._encoder_behaviour(behaviour, img, kwargs)
         if behaviour == "reconstruct_chunk":
-            # chunk=, pcd=, optional input_views=, eval_views=, fps_start=, generator=, bg_color=, lpips= (gbuffer.py)
+            # chunk=, optional pcd= (default: the chunk's own surface cloud), input_views=, eval_views=, fps_start=, generator=, bg_color=, lpips= (gbuffer.py)
             from .gbuffer import reconstruct_chunk
             return reconstruct_chunk(self, **kwargs)
         raise NotImplementedError("gaussiananything_b200.SurfelAE: behaviour %r is outside the decode / render path "

@@ -598,6 +598,52 @@ int ga_lpips_tap_backward(const void *feat, int n, int H, int W, int C, int side
 int ga_lpips_input_backward(const void *g0, int n, int H, int W, const float *w_flip, const float *scale,
                             int normalize, float *dx, void *stream);
 
+/*
+ * ---------------------------------------------------------------------------
+ * Part 10: surface point clouds, the inputs the reference's scripts/save_pcd.py (save_pcd_from_depth :323-403) and
+ * scripts/save_pcd_from_gs.py (:158-185) make with pytorch3d.ops.sample_farthest_points: a G-buffer chunk's depth
+ * maps fused into one cloud, and farthest-point sampling of clouds of up to 4M points.
+ * pcd_ops.cu is compiled without FMA contraction: every operation below is rounded to fp32 on its own.
+ * ---------------------------------------------------------------------------
+ */
+/* ga_fps's range: the one-CTA kernel holds a cloud in registers. */
+#define GA_FPS_MAX_N 16384
+#define GA_FPS_MAX_K 1024
+/* ga_fps_ex's range. */
+#define GA_FPS_EX_MAX_N 4194304
+#define GA_FPS_EX_MAX_K 32768
+/* Bytes of the workspace ga_fps_ex needs: a 64-bit slot per (cloud, round) and the running minimum distance of
+ * every point.  Host-only, no CUDA call. */
+size_t ga_fps_ex_workspace_bytes(int batch, int N, int K);
+/* Farthest-point sampling with ga_fps's selection rule (Part 5: point 0 is start_idx[b], point k the one farthest
+ * from the points already chosen, distance (dx*dx + dy*dy) + dz*dz with each operation rounded on its own, ties to the
+ * lowest index) over clouds of different lengths, as pytorch3d's sample_farthest_points pads them.
+ * pcd fp32 [batch, N, 3]; lengths int32 [batch] (device) or NULL: cloud b is its first min(lengths[b], N) points
+ * (every cloud has N points when NULL); start_idx int32 [batch] in [0, lengths[b]) (device; not read for an empty
+ * cloud).  idx_out int32 [batch, K], xyz_out fp32 [batch, K, 3]: the first min(K, lengths[b]) entries of cloud b
+ * are its samples, the rest -1 and (0, 0, 0).  N <= GA_FPS_EX_MAX_N and K <= GA_FPS_EX_MAX_K (GA_ERR_SIZE above).
+ * Without lengths, where N <= GA_FPS_MAX_N and K <= min(N, GA_FPS_MAX_K), this is ga_fps (the workspace is not read
+ * and may be NULL).  Otherwise one cooperative launch: each cloud gets several CTAs that keep a slice of its points
+ * in registers (the rest, and their distances, in the workspace), and each round is reduced by a 64-bit atomicMax
+ * of (distance bits << 32 | ~index) into the round's slot, then one grid-wide barrier.  GA_ERR_SIZE when the device
+ * cannot hold batch CTAs of it at once (batch > 132 on an H100 SXM).  The same inputs give the same bits. */
+int ga_fps_ex(const float *pcd, const int32_t *lengths, int batch, int N, int K, const int32_t *start_idx,
+              int32_t *idx_out, float *xyz_out, void *workspace, size_t workspace_bytes, void *stream);
+/* Bytes of scratch ga_chunk_surface_points needs.  Host-only, no CUDA call. */
+size_t ga_chunk_surface_points_scratch_bytes(int n_views, int H, int W);
+/* The surface points of a chunk's views, fused.  alpha uint8 [H, n_chunk * W] and depth fp32 [n_chunk, H, W],
+ * cams fp32 [n_chunk, 25] as ga_gbuffer_pack takes them; views int32 [n_views] in [0, n_chunk) (the caller checks
+ * the range).  W % 4 == 0.  Pixel (x, y) of view views[s] is unprojected exactly as ga_gbuffer_pack's encoder
+ * channels 12-14 (the same device code: RaySampler, clip to [-0.45, 0.45], 0 where |p| == 0.45) and kept where
+ *   alpha >= alpha_min  and  depth >= min_depth  and  all three coordinates != 0
+ * (save_pcd_from_depth with alpha_min 255, its alpha_mask == 1, and min_depth 1.05: a kept coordinate is strictly
+ * inside +-0.45).  points fp32 [n_views * H * W, 3] (room for every pixel) receives the kept points in view order
+ * (s), then row-major pixel order; count int32 [1] (device) = their number.  Three launches (count per block, scan,
+ * emit), no atomics. */
+int ga_chunk_surface_points(const uint8_t *alpha, const float *depth, const float *cams, int n_chunk, int H, int W,
+                            const int32_t *views, int n_views, int alpha_min, float min_depth, float *points,
+                            int32_t *count, void *scratch, size_t scratch_bytes, void *stream);
+
 /* Measurement aid: when enabled, cudaEvents are recorded around every kernel
  * stage of the next forward/backward; ga_profile_read synchronises on them and
  * returns per-stage milliseconds: [0] preprocess, [1] binning, [2] render fwd,
