@@ -46,3 +46,5 @@ def install_shims(replace_classes: bool = True):
         if m is not None:
             from . import lpips as _lpips
             m.LPIPSLoss = _lpips.LPIPSLoss
+        # nsr.losses.disc.NLayerDiscriminator is left to the reference: gaussiananything_b200.disc's is slower than
+        # bf16 cuDNN autocast on an H100 (profiles/disc_h100.md), so it is not swapped in (INTEGRATION.md section 3j)

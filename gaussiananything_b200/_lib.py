@@ -110,6 +110,21 @@ ABI = {
     "ga_fps_ex": (i32, [vp, vp, i32, i32, i32, vp, vp, vp, vp, sz, vp]),
     "ga_chunk_surface_points_scratch_bytes": (sz, [i32, i32, i32]),
     "ga_chunk_surface_points": (i32, [vp, vp, vp, i32, i32, i32, vp, i32, i32, f32, vp, vp, vp, sz, vp]),
+    "ga_conv4x4_out_size": (i32, [i32, i32]),
+    "ga_conv4x4_lrelu_bf16": (i32, [vp, i32, i32, i32, i32, vp, i32, vp, i32, i32, vp, vp]),
+    "ga_conv4x4_stats": (i32, [vp, i32, i32, i32, i32, vp, i32, i32, i32, vp, vp, vp]),
+    "ga_disc_bn_forward": (i32, [vp, vp, i64, i32, vp, vp, i32, f32, f32, vp, vp, vp, vp, vp, vp]),
+    "ga_disc_conv5": (i32, [vp, i32, i32, i32, vp, vp, vp, vp]),
+    "ga_disc_conv5_partials": (i32, [i32, i32, i32]),
+    "ga_disc_conv5_backward": (i32, [vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "ga_disc_dgrad_partials": (i32, [i32, i32, i32, i32]),
+    "ga_disc_dgrad": (i32, [vp, i32, i32, i32, i32, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "ga_disc_bn_backward": (i32, [vp, vp, i64, i32, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp]),
+    "ga_disc_wgrad_workspace_bytes": (sz, [i32, i32, i32, i32, i32]),
+    "ga_disc_wgrad": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, sz, vp, vp]),
+    "ga_disc_colsum_scratch_bytes": (sz, [i64, i32]),
+    "ga_disc_colsum": (i32, [vp, i32, i64, i32, vp, sz, vp, vp]),
+    "ga_disc_input_backward": (i32, [vp, i32, i32, i32, vp, vp, vp]),
     "ga_profile_enable": (i32, [i32]),
     "ga_profile_read": (i32, [C.POINTER(f32), i32]),
     "ga_b200_version": (C.c_char_p, []),

@@ -31,6 +31,8 @@ EXTRA = {
     "lpips_grad.cu": ["--fmad=false"],
     # chunk surface points (gbuffer_pack_kernel's unprojection to the bit) and FPS distances, include/ga_b200.h Part 10
     "pcd_ops.cu": ["--fmad=false"],
+    # PatchGAN discriminator: BatchNorm, conv 5 and the reductions rounded as include/ga_b200.h Part 11 states them
+    "disc_ops.cu": ["--fmad=false"],
 }
 
 

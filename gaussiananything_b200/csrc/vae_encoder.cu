@@ -3,169 +3,9 @@
 // farthest-point sampling, the input / token-xyz packing, the head-32 split of the SRT blocks and the readout head
 // with the posterior.  The 1x1 convolutions, linears and attentions run on the Part 2 GEMM / attention entry points.
 #include "../../include/ga_b200.h"
-#include "device_once.cuh"
-#include "sm90_ptx.cuh"
-
-using namespace sm90;
+#include "conv_igemm.cuh"
 
 namespace {
-
-// ---------------------------------------------------------------------------------------------------------------
-// 3x3 convolution, implicit GEMM: out[m, n] = bias[n] + sum_k A[m, k] W[n, k] (+ residual[m, n]), then the epilogue
-// EPI: kEpiNone as is, kEpiRelu max(., 0), kEpiMask mask[m, n] > 0 ? . : 0 (a select: the ReLU backward, where mask is
-// the forward's ReLU output, so a non-finite value never leaks through a masked zero),
-// m = (image, oy, ox), k = (ky * 3 + kx) * Cin + c.  A is never materialised: every 16-byte piece (8 channels of one
-// tap of one output pixel) is gathered with cp.async straight from the NHWC input, zero-filled where the tap falls
-// into the padding or k runs past 9 * Cin.  The pieces land in the 128-byte-swizzled K-major layout that
-// wgmma_desc_k_sw128 describes, the layout the TMA GEMM uses.  Two warpgroups, each 64 output pixels x BN channels;
-// a kConvStages-deep cp.async ring keeps kConvStages - 2 K-blocks in flight ahead of the MMAs.
-// ---------------------------------------------------------------------------------------------------------------
-constexpr int CBM = 128, CBK = 64;
-constexpr int kConvThreads = 256;
-constexpr int kConvStages = 5;
-
-template <int BN> struct ConvCfg {
-    static constexpr int kABytes = CBM * CBK * 2;
-    static constexpr int kBBytes = BN * CBK * 2;
-    static constexpr int kStageBytes = kABytes + kBBytes;
-    static constexpr int kSmem = kConvStages * kStageBytes + 1024;
-};
-
-struct ConvArgs {
-    const __nv_bfloat16 *x;     // [n, H, W, Cin]
-    const __nv_bfloat16 *w;     // [Cout, k_pitch]
-    const float *bias;          // [Cout] or NULL
-    const float *residual;      // [M, Cout] fp32 or NULL
-    float *out_f32;             // [M, Cout] or NULL
-    __nv_bfloat16 *out_bf16;    // [M, Cout] or NULL
-    int H, W, Cin, Ho, Wo, Cout, k_pitch, stride, M, K;
-    const __nv_bfloat16 *mask;  // [M, Cout] for kEpiMask
-};
-
-constexpr int kEpiNone = 0, kEpiRelu = 1, kEpiMask = 2;
-
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid)
-{
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
-template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
-// cp.async writes through the generic proxy, wgmma reads through the async proxy
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
-
-template <int BN, int EPI>
-__global__ void __launch_bounds__(kConvThreads, 1) conv3x3_kernel(const ConvArgs a)
-{
-    using Cfg = ConvCfg<BN>;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int wg = warp >> 2, wi = warp & 3;
-    const int m0 = blockIdx.x * CBM, n0 = blockIdx.y * BN;
-    const int nk = (a.K + CBK - 1) / CBK;
-    const int chunk = tid & 7;
-
-    // the 4 output pixels this thread gathers for: rows r = tid / 8 + 32 i of the tile
-    int img_base[4], oy0[4], ox0[4];
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-        const int m = m0 + (tid >> 3) + 32 * i;
-        if (m < a.M) {
-            const int hw = a.Ho * a.Wo;
-            const int img = m / hw, p = m - img * hw;
-            const int oy = p / a.Wo, ox = p - oy * a.Wo;
-            img_base[i] = img;
-            // stride 1: pad 1 on every side; stride 2: pad (0, 1, 0, 1), i.e. none on the top / left
-            oy0[i] = a.stride == 1 ? oy - 1 : 2 * oy;
-            ox0[i] = a.stride == 1 ? ox - 1 : 2 * ox;
-        } else {
-            img_base[i] = -1; oy0[i] = 0; ox0[i] = 0;
-        }
-    }
-
-    pdl_wait();
-    pdl_launch_dependents();
-
-    auto load_stage = [&](int kb) {
-        if (kb < nk) {
-            const int s = kb % kConvStages;
-            const uint32_t sa = smem_u32(smem + s * Cfg::kStageBytes);
-            const uint32_t sb = sa + Cfg::kABytes;
-            const int k = kb * CBK + chunk * 8;
-            const bool kin = k < a.K;
-            const int tap = kin ? k / a.Cin : 0;
-            const int c = k - tap * a.Cin;
-            const int ky = tap / 3, kx = tap - ky * 3;
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                const int r = (tid >> 3) + 32 * i;
-                const int iy = oy0[i] + ky, ix = ox0[i] + kx;
-                const bool v = kin && img_base[i] >= 0 && iy >= 0 && iy < a.H && ix >= 0 && ix < a.W;
-                const __nv_bfloat16 *src = v ? a.x + (((size_t)img_base[i] * a.H + iy) * a.W + ix) * a.Cin + c : a.x;
-                cp_async16(sa + r * 128 + ((chunk ^ (r & 7)) << 4), src, v);
-            }
-#pragma unroll
-            for (int i = 0; i < BN / 32; i++) {
-                const int r = (tid >> 3) + 32 * i;
-                cp_async16(sb + r * 128 + ((chunk ^ (r & 7)) << 4), a.w + (size_t)(n0 + r) * a.k_pitch + kb * CBK + chunk * 8,
-                           true);
-            }
-        }
-        cp_async_commit();                  // an empty group past the end keeps the wait counts uniform
-    };
-
-    for (int kb = 0; kb < kConvStages - 2; kb++) load_stage(kb);
-
-    float acc[BN / 2];
-#pragma unroll
-    for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
-    for (int kb = 0; kb < nk; kb++) {
-        cp_async_wait<kConvStages - 3>();   // this thread's pieces of K-block kb have landed
-        fence_proxy_async();
-        __syncthreads();                    // ... and everyone's; both warpgroups have retired the MMAs of kb - 2
-        load_stage(kb + kConvStages - 2);   // into the slot of kb - 2
-        const int s = kb % kConvStages;
-        const uint64_t ad = wgmma_desc_k_sw128(smem_u32(smem + s * Cfg::kStageBytes + wg * 64 * 128));
-        const uint64_t bd = wgmma_desc_k_sw128(smem_u32(smem + s * Cfg::kStageBytes + Cfg::kABytes));
-        fence_regs(acc);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < CBK / 16; k++) wgmma_ss<BN>(acc, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), 1u);
-        wgmma_commit();
-        wgmma_wait<1>();
-        fence_regs(acc);
-    }
-    wgmma_wait<0>();
-    fence_regs(acc);
-    cp_async_wait<0>();
-
-    // epilogue straight from the fragment: row 16 wi + lane/4 (+8), columns 8 j + 2 (lane%4) (+1)
-    const int r = lane >> 2, cq = lane & 3;
-#pragma unroll
-    for (int j = 0; j < BN / 8; j++) {
-        const int n = n0 + 8 * j + 2 * cq;
-        const float b0 = a.bias ? __ldg(a.bias + n) : 0.f, b1 = a.bias ? __ldg(a.bias + n + 1) : 0.f;
-#pragma unroll
-        for (int hf = 0; hf < 2; hf++) {
-            const int m = m0 + wg * 64 + wi * 16 + r + 8 * hf;
-            if (m >= a.M) continue;
-            float v0 = acc[4 * j + 2 * hf] + b0, v1 = acc[4 * j + 2 * hf + 1] + b1;
-            const size_t o = (size_t)m * a.Cout + n;
-            if (a.residual) {
-                const float2 rr = *reinterpret_cast<const float2 *>(a.residual + o);
-                v0 += rr.x; v1 += rr.y;
-            }
-            if (EPI == kEpiRelu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-            if (EPI == kEpiMask) {
-                const float2 mk = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(a.mask + o));
-                v0 = mk.x > 0.f ? v0 : 0.f;
-                v1 = mk.y > 0.f ? v1 : 0.f;
-            }
-            if (a.out_f32) *reinterpret_cast<float2 *>(a.out_f32 + o) = make_float2(v0, v1);
-            if (a.out_bf16) *reinterpret_cast<__nv_bfloat162 *>(a.out_bf16 + o) = __floats2bfloat162_rn(v0, v1);
-        }
-    }
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // GroupNorm(32) over NHWC fp32, deterministic split reduction.  Pass 1: one CTA per (pixel chunk, image) writes the
@@ -472,40 +312,18 @@ __global__ void __launch_bounds__(kHeadThreads) readout_head_kernel(const GaVaeE
 }  // namespace
 
 // ---- host side ----------------------------------------------------------------------------------------------------
-template <int BN, int EPI>
-static int launch_conv(const ConvArgs &a, cudaStream_t s)
-{
-    using Cfg = ConvCfg<BN>;
-    static GaPerDevice attr_set;
-    if (ga_first_use_on_device(attr_set)) {
-        cudaError_t e = cudaFuncSetAttribute(conv3x3_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             Cfg::kSmem);
-        if (e != cudaSuccess) return (int)e;
-    }
-    dim3 grid((a.M + CBM - 1) / CBM, a.Cout / BN);
-    return (int)ga_launch_pdl(conv3x3_kernel<BN, EPI>, grid, dim3(kConvThreads), (size_t)Cfg::kSmem, s, a);
-}
-
-// the argument checks of both conv entry points; fills `a` and returns 0, or the error code
+// the argument checks of the 3x3 entry points; fills `a` and returns 0, or the error code
 static int conv_args(ConvArgs &a, const void *x, int n, int H, int W, int Cin, const void *w_packed, int k_pitch,
                      const float *bias, int Cout, int stride, const float *residual, float *out_f32, void *out_bf16)
 {
-    if (!x || !w_packed || n <= 0 || Cin <= 0 || Cin % 8 || Cout <= 0 || Cout % 64) return GA_ERR_BADARG;
+    if (n <= 0 || Cin <= 0 || Cin % 8 || Cout <= 0 || Cout % 64) return GA_ERR_BADARG;
     if (!out_f32 && !out_bf16) return GA_ERR_BADARG;
     const int Ho = ga_conv3x3_out_size(H, stride), Wo = ga_conv3x3_out_size(W, stride);
     if (Ho <= 0 || Wo <= 0) return GA_ERR_BADARG;
-    if (k_pitch < ((9 * Cin + CBK - 1) / CBK) * CBK || (reinterpret_cast<uintptr_t>(w_packed) & 15) ||
-        (reinterpret_cast<uintptr_t>(x) & 15))
-        return GA_ERR_BADARG;
-    if ((int64_t)n * Ho * Wo >= (int64_t)1 << 31) return GA_ERR_SIZE;
-    a.x = reinterpret_cast<const __nv_bfloat16 *>(x);
-    a.w = reinterpret_cast<const __nv_bfloat16 *>(w_packed);
-    a.bias = bias; a.residual = residual; a.out_f32 = out_f32;
-    a.out_bf16 = reinterpret_cast<__nv_bfloat16 *>(out_bf16);
-    a.H = H; a.W = W; a.Cin = Cin; a.Ho = Ho; a.Wo = Wo; a.Cout = Cout; a.k_pitch = k_pitch; a.stride = stride;
-    a.M = n * Ho * Wo; a.K = 9 * Cin;
-    a.mask = nullptr;
-    return 0;
+    // stride 1: pad 1 on every side; stride 2: pad (0, 1, 0, 1), i.e. none on the top / left
+    const int pad = stride == 1 ? 1 : 0;
+    return conv_args_common(a, 3, x, n, H, W, Cin, Ho, Wo, w_packed, k_pitch, bias, Cout, stride, pad, pad, residual,
+                            out_f32, out_bf16);
 }
 
 extern "C" int ga_conv3x3_out_size(int H, int stride)
@@ -524,7 +342,7 @@ extern "C" int ga_conv3x3_bf16(const void *x, int n, int H, int W, int Cin, cons
     const int rc = conv_args(a, x, n, H, W, Cin, w_packed, k_pitch, bias, Cout, stride, residual, out_f32, out_bf16);
     if (rc) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    return Cout % 128 == 0 ? launch_conv<128, kEpiNone>(a, s) : launch_conv<64, kEpiNone>(a, s);
+    return Cout % 128 == 0 ? launch_conv<3, 128, kEpiNone>(a, s) : launch_conv<3, 64, kEpiNone>(a, s);
 }
 
 extern "C" int ga_conv3x3_relu_bf16(const void *x, int n, int H, int W, int Cin, const void *w_packed, int k_pitch,
@@ -534,7 +352,7 @@ extern "C" int ga_conv3x3_relu_bf16(const void *x, int n, int H, int W, int Cin,
     const int rc = conv_args(a, x, n, H, W, Cin, w_packed, k_pitch, bias, Cout, 1, nullptr, nullptr, out_bf16);
     if (rc) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    return Cout % 128 == 0 ? launch_conv<128, kEpiRelu>(a, s) : launch_conv<64, kEpiRelu>(a, s);
+    return Cout % 128 == 0 ? launch_conv<3, 128, kEpiRelu>(a, s) : launch_conv<3, 64, kEpiRelu>(a, s);
 }
 
 extern "C" int ga_conv3x3_mask_bf16(const void *x, int n, int H, int W, int Cin, const void *w_packed, int k_pitch,
@@ -546,7 +364,7 @@ extern "C" int ga_conv3x3_mask_bf16(const void *x, int n, int H, int W, int Cin,
     if (rc) return rc;
     a.mask = reinterpret_cast<const __nv_bfloat16 *>(mask);
     cudaStream_t s = (cudaStream_t)stream;
-    return Cout % 128 == 0 ? launch_conv<128, kEpiMask>(a, s) : launch_conv<64, kEpiMask>(a, s);
+    return Cout % 128 == 0 ? launch_conv<3, 128, kEpiMask>(a, s) : launch_conv<3, 64, kEpiMask>(a, s);
 }
 
 extern "C" size_t ga_group_norm_scratch_bytes(int n, int HW)

@@ -644,6 +644,122 @@ int ga_chunk_surface_points(const uint8_t *alpha, const float *depth, const floa
                             const int32_t *views, int n_views, int alpha_min, float min_depth, float *points,
                             int32_t *count, void *scratch, size_t scratch_bytes, void *stream);
 
+/*
+ * ---------------------------------------------------------------------------
+ * Part 11: PatchGAN discriminator, the reference's nsr/losses/disc.py NLayerDiscriminator(input_nc=3, ndf=64,
+ * n_layers=3, use_actnorm=False): five 4x4 convolutions with pad 1 (strides 2, 2, 2, 1, 1; channels 3 -> 64 -> 128 ->
+ * 256 -> 512 -> 1), BatchNorm2d after convs 2-4, LeakyReLU(0.2) after convs 1-4; forward in training and eval mode,
+ * input and weight gradients.  Activations NHWC; every weight is repacked from the fp32 parameters on every call.
+ *   conv 1: the image packed by ga_vae_enc_input (c_pad 8, bf16), ga_conv4x4_lrelu_bf16 -> a1 bf16
+ *   conv k = 2..4: ga_conv4x4_stats -> z_k fp32 and per-CTA partials, ga_disc_bn_forward -> a_k bf16
+ *   conv 5: ga_disc_conv5 -> fp32 logits
+ * Packed weights of a 4x4 conv W [Co, Ci, 4, 4]: bf16 [Co, k_pitch], column (ky * 4 + kx) * Ci' + ci = W[co, ci, ky, kx]
+ * (Ci' = 8 for conv 1, channels 3-7 zero), k_pitch = 16 Ci' rounded up to 64.
+ * Backward, from the logits' fp32 gradient g5:
+ *   ga_disc_conv5_backward -> gy4 = dL/dy4 (y4 = BN 4's output) fp32, BN 4's partials, dW5
+ *   ga_disc_bn_backward    -> dgamma, dbeta, dz4 = dL/dz4 bf16
+ *   ga_disc_wgrad(dz_k, a_{k-1}) -> dW_k;  ga_disc_dgrad(dz_k, flipped W_k) -> gy_{k-1} fp32 (k = 3, 4) or dz1 bf16
+ *   conv 1: ga_disc_wgrad(dz1, packed image) -> dW1, ga_disc_colsum(dz1) -> db1, ga_disc_input_backward -> dx.
+ * dgrad weights: stride 1 (conv 4), the 4x4 conv of the gradient padded by 2: bf16 [Ci, k_pitch], column
+ * (ky * 4 + kx) * Co + co = W[co, ci, 3 - ky, 3 - kx].  Stride 2 (convs 2, 3): the input pixel (2a + py, 2b + px) of
+ * parity class (py, px) receives a 2x2 stride-1 conv of the gradient at rows a - 1 + py + ty (ty = 0, 1) and columns
+ * b - 1 + px + tx with W[co, ci, 3 - py - 2 ty, 3 - px - 2 tx]; four packs [4 = 2 py + px][Ci, k_pitch], column
+ * (ty * 2 + tx) * Co + co, k_pitch = 4 Co rounded up to 64.
+ * Rounding: bf16 operands (activations a_k, packed weights, dz_k), fp32 accumulation in the wgmma's order; z_k, gy_k
+ * and the logits fp32; conv 5's weights fp32.  disc_ops.cu is compiled without FMA contraction: every operation of
+ * the non-GEMM kernels below is rounded to fp32 on its own, in the order written.  No atomics: the same inputs give
+ * the same bits.
+ * BatchNorm statistics: each conv CTA (128 output pixels) writes its channel mean m_b (fp32 sum / count) and
+ * M2_b = sum (z - m_b)^2 (fp32, from the accumulator registers); the finalize merges them in fp64 with Chan's rule
+ * (mean += d n_b / n, M2 += M2_b + d^2 n_a n_b / n), so no E[z^2] - mean^2 cancellation: thread t of 128 merges CTAs
+ * t, t + 128, ... in order, then the 128 states are merged by a fixed tree (t with t + s, s = 64, 32, ..., 1).
+ * var = M2 / M.  The backward's sums (sum gy, sum gy xhat) are added in fp64 in the same fixed pattern.
+ * Test bounds: the bf16-emulating oracle (oracle/disc_oracle.py) rounds where these kernels round, with every sum in
+ * fp64.  Its relative L2 distance from fp64 was measured on the golden cases (tests/golden/disc_small.npz, 64 x 64 /
+ * 50 x 70, 4 images, the d-step of make_disc_golden.py), and the GPU tests allow 1.5 times it plus 1e-5:
+ *   logits, train mode: real 5.1e-3 / 5.1e-3, fake 7.1e-3 / 6.9e-3; eval mode 1.9e-3 / 2.2e-3
+ *   input gradient of the g-loss 0.143 / 0.144
+ *   d-loss parameter gradients: conv 1 weight 0.096 / 0.133, bias 0.104 / 0.156; conv 2 0.104 / 0.111;
+ *   BN 2 weight 0.097 / 0.104, bias 0.121 / 0.114; conv 3 0.088 / 0.097; BN 3 weight 0.065 / 0.071, bias 0.101 /
+ *   0.099; conv 4 0.066 / 0.073; BN 4 weight 3.0e-3 / 4.4e-3, bias 0.017 / 0.029; conv 5 weight 3.1e-3 / 4.6e-3,
+ *   bias 0 / 0.
+ * The gradients are far from fp64 because, with random weights, BatchNorm's backward subtracts nearly equal terms,
+ * and bf16 rounding of the activations decides them.  Timings: profiles/disc_h100.md (H100 80GB HBM3, 700 W).
+ * ---------------------------------------------------------------------------
+ */
+/* Output size of a 4x4 pad-1 convolution: (H - 2) / stride + 1, stride 1 or 2; GA_ERR_BADARG when H < 2.  Host only. */
+int ga_conv4x4_out_size(int H, int stride);
+/* 4x4 pad-1 convolution (Part 5's implicit GEMM generalised to 4x4 taps) with bias and LeakyReLU(0.2):
+ * out_bf16[m, c] = bf16(v > 0 ? v : 0.2 v), v = bias[c] + conv.  x bf16 NHWC [n, H, W, Cin], Cin % 8 == 0;
+ * w_packed as above; Cout % 64 == 0; out [n, Ho, Wo, Cout]. */
+int ga_conv4x4_lrelu_bf16(const void *x, int n, int H, int W, int Cin, const void *w_packed, int k_pitch,
+                          const float *bias, int Cout, int stride, void *out_bf16, void *stream);
+/* 4x4 pad-1 convolution without bias: z fp32 [M = n Ho Wo, Cout], and partial float2 [ceil(M / 128), Cout]: CTA b's
+ * (m_b, M2_b) over rows [128 b, 128 b + 128) as stated above.  partial NULL: z only (eval mode). */
+int ga_conv4x4_stats(const void *x, int n, int H, int W, int Cin, const void *w_packed, int k_pitch, int Cout,
+                     int stride, float *z, void *partial, void *stream);
+/* BatchNorm2d + LeakyReLU(0.2) on z fp32 [M, C].  training != 0: mean and var (biased) from ga_conv4x4_stats's
+ * partials (Chan, fp64), rstd = fp32(1 / sqrt(var + eps)) in fp64; running_mean = fp32((1 - momentum) rm + momentum
+ * mean), running_var = fp32((1 - momentum) rv + momentum M2 / (M - 1)), in fp64 (M >= 2).  training == 0: mean =
+ * running_mean, rstd from running_var; the running stats are not written.  mean_out, rstd_out fp32 [C];
+ * a_out bf16 [M, C] = bf16(lrelu(((z - mean) rstd) gamma + beta)). */
+int ga_disc_bn_forward(const float *z, const void *partial, int64_t M, int C, const float *gamma, const float *beta,
+                       int training, float momentum, float eps, float *running_mean, float *running_var,
+                       float *mean_out, float *rstd_out, void *a_out, void *stream);
+/* Conv 5 (512 -> 1, 4x4, pad 1, stride 1): x bf16 NHWC [n, H, W, 512], w5 fp32 [16, 512] (w5[ky * 4 + kx, ci] =
+ * W5[0, ci, ky, kx]), bias fp32 [1] (device).  out fp32 [n, H - 1, W - 1] = bias + sum over taps in row-major order
+ * of (lane sums of channels 8 l .. 8 l + 7 then 256 + 8 l .., increasing), then an xor butterfly over 32 lanes. */
+int ga_disc_conv5(const void *x, int n, int H, int W, const float *w5, const float *bias, float *out, void *stream);
+/* Number of partial rows ga_disc_conv5_backward writes for conv 5's input [n, H, W]. */
+int ga_disc_conv5_partials(int n, int H, int W);
+/* Conv 5's backward through LeakyReLU 4 to BatchNorm 4's output.  g5 fp32 [n, H - 1, W - 1]; a4 bf16 and z4 fp32
+ * [n, H, W, 512]; mean4, rstd4 BN 4's.  Per input pixel p and channel c: ga = sum over taps (row-major) of g5[o] w5[tap,
+ * c] where o is the output the tap reaches; gy4[p, c] = a4 > 0 ? ga : 0.2 ga.  Block b of 256 pixels: bn_partial float2
+ * [b, 512] = (sum gy4, sum gy4 xhat) in pixel order, xhat = (z4 - mean4) rstd4; dw_partial fp32 [b, 16, 512] = sum
+ * g5[o] a4[p]; dw5 fp32 [16, 512] = the fp64 sum of dw_partial over blocks in order (both NULL: no weight
+ * gradient is formed). */
+int ga_disc_conv5_backward(const float *g5, int n, int H, int W, const float *w5, const void *a4, const float *z4,
+                           const float *mean4, const float *rstd4, float *gy4, void *bn_partial, float *dw_partial,
+                           float *dw5, void *stream);
+/* Number of partial rows ga_disc_dgrad writes for an output (the forward's input) of [n, H, W]. */
+int ga_disc_dgrad_partials(int n, int H, int W, int stride);
+/* dgrad of a 4x4 pad-1 convolution whose input is [n, H, W, Cout] (its gradient is this call's output) and whose
+ * output gradient is g bf16 [n, Ho, Wo, Cg]; w_packed: the flipped packs above (Cout = the forward's Ci).  act bf16
+ * [n, H, W, Cout]: the LeakyReLU output at the forward's input.  With v the dgrad:
+ *   z == NULL: out_bf16 = bf16(act > 0 ? v : 0.2 v)                      (conv 1's LeakyReLU, no BatchNorm)
+ *   z != NULL: gy_out fp32 = act > 0 ? v : 0.2 v, and per CTA (class by class for stride 2, classes in order 2 py +
+ *              px) partial float2 [ga_disc_dgrad_partials, Cout] = (sum gy, sum gy xhat), xhat = (z - mean) rstd. */
+int ga_disc_dgrad(const void *g, int n, int H, int W, int Cg, const void *w_packed, int k_pitch, int Cout, int stride,
+                  const void *act, const float *z, const float *mean, const float *rstd, float *gy_out, void *partial,
+                  void *out_bf16, void *stream);
+/* BatchNorm backward on gy fp32 [M, C] (the gradient at the BN output): sums S = sum gy, T = sum gy xhat over the
+ * n_partial rows of partial (fp64, the fixed pattern above); dbeta = fp32(S), dgamma = fp32(T) (either may be NULL); k = (fp32(S / M),
+ * fp32(T / M)) in training mode, (0, 0) in eval mode (fixed statistics), into k_scratch (float2 [C]);
+ * dz_bf16 [M, C] = bf16((gamma rstd) ((gy - k.x) - xhat k.y)). */
+int ga_disc_bn_backward(const float *gy, const float *z, int64_t M, int C, const float *mean, const float *rstd,
+                        const float *gamma, const void *partial, int n_partial, int training, float *dgamma, float *dbeta,
+                        void *k_scratch, void *dz_bf16, void *stream);
+/* Bytes of workspace ga_disc_wgrad needs.  Host only. */
+size_t ga_disc_wgrad_workspace_bytes(int n, int Ho, int Wo, int Co, int Cin);
+/* Weight gradient of a 4x4 pad-1 convolution: dy bf16 [n, Ho, Wo, Co] (Co % 64 == 0), x bf16 NHWC [n, H, W, Cin]
+ * (Cin % 8 == 0).  D[co, (ky * 4 + kx) Cin + ci] = sum over output pixels p of dy[p, co] x[p's tap, ci]: a GEMM whose
+ * K is the pixel count, both operands MN-major; they are staged with cp.async as they lie and transposed by
+ * ldmatrix.trans into mma.sync m16n8k16 (fp32 accumulation).  Split over pixels into S fp32 partials (S from the
+ * shapes only), summed in split order in fp64: dw fp32 [Co, cin_out, 4, 4] (the parameter layout, channels past
+ * cin_out dropped). */
+int ga_disc_wgrad(const void *dy, const void *x, int n, int H, int W, int Cin, int Co, int stride, int cin_out,
+                  void *workspace, size_t workspace_bytes, float *dw, void *stream);
+/* Bytes of scratch ga_disc_colsum needs.  Host only. */
+size_t ga_disc_colsum_scratch_bytes(int64_t rows, int C);
+/* out fp32 [C] = column sums of x [rows, C] (bf16 when is_bf16, else fp32), 256 % C == 0: blocks of 1024 rows summed
+ * in fp32 in a fixed order, the blocks in order in fp64. */
+int ga_disc_colsum(const void *x, int is_bf16, int64_t rows, int C, void *scratch, size_t scratch_bytes, float *out,
+                   void *stream);
+/* Conv 1's dgrad to the image: g1 bf16 [n, Ho, Wo, 64] (dz1), w1 fp32 [16, 64, 3] (w1[ky * 4 + kx, co, c] =
+ * bf16(W1[co, c, ky, kx]) as fp32).  dx fp32 NCHW [n, 3, H, W]: per pixel the taps reaching it in row-major order,
+ * within a tap co increasing (the straight-through gradient of the input's bf16 rounding). */
+int ga_disc_input_backward(const void *g1, int n, int H, int W, const float *w1, float *dx, void *stream);
+
 /* Measurement aid: when enabled, cudaEvents are recorded around every kernel
  * stage of the next forward/backward; ga_profile_read synchronises on them and
  * returns per-stage milliseconds: [0] preprocess, [1] binning, [2] render fwd,
