@@ -48,3 +48,6 @@ def install_shims(replace_classes: bool = True):
             m.LPIPSLoss = _lpips.LPIPSLoss
         # nsr.losses.disc.NLayerDiscriminator is left to the reference: gaussiananything_b200.disc's is slower than
         # bf16 cuDNN autocast on an H100 (profiles/disc_h100.md), so it is not swapped in (INTEGRATION.md section 3j)
+        # xformers.ops.memory_efficient_attention is left alone too: attention.memory_efficient_attention's forward +
+        # backward is slower than torch's bf16 SDPA at the DiT and encoder shapes (profiles/attention_grad_h100.md);
+        # attention.install_shims() is the opt-in (INTEGRATION.md section 3k)

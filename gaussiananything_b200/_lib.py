@@ -125,6 +125,11 @@ ABI = {
     "ga_disc_colsum_scratch_bytes": (sz, [i64, i32]),
     "ga_disc_colsum": (i32, [vp, i32, i64, i32, vp, sz, vp, vp]),
     "ga_disc_input_backward": (i32, [vp, i32, i32, i32, vp, vp, vp]),
+    "ga_attention_grad_validate": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp,
+                                         i32]),
+    "ga_attention_fwd_lse_bf16": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, f32, vp]),
+    "ga_attention_bwd_bf16": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, f32,
+                                    vp]),
     "ga_profile_enable": (i32, [i32]),
     "ga_profile_read": (i32, [C.POINTER(f32), i32]),
     "ga_b200_version": (C.c_char_p, []),

@@ -760,6 +760,45 @@ int ga_disc_colsum(const void *x, int is_bf16, int64_t rows, int C, void *scratc
  * within a tap co increasing (the straight-through gradient of the input's bf16 rounding). */
 int ga_disc_input_backward(const void *g1, int n, int H, int W, const float *w1, float *dx, void *stream);
 
+/*
+ * ---------------------------------------------------------------------------
+ * Part 12: differentiable attention, xformers.ops.memory_efficient_attention for training (csrc/attention_grad.cu).
+ * O = softmax(S) V with S = q k^T * scale, lse[bh, i] = ln sum_j exp(S_ij) (fp32), and the backward
+ *   Delta_i = sum_c dO_ic O_ic,  P = exp(S - lse),  dV = P^T dO,  dS = P o (dO V^T - Delta),  dK = scale dS^T q,
+ *   dQ = scale dS k.
+ * Tensors are bf16 and addressed where they lie: element (b, n, h, c) of tensor t at t + b s0 + n s1 + h s2 + c, with
+ * strides = int64 [8][3] (host) for q, k, v, o, dout, dq, dk, dv in that order, in elements (a 3-D [B, N, d] tensor:
+ * heads 1, s2 0).  Every stride a multiple of 8 and every tensor 16-byte aligned.  Head dimensions d_qk (q, k) and
+ * d_v (v, o) are 32 or 64; 32 is zero-padded to 64 in shared memory, which is exact.  lse and delta fp32
+ * [batch * heads, Nq].  Any Nq, Nk >= 1; rows past the end are zero-filled on load and masked, never read.
+ * Nq <= 16 and Nk <= 16: one warp per (sequence, head) on CUDA cores, bf16 operands and fp32 arithmetic.  Otherwise
+ * wgmma m64n64k16 (bf16 operands, fp32 accumulation) over 64 x 64 tiles; P is rounded to bf16 before P V and
+ * P^T dO, dS before dS^T q and dS k.  The backward runs a Delta pass, a dK/dV kernel (one CTA per key block over all
+ * query blocks) and a dQ kernel (one CTA per query block over all key blocks): no atomics, the same inputs give the
+ * same bits.  The grid is one-dimensional, so batch * heads may exceed 65535.
+ * Test bounds (tests/attention_grad_ref.py): a bf16-emulating fp64 reference rounds where the tiled kernels round;
+ * the GPU result is held to 1.5 times its measured distance from fp64.  Timings: profiles/attention_grad_h100.md.
+ * ---------------------------------------------------------------------------
+ */
+/* Host only, no CUDA call: 0 when the arguments are accepted, else GA_ERR_BADARG (a NULL q, k, v, o, lse or strides;
+ * batch, heads, Nq or Nk < 1; d_qk or d_v not 32 or 64; backward with a NULL dout or delta; a misaligned tensor or
+ * a negative or non-multiple-of-8 stride of a tensor in use; a zero stride of o, dq, dk or dv on a dimension of size
+ * > 1, where CTAs would write the same elements) or GA_ERR_SIZE (more than 2^31 - 1 CTAs).  dq, dk, dv
+ * may each be NULL: that gradient is not formed. */
+int ga_attention_grad_validate(const void *q, const void *k, const void *v, const void *o, const float *lse,
+                               const void *dout, const float *delta, const void *dq, const void *dk, const void *dv,
+                               int batch, int heads, int Nq, int Nk, int d_qk, int d_v, const int64_t *strides,
+                               int backward);
+/* Forward: o (written, strides row 3) and lse. */
+int ga_attention_fwd_lse_bf16(const void *q, const void *k, const void *v, void *o, float *lse, int batch, int heads,
+                              int Nq, int Nk, int d_qk, int d_v, const int64_t *strides, float scale, void *stream);
+/* Backward from the forward's o and lse and the output gradient dout; delta is fp32 scratch [batch * heads, Nq].
+ * The dQ kernel is skipped when dq is NULL, the dK/dV kernel when dk and dv are both NULL; with dk and dq NULL (dV
+ * alone) neither the Delta pass nor dS is formed. */
+int ga_attention_bwd_bf16(const void *q, const void *k, const void *v, const void *o, const float *lse,
+                          const void *dout, float *delta, void *dq, void *dk, void *dv, int batch, int heads, int Nq,
+                          int Nk, int d_qk, int d_v, const int64_t *strides, float scale, void *stream);
+
 /* Measurement aid: when enabled, cudaEvents are recorded around every kernel
  * stage of the next forward/backward; ga_profile_read synchronises on them and
  * returns per-stage milliseconds: [0] preprocess, [1] binning, [2] render fwd,
