@@ -3,7 +3,15 @@
 See INTEGRATION.md.  Nothing here falls back to CPU or to a library path."""
 import sys
 
-__all__ = ["install_shims"]
+__all__ = ["install_shims", "mlp"]
+
+
+def __getattr__(name):
+    # gaussiananything_b200.mlp (the differentiable FusedMLP, INTEGRATION.md section 3l), imported on first use
+    if name == "mlp":
+        import importlib
+        return importlib.import_module(__name__ + ".mlp")
+    raise AttributeError("module %r has no attribute %r" % (__name__, name))
 
 
 def install_shims(replace_classes: bool = True):
@@ -51,3 +59,4 @@ def install_shims(replace_classes: bool = True):
         # xformers.ops.memory_efficient_attention is left alone too: attention.memory_efficient_attention's forward +
         # backward is slower than torch's bf16 SDPA at the DiT and encoder shapes (profiles/attention_grad_h100.md);
         # attention.install_shims() is the opt-in (INTEGRATION.md section 3k)
+        # xformers' FusedMLP is left alone as well; mlp.install_shims() is the opt-in (INTEGRATION.md section 3l)

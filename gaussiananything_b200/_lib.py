@@ -30,6 +30,8 @@ class GaGemmEpilogue(C.Structure):
 
 # GaGemmEpilogue.mode: the header's GA_EPI_* (tests/test_abi.py checks them against it)
 EPI_BF16, EPI_GELU_BF16, EPI_F32, EPI_RESID_GATE_F32, EPI_HEADS, EPI_GEGLU_BF16 = 0, 1, 2, 3, 4, 5
+# ga_linear_grad_validate's op: the header's GA_LINEAR_*
+LINEAR_FC1, LINEAR_DGRAD, LINEAR_WGRAD, LINEAR_BGRAD = 0, 1, 2, 3
 
 
 class GaVaeEncHead(C.Structure):
@@ -130,6 +132,14 @@ ABI = {
     "ga_attention_fwd_lse_bf16": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, f32, vp]),
     "ga_attention_bwd_bf16": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, f32,
                                     vp]),
+    "ga_linear_grad_validate": (i32, [i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, sz]),
+    "ga_linear_fc1_gelu_bf16": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]),
+    "ga_linear_dgrad_bf16": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp]),
+    "ga_linear_wgrad_splits": (i32, [i32, i32, i32]),
+    "ga_linear_wgrad_workspace_bytes": (sz, [i32, i32, i32]),
+    "ga_linear_wgrad_bf16": (i32, [vp, vp, vp, i32, i32, i32, vp, sz, vp]),
+    "ga_linear_bias_grad_workspace_bytes": (sz, [i32, i32]),
+    "ga_linear_bias_grad_bf16": (i32, [vp, vp, i32, i32, vp, sz, vp]),
     "ga_profile_enable": (i32, [i32]),
     "ga_profile_read": (i32, [C.POINTER(f32), i32]),
     "ga_b200_version": (C.c_char_p, []),

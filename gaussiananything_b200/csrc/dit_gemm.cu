@@ -66,6 +66,11 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b)
 constexpr int kStageBytes = 2048;          // per consumer warp
 constexpr int kWarpRows = 16;              // accumulator rows per warp
 
+// Epilogue of ga_linear_fc1_gelu_bf16 (include/ga_b200.h Part 13), outside the GA_EPI_* range so that
+// ga_gemm_bf16_tn never reaches it: H = bf16(gelu_erf(v)) to out and Z = bf16(v) to q, v = acc + bias, both bf16
+// [M, ld_out].  GaGemmEpilogue has no field for a second output; q is the one pointer this mode does not otherwise use.
+constexpr int kEpiGeluKeepPre = 100;
+
 // columns [32 ch, 32 ch + 32) of the warp's 16 rows -> staging (fp32, row-major, 128 B per row)
 template <int R>
 __device__ __forceinline__ void stage_chunk(uint32_t stg, int lane, const float (&acc)[R], int ch)
@@ -185,6 +190,21 @@ __device__ __forceinline__ void epilogue_chunk(const GaGemmEpilogue &ep, uint32_
             } else {
 #pragma unroll
                 for (int j = 0; j < 4; j++) if (nn + j < N) dst[j] += g[j] * v[j];
+            }
+        } else if (MODE == kEpiGeluKeepPre) {
+            __nv_bfloat16 *dh = reinterpret_cast<__nv_bfloat16 *>(ep.out) + (size_t)m * ep.ld_out + nn;
+            __nv_bfloat16 *dz = reinterpret_cast<__nv_bfloat16 *>(ep.q) + (size_t)m * ep.ld_out + nn;
+            if (vec) {
+                *reinterpret_cast<uint2 *>(dz) = make_uint2(pack_bf16(v[0], v[1]), pack_bf16(v[2], v[3]));
+                *reinterpret_cast<uint2 *>(dh) = make_uint2(pack_bf16(gelu_erf(v[0]), gelu_erf(v[1])),
+                                                            pack_bf16(gelu_erf(v[2]), gelu_erf(v[3])));
+            } else {
+#pragma unroll
+                for (int j = 0; j < 4; j++)
+                    if (nn + j < N) {
+                        dz[j] = __float2bfloat16(v[j]);
+                        dh[j] = __float2bfloat16(gelu_erf(v[j]));
+                    }
             }
         }
     }
@@ -535,4 +555,34 @@ extern "C" int ga_gemm_bf16_tn(const void *A, int lda, const void *W, int ldw, i
     if (bn == 128) return launch_gemm<128>(A, lda, W, ldw, *epi, M, N, K, s);
     if (bn == 192) return launch_gemm<192>(A, lda, W, ldw, *epi, M, N, K, s);
     return launch_gemm<256>(A, lda, W, ldw, *epi, M, N, K, s);
+}
+
+// fc1 of a FusedMLP for training (Part 13): the GEMM above with the kEpiGeluKeepPre epilogue.
+template <int BN>
+static int launch_fc1(const void *x, const void *w1, const GaGemmEpilogue &ep, int M, int N, int K, cudaStream_t s)
+{
+    CUtensorMap ta, tb;
+    int rc = ga_make_tmap_bf16(&ta, x, (uint64_t)M, (uint64_t)K, (uint64_t)K, BM);
+    if (rc) return rc;
+    rc = ga_make_tmap_bf16(&tb, w1, (uint64_t)N, (uint64_t)K, (uint64_t)K, (uint32_t)BN);
+    if (rc) return rc;
+    return launch_gemm_mode<BN, kEpiGeluKeepPre>(ta, tb, ep, M, N, K, s);
+}
+
+extern "C" int ga_linear_fc1_gelu_bf16(const void *x, const void *w1, const float *b1, void *h, void *z, int M, int N,
+                                       int K, int block_n, void *stream)
+{
+    const int rc = ga_linear_grad_validate(GA_LINEAR_FC1, x, w1, z, h, 0, M, N, K, block_n, nullptr, 0);
+    if (rc) return rc;
+    GaGemmEpilogue ep = {};
+    ep.mode = kEpiGeluKeepPre;
+    ep.bias = b1;
+    ep.out = h;
+    ep.ld_out = N;
+    ep.q = z;
+    cudaStream_t s = (cudaStream_t)stream;
+    if (block_n == 64) return launch_fc1<64>(x, w1, ep, M, N, K, s);
+    if (block_n == 128) return launch_fc1<128>(x, w1, ep, M, N, K, s);
+    if (block_n == 192) return launch_fc1<192>(x, w1, ep, M, N, K, s);
+    return launch_fc1<256>(x, w1, ep, M, N, K, s);
 }

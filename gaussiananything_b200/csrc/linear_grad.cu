@@ -1,0 +1,403 @@
+// Linear-layer gradients on wgmma for training (include/ga_b200.h Part 13): for y = x W^T with x [M, K] and the
+// nn.Linear weight W [N, K],
+//   dgrad  out[M, K] = G[M, N] W[N, K]     (optionally fused with the GELU backward: dZ = bf16(v gelu'(Z)))
+//   wgrad  dW[N, K]  = G^T x               (fp32, the parameter layout, split over M)
+//   bias   db[N]     = column sums of G
+// bf16 operands, fp32 accumulation in registers, no atomics.
+//
+// The GEMMs are the persistent kernel of dit_gemm.cu with different operand majors: one CTA per SM loops over
+// 128 x 128 output tiles; warpgroup 0 is the TMA producer (one elected thread), warpgroups 1-2 each own 64 rows and
+// run wgmma m64n128k16 from a ring of shared-memory stages guarded by full/empty mbarriers.  The operands that are
+// contiguous along an output dimension ("MN-major": W in dgrad, both G and x in wgrad) are fed with wgmma's
+// transposed operand mode on the 128-byte-swizzled TMA box as it lands: a box {64 along M or N, 64 along K} is
+// exactly the MN-major swizzle atom wgmma reads (wgmma_desc_mn_sw128), so these operands go from global memory to
+// the tensor cores with no shared-memory pass and the same pipeline as the forward.  attention_grad.cu builds
+// transposed copies instead because it stages with cp.async through arbitrary strides and uses the same tiles as
+// K-major operands of other products in the kernel; neither applies here.
+//
+// wgrad splits its contraction (the M rows) into S consecutive ranges of 64-row blocks so that small weights still
+// fill the GPU (the SRT's 256 x 1024 weight has 16 output tiles); S depends on the shapes alone, so the bits do not
+// depend on the card.  Each range writes an fp32 partial; a second kernel adds them in split order.
+#include "../../include/ga_b200.h"
+#include "device_once.cuh"
+#include "sm90_ptx.cuh"
+
+using namespace sm90;
+
+int ga_make_tmap_bf16(CUtensorMap *map, const void *ptr, uint64_t rows, uint64_t cols, uint64_t ld_elems,
+                      uint32_t box_rows);
+
+namespace {
+
+constexpr int BM = 128, BN = 128, BK = 64;
+constexpr int kThreads = 128 + 256;                 // producer warpgroup + 2 consumer warpgroups
+constexpr int kConsumerWarps = 8;
+constexpr int kABytes = BM * BK * 2, kBBytes = BN * BK * 2;
+constexpr int kHalf = 64 * BK * 2;                  // one 64-wide box: 8 KB
+constexpr int kStages = 6;
+constexpr int kSmem = kStages * (kABytes + kBBytes) + 1024;
+
+constexpr int kDgrad = 0, kWgrad = 1;               // kernel kinds: A K-major or MN-major (B is MN-major in both)
+constexpr int kEpiBf16 = 0, kEpiF32 = 1, kEpiGeluBwd = 2;
+
+constexpr int kColRows = 256;                       // bias gradient: rows per chunk
+constexpr int kColWarps = 8;
+
+struct GradArgs {
+    void *out;                      // [Mo, No] (+ split * split_stride for wgrad partials)
+    const __nv_bfloat16 *z;         // kEpiGeluBwd: fc1's pre-activation, bf16 [Mo, No]
+    int Mo, No;                     // output rows and columns
+    int nkb;                        // 64-deep blocks of the contraction
+    int splits;
+    long long split_stride;         // elements between partials
+};
+
+__device__ __forceinline__ uint32_t pack_bf16(float a, float b)
+{
+    __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+    return *reinterpret_cast<uint32_t *>(&h);
+}
+
+// d/dz of z Phi(z): Phi(z) + z phi(z), fp32
+__device__ __forceinline__ float gelu_grad(float z)
+{
+    const float cdf = 0.5f * (1.0f + erff(z * 0.70710678118654752f));
+    const float pdf = 0.39894228040143268f * expf(-0.5f * z * z);
+    return fmaf(z, pdf, cdf);
+}
+
+struct TileCoord { int m0, n0, kb0, kb1; long long split; };
+
+__device__ __forceinline__ TileCoord tile_coord(const GradArgs &a, int tile, int num_m, int per_split)
+{
+    TileCoord t;
+    const int split = tile / per_split, r = tile - split * per_split;
+    t.m0 = (r % num_m) * BM;
+    t.n0 = (r / num_m) * BN;
+    t.kb0 = (int)((long long)split * a.nkb / a.splits);
+    t.kb1 = (int)((long long)(split + 1) * a.nkb / a.splits);
+    t.split = split;
+    return t;
+}
+
+// Accumulator of wgmma m64n128 (warp w of the warpgroup, lane l): acc[4 j + e] is row 16 w + l / 4 + 8 (e >> 1),
+// column 8 j + 2 (l % 4) + (e & 1).  Stored straight from registers as column pairs (No % 8 == 0, so a pair is
+// either wholly inside or wholly outside).
+template <int EPI>
+__device__ __forceinline__ void epilogue(const GradArgs &a, const float (&acc)[64], int row0, int n0, long long split,
+                                         int lane)
+{
+    const int r = lane >> 2, c = 2 * (lane & 3);
+    // Z is read up front, all in flight at once: interleaved with the stores below the compiler must assume they
+    // alias, and each element would wait for its own load
+    uint32_t zr[2][BN / 8];
+    if constexpr (EPI == kEpiGeluBwd) {
+#pragma unroll
+        for (int hf = 0; hf < 2; hf++) {
+            const int row = row0 + r + 8 * hf;
+#pragma unroll
+            for (int j = 0; j < BN / 8; j++) {
+                const int col = n0 + 8 * j + c;
+                zr[hf][j] = (row < a.Mo && col < a.No)
+                                ? __ldg(reinterpret_cast<const unsigned int *>(a.z + (size_t)row * a.No + col))
+                                : 0u;
+            }
+        }
+    }
+#pragma unroll
+    for (int hf = 0; hf < 2; hf++) {
+        const int row = row0 + r + 8 * hf;
+        if (row >= a.Mo) continue;
+#pragma unroll
+        for (int j = 0; j < BN / 8; j++) {
+            const int col = n0 + 8 * j + c;
+            if (col >= a.No) continue;
+            const size_t idx = (size_t)row * a.No + col;
+            const float v0 = acc[4 * j + 2 * hf], v1 = acc[4 * j + 2 * hf + 1];
+            if constexpr (EPI == kEpiBf16) {
+                *reinterpret_cast<uint32_t *>(reinterpret_cast<__nv_bfloat16 *>(a.out) + idx) = pack_bf16(v0, v1);
+            } else if constexpr (EPI == kEpiF32) {
+                *reinterpret_cast<float2 *>(reinterpret_cast<float *>(a.out) + split * a.split_stride + idx) =
+                    make_float2(v0, v1);
+            } else {
+                const float2 zz = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&zr[hf][j]));
+                *reinterpret_cast<uint32_t *>(reinterpret_cast<__nv_bfloat16 *>(a.out) + idx) =
+                    pack_bf16(v0 * gelu_grad(zz.x), v1 * gelu_grad(zz.y));
+            }
+        }
+    }
+}
+
+// Persistent: grid = min(#tiles, #SMs); producer and consumers walk the same tile sequence.  Which CTA takes a tile
+// does not change its result.
+template <int KIND, int EPI>
+__global__ void __launch_bounds__(kThreads, 1)
+linear_grad_gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
+                        const GradArgs a)
+{
+    extern __shared__ uint8_t smem_raw[];
+    __shared__ uint64_t full_bar[kStages], empty_bar[kStages];
+    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t *smem_a = smem, *smem_b = smem + kStages * kABytes;
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;
+    const int num_m = (a.Mo + BM - 1) / BM, num_n = (a.No + BN - 1) / BN;
+    const int per_split = num_m * num_n, tiles = per_split * a.splits;
+
+    if (threadIdx.x == 0) {
+        prefetch_tmap(&tma_a);
+        prefetch_tmap(&tma_b);
+        for (int s = 0; s < kStages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps); }
+        fence_barrier_init();
+    }
+    __syncthreads();
+    pdl_wait();
+    pdl_launch_dependents();
+
+    if (wg == 0) {
+        setmaxnreg_dec<40>();
+        if (warp == 0 && elect_one()) {
+            int it = 0;
+            for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+                const TileCoord t = tile_coord(a, tile, num_m, per_split);
+                for (int kb = t.kb0; kb < t.kb1; kb++, it++) {
+                    const int s = it % kStages;
+                    mbar_wait(&empty_bar[s], ((it / kStages) & 1) ^ 1);
+                    mbar_expect_tx(&full_bar[s], kABytes + kBBytes);
+                    uint8_t *sa = smem_a + s * kABytes, *sb = smem_b + s * kBBytes;
+                    if (KIND == kDgrad) {
+                        tma_load_2d(sa, &tma_a, &full_bar[s], kb * BK, t.m0);            // G [M, N]: 128 rows
+                    } else {
+                        tma_load_2d(sa, &tma_a, &full_bar[s], t.m0, kb * BK);            // G [M, N]: columns m0..
+                        tma_load_2d(sa + kHalf, &tma_a, &full_bar[s], t.m0 + 64, kb * BK);
+                    }
+                    tma_load_2d(sb, &tma_b, &full_bar[s], t.n0, kb * BK);
+                    tma_load_2d(sb + kHalf, &tma_b, &full_bar[s], t.n0 + 64, kb * BK);
+                }
+            }
+        }
+    } else {
+        setmaxnreg_inc<232>();
+        const int cw = wg - 1;                      // which 64-row half of the tile
+        const int wi = warp & 3;                    // 16-row slice of that half
+        float acc[64];
+        int it = 0;
+        for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+            const TileCoord t = tile_coord(a, tile, num_m, per_split);
+            for (int kb = t.kb0; kb < t.kb1; kb++, it++) {
+                const int s = it % kStages;
+                mbar_wait(&full_bar[s], (it / kStages) & 1);
+                const uint32_t sa = smem_u32(smem_a + s * kABytes + cw * kHalf);
+                const uint64_t ad = KIND == kDgrad ? wgmma_desc_k_sw128(sa) : wgmma_desc_mn_sw128(sa, kHalf);
+                const uint64_t bd = wgmma_desc_mn_sw128(smem_u32(smem_b + s * kBBytes), kHalf);
+                constexpr uint64_t a_step = KIND == kDgrad ? 2 : 128;      // 16 columns (32 B) or 16 rows (2 KB)
+                fence_regs(acc);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; k++)
+                    wgmma_m64n128k16_ss_t<KIND == kDgrad ? 0 : 1, 1>(acc, ad + a_step * k, bd + 128 * k,
+                                                                     (uint32_t)((kb != t.kb0) | k));
+                wgmma_commit();
+                fence_regs(acc);
+                wgmma_wait<1>();                    // the previous stage's MMAs have retired: release its slot
+                fence_regs(acc);
+                if (kb > t.kb0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % kStages]);
+            }
+            wgmma_wait<0>();
+            fence_regs(acc);
+            if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % kStages]);
+            epilogue<EPI>(a, acc, t.m0 + cw * 64 + wi * 16, t.n0, t.split, lane);
+        }
+    }
+}
+
+// dw = sum over s of ws[s], in split order (float4 lanes; N K is a multiple of 64)
+__global__ void split_sum_kernel(const float4 *__restrict__ ws, float4 *__restrict__ dw, long long n4, int splits)
+{
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+        float4 v = ws[i];
+        for (int s = 1; s < splits; s++) {
+            const float4 w = ws[s * n4 + i];
+            v.x += w.x; v.y += w.y; v.z += w.z; v.w += w.w;
+        }
+        dw[i] = v;
+    }
+}
+
+// Column sums of g bf16 [M, N], one block per (64 columns, chunk of kColRows rows): warp w adds rows w, w + 8, ...
+// of the chunk in order, lane l columns 2 l, 2 l + 1; the warp sums are added in warp order into out[chunk, :].
+__global__ void __launch_bounds__(32 * kColWarps)
+colsum_chunk_kernel(const __nv_bfloat16 *__restrict__ g, float *__restrict__ out, int M, int N, int col_blocks)
+{
+    __shared__ float2 part[kColWarps][32];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int chunk = blockIdx.x / col_blocks, cb = blockIdx.x - chunk * col_blocks;
+    const int c = cb * 64 + 2 * lane;
+    const long long r0 = (long long)chunk * kColRows, r1 = min((long long)M, r0 + kColRows);
+    float2 s = make_float2(0.f, 0.f);
+    if (c < N) {
+#pragma unroll 4
+        for (long long r = r0 + warp; r < r1; r += kColWarps) {
+            const float2 v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(g + r * N + c));
+            s.x += v.x;
+            s.y += v.y;
+        }
+    }
+    part[warp][lane] = s;
+    __syncthreads();
+    if (warp == 0 && c < N) {
+        float2 t = part[0][lane];
+#pragma unroll
+        for (int w = 1; w < kColWarps; w++) { t.x += part[w][lane].x; t.y += part[w][lane].y; }
+        *reinterpret_cast<float2 *>(out + (long long)chunk * N + c) = t;
+    }
+}
+
+// db[c] = sum over chunks, in chunk order, of part[chunk, c]
+__global__ void colsum_final_kernel(const float *__restrict__ part, float *__restrict__ db, int chunks, int N)
+{
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= N) return;
+    float s = part[c];
+    for (int k = 1; k < chunks; k++) s += part[(long long)k * N + c];
+    db[c] = s;
+}
+
+int wgrad_splits(int M, int N, int K)
+{
+    const long long tiles = (long long)((N + BM - 1) / BM) * ((K + BN - 1) / BN);
+    const int nkb = (M + BK - 1) / BK;
+    long long s = (256 + tiles - 1) / tiles;        // about 256 tiles in all
+    if (s > nkb / 2) s = nkb / 2;                   // at least two 64-row blocks per split
+    if (s > 32) s = 32;
+    return s < 1 ? 1 : (int)s;
+}
+
+int col_chunks(int M) { return (M + kColRows - 1) / kColRows; }
+
+bool misaligned(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
+
+template <int KIND, int EPI>
+int launch_grad_gemm(const CUtensorMap &ta, const CUtensorMap &tb, const GradArgs &a, cudaStream_t s)
+{
+    static GaPerDevice attr_set;
+    if (ga_first_use_on_device(attr_set)) {
+        cudaError_t e = cudaFuncSetAttribute(linear_grad_gemm_kernel<KIND, EPI>,
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
+        if (e != cudaSuccess) return (int)e;
+    }
+    const long long tiles = (long long)((a.Mo + BM - 1) / BM) * ((a.No + BN - 1) / BN) * a.splits;
+    const int sms = ga_sm_count();
+    const int grid = tiles < sms ? (int)tiles : sms;
+    return (int)ga_launch_pdl(linear_grad_gemm_kernel<KIND, EPI>, dim3(grid), dim3(kThreads), (size_t)kSmem, s, ta, tb,
+                              a);
+}
+
+}  // namespace
+
+extern "C" int ga_linear_wgrad_splits(int M, int N, int K)
+{
+    if (M < 1 || N < 1 || K < 1) return 1;
+    return wgrad_splits(M, N, K);
+}
+
+extern "C" size_t ga_linear_wgrad_workspace_bytes(int M, int N, int K)
+{
+    const int s = ga_linear_wgrad_splits(M, N, K);
+    return s > 1 ? (size_t)s * (size_t)N * (size_t)K * sizeof(float) : 0;
+}
+
+extern "C" size_t ga_linear_bias_grad_workspace_bytes(int M, int N)
+{
+    if (M < 1 || N < 1) return 0;
+    const int chunks = col_chunks(M);
+    return chunks > 1 ? (size_t)chunks * (size_t)N * sizeof(float) : 0;
+}
+
+extern "C" int ga_linear_grad_validate(int op, const void *a, const void *b, const void *aux, const void *out,
+                                       int out_f32, int M, int N, int K, int block_n, const void *workspace,
+                                       size_t workspace_bytes)
+{
+    if (op < GA_LINEAR_FC1 || op > GA_LINEAR_BGRAD) return GA_ERR_BADARG;
+    if (M < 1 || N < 8 || N % 8) return GA_ERR_BADARG;
+    if (op != GA_LINEAR_BGRAD && (K < 8 || K % 8)) return GA_ERR_BADARG;
+    const long long wide = (op == GA_LINEAR_BGRAD || N >= K) ? N : K;
+    if ((long long)M * wide >= (1LL << 31)) return GA_ERR_BADARG;
+    if (!a || misaligned(a) || !out || misaligned(out)) return GA_ERR_BADARG;
+    size_t need = 0;
+    switch (op) {
+    case GA_LINEAR_FC1:
+        if (!b || misaligned(b) || !aux || misaligned(aux) || out_f32 != 0) return GA_ERR_BADARG;
+        if (block_n != 64 && block_n != 128 && block_n != 192 && block_n != 256) return GA_ERR_BADARG;
+        return 0;
+    case GA_LINEAR_DGRAD:
+        if (!b || misaligned(b) || (out_f32 != 0 && out_f32 != 1)) return GA_ERR_BADARG;
+        if (aux && (misaligned(aux) || out_f32)) return GA_ERR_BADARG;
+        return 0;
+    case GA_LINEAR_WGRAD:
+        if (!b || misaligned(b) || out_f32 != 1) return GA_ERR_BADARG;
+        need = ga_linear_wgrad_workspace_bytes(M, N, K);
+        break;
+    default:
+        if (out_f32 != 1) return GA_ERR_BADARG;
+        need = ga_linear_bias_grad_workspace_bytes(M, N);
+        break;
+    }
+    if (workspace_bytes < need || (need > 0 && (!workspace || misaligned(workspace)))) return GA_ERR_BADARG;
+    return 0;
+}
+
+extern "C" int ga_linear_dgrad_bf16(const void *g, const void *w, const void *z, void *out, int out_f32, int M, int N,
+                                    int K, void *stream)
+{
+    int rc = ga_linear_grad_validate(GA_LINEAR_DGRAD, g, w, z, out, out_f32, M, N, K, 0, nullptr, 0);
+    if (rc) return rc;
+    CUtensorMap ta, tb;
+    rc = ga_make_tmap_bf16(&ta, g, (uint64_t)M, (uint64_t)N, (uint64_t)N, BM);        // K-major: 128 rows
+    if (rc) return rc;
+    rc = ga_make_tmap_bf16(&tb, w, (uint64_t)N, (uint64_t)K, (uint64_t)K, BK);        // MN-major: 64 rows along N
+    if (rc) return rc;
+    GradArgs a = {out, reinterpret_cast<const __nv_bfloat16 *>(z), M, K, (N + BK - 1) / BK, 1, 0};
+    cudaStream_t s = (cudaStream_t)stream;
+    if (z) return launch_grad_gemm<kDgrad, kEpiGeluBwd>(ta, tb, a, s);
+    if (out_f32) return launch_grad_gemm<kDgrad, kEpiF32>(ta, tb, a, s);
+    return launch_grad_gemm<kDgrad, kEpiBf16>(ta, tb, a, s);
+}
+
+extern "C" int ga_linear_wgrad_bf16(const void *g, const void *x, float *dw, int M, int N, int K, void *workspace,
+                                    size_t workspace_bytes, void *stream)
+{
+    int rc = ga_linear_grad_validate(GA_LINEAR_WGRAD, g, x, nullptr, dw, 1, M, N, K, 0, workspace, workspace_bytes);
+    if (rc) return rc;
+    CUtensorMap ta, tb;
+    rc = ga_make_tmap_bf16(&ta, g, (uint64_t)M, (uint64_t)N, (uint64_t)N, BK);        // MN-major: 64 rows along M
+    if (rc) return rc;
+    rc = ga_make_tmap_bf16(&tb, x, (uint64_t)M, (uint64_t)K, (uint64_t)K, BK);
+    if (rc) return rc;
+    const int S = wgrad_splits(M, N, K);
+    GradArgs a = {S > 1 ? workspace : dw, nullptr, N, K, (M + BK - 1) / BK, S, (long long)N * K};
+    cudaStream_t s = (cudaStream_t)stream;
+    rc = launch_grad_gemm<kWgrad, kEpiF32>(ta, tb, a, s);
+    if (rc || S == 1) return rc;
+    const long long n4 = (long long)N * K / 4;
+    const long long blocks = (n4 + 255) / 256;
+    split_sum_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, s>>>(
+        reinterpret_cast<const float4 *>(workspace), reinterpret_cast<float4 *>(dw), n4, S);
+    return (int)cudaGetLastError();
+}
+
+extern "C" int ga_linear_bias_grad_bf16(const void *g, float *db, int M, int N, void *workspace, size_t workspace_bytes,
+                                        void *stream)
+{
+    const int rc = ga_linear_grad_validate(GA_LINEAR_BGRAD, g, nullptr, nullptr, db, 1, M, N, 0, 0, workspace,
+                                           workspace_bytes);
+    if (rc) return rc;
+    cudaStream_t s = (cudaStream_t)stream;
+    const int chunks = col_chunks(M), col_blocks = (N + 63) / 64;
+    float *part = chunks > 1 ? reinterpret_cast<float *>(workspace) : db;
+    colsum_chunk_kernel<<<(unsigned)((long long)chunks * col_blocks), 32 * kColWarps, 0, s>>>(
+        reinterpret_cast<const __nv_bfloat16 *>(g), part, M, N, col_blocks);
+    if (chunks > 1) colsum_final_kernel<<<(N + 255) / 256, 256, 0, s>>>(part, db, chunks, N);
+    return (int)cudaGetLastError();
+}

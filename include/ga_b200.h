@@ -799,6 +799,71 @@ int ga_attention_bwd_bf16(const void *q, const void *k, const void *v, const voi
                           const void *dout, float *delta, void *dq, void *dk, void *dv, int batch, int heads, int Nq,
                           int Nk, int d_qk, int d_v, const int64_t *strides, float scale, void *stream);
 
+/*
+ * ---------------------------------------------------------------------------
+ * Part 13: linear-layer gradients and a differentiable FusedMLP (xformers' FusedMLP: Linear(D -> hidden, no bias),
+ * bias + exact GELU, Linear(hidden -> D, no bias), bias; csrc/linear_grad.cu and csrc/dit_gemm.cu).
+ * For y = x W^T + b with x [M, K], W [N, K] (the nn.Linear parameter layout) and the output gradient G = dy [M, N]:
+ *   dx = G W          (dgrad: contracts W along its rows)
+ *   dW = G^T x        (wgrad: contracts both along the M rows)
+ *   db = sum_m G[m, :]
+ * The MLP forward for training keeps fc1's pre-activation: v = x W1^T + b1, Z = bf16(v), H = bf16(gelu_erf(v)),
+ * y = H W2^T + b2.  Its backward: db2 = colsum(dY), dW2 = dY^T H, dZ = bf16((dY W2) o gelu'(Z)), db1 = colsum(dZ),
+ * dW1 = dZ^T x, dx = dZ W1, with gelu'(z) = Phi(z) + z phi(z) evaluated in fp32 from the bf16 Z.
+ * Rounding: every GEMM operand is bf16 (x, W1, W2, H, dY, dZ; the fp32 parameters are packed to bf16 row-major on
+ * every call), products are accumulated in fp32 by wgmma; Z and H are stored as bf16; dgrad outputs are bf16 or fp32
+ * as asked; dW and db are fp32.  No atomics anywhere: the same inputs give the same bits on any H100.
+ * Every row count M >= 1 is accepted; N and K (and every pitch, which equals the row length) are multiples of 8, the
+ * TMA pitch; rows and columns past the end of a tile are zero-filled by TMA and never written.
+ * wgrad splits the M rows into S consecutive ranges of 64-row blocks (S from ga_linear_wgrad_splits: the shapes only,
+ * never the SM count), each range's fp32 partial [N, K] is written to the workspace, and dW = the partials added in
+ * fp32 in split order (S = 1 writes dW directly).  Bias gradients (ga_linear_bias_grad_bf16) sum the bf16 matrix
+ * given (dY for db2, the bf16 dZ for db1) in fp32: within a chunk of 256 rows, warp w (0..7) adds rows w, w + 8, ...
+ * in increasing order, the eight warp sums are added in warp order, then the chunks are added in chunk order.
+ * Test bounds (tests/mlp_grad_ref.py): a bf16-emulating fp64 reference rounds where these kernels round; the GPU
+ * results are held to 1.5 times its measured distance from fp64.  Timings: profiles/mlp_grad_h100.md.
+ * ---------------------------------------------------------------------------
+ */
+#define GA_LINEAR_FC1    0   /* ga_linear_fc1_gelu_bf16 */
+#define GA_LINEAR_DGRAD  1   /* ga_linear_dgrad_bf16 */
+#define GA_LINEAR_WGRAD  2   /* ga_linear_wgrad_bf16 */
+#define GA_LINEAR_BGRAD  3   /* ga_linear_bias_grad_bf16 */
+/* Host only, no CUDA call: 0 when the entry point `op` (GA_LINEAR_*) accepts the arguments, else GA_ERR_BADARG.
+ * The arguments of each op (a, b, aux, out as below; every pointer given must be 16-byte aligned):
+ *   FC1:   a = x [M, K], b = W1 [N, K], aux = Z, out = H [M, N]; all non-NULL; out_f32 == 0; block_n in {64, 128,
+ *          192, 256} (ga_gemm_bf16_tn's tile widths);
+ *   DGRAD: a = G [M, N], b = W [N, K], out [M, K] (fp32 when out_f32, else bf16) non-NULL; aux = Z [M, K] or NULL,
+ *          and with Z the output is bf16 (out_f32 == 0); out_f32 0 or 1;
+ *   WGRAD: a = G [M, N], b = x [M, K], out = dW fp32 [N, K] non-NULL; out_f32 == 1; workspace_bytes >=
+ *          ga_linear_wgrad_workspace_bytes(M, N, K), and the workspace non-NULL when that is > 0;
+ *   BGRAD: a = G [M, N] non-NULL, out = db fp32 [N] non-NULL; out_f32 == 1; K is ignored; workspace as for WGRAD
+ *          with ga_linear_bias_grad_workspace_bytes(M, N).
+ * M >= 1; N >= 8 and K >= 8 multiples of 8 (K unused by BGRAD); M * max(N, K) < 2^31. */
+int ga_linear_grad_validate(int op, const void *a, const void *b, const void *aux, const void *out, int out_f32, int M,
+                            int N, int K, int block_n, const void *workspace, size_t workspace_bytes);
+/* fc1 of the MLP for training: v = x W1^T + b1 (b1 fp32 [N] or NULL), H = bf16(gelu_erf(v)), Z = bf16(v), both bf16
+ * [M, N] (row pitch N).  x bf16 [M, K], W1 bf16 [N, K].  The ga_gemm_bf16_tn kernel at tile width block_n, with an
+ * epilogue that writes both outputs from one accumulator; gelu_erf is GA_EPI_GELU_BF16's. */
+int ga_linear_fc1_gelu_bf16(const void *x, const void *w1, const float *b1, void *h, void *z, int M, int N, int K,
+                            int block_n, void *stream);
+/* dgrad: out[M, K] = G[M, N] W[N, K], G and W bf16 row-major (W as stored, the parameter packed to bf16).  z == NULL:
+ * out = the fp32 product (out_f32) or its bf16 rounding.  z bf16 [M, K]: out bf16 = bf16(v gelu'(z)), v the fp32
+ * product (fc2's dgrad fused with the GELU backward: dZ). */
+int ga_linear_dgrad_bf16(const void *g, const void *w, const void *z, void *out, int out_f32, int M, int N, int K,
+                         void *stream);
+/* Number of M splits ga_linear_wgrad_bf16 uses for these shapes (>= 1).  Host only. */
+int ga_linear_wgrad_splits(int M, int N, int K);
+/* Bytes of workspace ga_linear_wgrad_bf16 needs (0 when there is one split).  Host only. */
+size_t ga_linear_wgrad_workspace_bytes(int M, int N, int K);
+/* wgrad: dW fp32 [N, K] = G^T x, G bf16 [M, N], x bf16 [M, K], split over M as stated above. */
+int ga_linear_wgrad_bf16(const void *g, const void *x, float *dw, int M, int N, int K, void *workspace,
+                         size_t workspace_bytes, void *stream);
+/* Bytes of workspace ga_linear_bias_grad_bf16 needs (0 when M <= 256).  Host only. */
+size_t ga_linear_bias_grad_workspace_bytes(int M, int N);
+/* db fp32 [N] = column sums of G bf16 [M, N], in the order stated above. */
+int ga_linear_bias_grad_bf16(const void *g, float *db, int M, int N, void *workspace, size_t workspace_bytes,
+                             void *stream);
+
 /* Measurement aid: when enabled, cudaEvents are recorded around every kernel
  * stage of the next forward/backward; ga_profile_read synchronises on them and
  * returns per-stage milliseconds: [0] preprocess, [1] binning, [2] render fwd,
