@@ -140,6 +140,18 @@ ABI = {
     "ga_linear_wgrad_bf16": (i32, [vp, vp, vp, i32, i32, i32, vp, sz, vp]),
     "ga_linear_bias_grad_workspace_bytes": (sz, [i32, i32]),
     "ga_linear_bias_grad_bf16": (i32, [vp, vp, i32, i32, vp, sz, vp]),
+    "ga_dit_grad_partials": (i32, [i32, i32]),
+    "ga_dit_rmsnorm_bwd_validate": (i32, [vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32]),
+    "ga_dit_rmsnorm_bwd": (i32, [vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp]),
+    "ga_dit_gate_bwd_validate": (i32, [vp, vp, vp, i32, vp, vp, i32, i32, i32, i32]),
+    "ga_dit_gate_bwd": (i32, [vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, vp]),
+    "ga_dit_gate_residual_validate": (i32, [vp, vp, vp, i32, vp, vp, vp, vp, i32, vp, i32, i32, i32]),
+    "ga_dit_gate_residual": (i32, [vp, vp, vp, i32, vp, vp, vp, vp, i32, vp, i32, i32, i32, f32, vp]),
+    "ga_dit_qk_norm_validate": (i32, [i32, vp, i32, vp, i32, vp, i32, vp, vp, vp, i32, i32, i32]),
+    "ga_dit_qk_norm_fwd_bf16": (i32, [vp, i32, vp, i32, vp, vp, i32, i32, i32, f32, vp]),
+    "ga_dit_qk_norm_bwd_bf16": (i32, [vp, i32, vp, i32, vp, i32, vp, vp, vp, i32, i32, i32, f32, vp]),
+    "ga_dit_grad_reduce_validate": (i32, [vp, vp, i32, i32, i32]),
+    "ga_dit_grad_reduce": (i32, [vp, vp, i32, i32, i32, vp]),
     "ga_profile_enable": (i32, [i32]),
     "ga_profile_read": (i32, [C.POINTER(f32), i32]),
     "ga_b200_version": (C.c_char_p, []),

@@ -21,7 +21,7 @@ import math
 import torch
 import torch.nn as nn
 
-from . import _launch, _lib
+from . import _launch, _lib, dit_grad
 from ._launch import epilogue, gemm, ptr as _p, round_up as _round_up
 from ._lib import EPI_F32, EPI_GELU_BF16, EPI_HEADS, EPI_RESID_GATE_F32
 # dit.EPI_*, dit.GaGemmEpilogue, dit._gemm_config and dit._p: earlier homes of these names, still read by tools and tests
@@ -81,10 +81,12 @@ class _FusedMLP(nn.Module):     # xformers FusedMLP key layout: mlp.{0.weight, 1
 
 
 class ImageCondDiTBlockPixelArtRMSNormClayLRM(nn.Module):
-    """Parameter layout of /root/reference/dit/dit_models_xformers.py:717-763 (CA -> gated SA -> gated FFN)."""
+    """Parameter layout of /root/reference/dit/dit_models_xformers.py:717-763 (CA -> gated SA -> gated FFN), with the
+    reference's forward (:765-787) as a differentiable call of dit_grad.block_forward for training."""
 
     def __init__(self, hidden_size, num_heads, context_dim, mlp_ratio=4, **kw):
         super().__init__()
+        self.num_heads = num_heads
         self.scale_shift_table = nn.Parameter(torch.randn(6, hidden_size) / hidden_size ** 0.5)
         self.norm1 = _Weight(hidden_size)
         self.norm2 = _Weight(hidden_size)
@@ -94,6 +96,12 @@ class ImageCondDiTBlockPixelArtRMSNormClayLRM(nn.Module):
         self.cross_attn_dino = _CrossAttn(hidden_size, context_dim, num_heads)
         self.prenorm_ca_dino = _Weight(hidden_size)
         self.adaLN_modulation = None
+
+    def forward(self, x, t, dino_spatial_token, clip_caption_token=None, freqs_cis=None, **kwargs):
+        """x [B, N, D] + cross-attention on dino_spatial_token [B, M, Dc], gated self-attention and gated FFN
+        modulated by scale_shift_table + t (t [B, 6 D]).  clip_caption_token is ignored, as in the reference, where
+        the text cross-attention returns zeros; freqs_cis (RoPE) raises NotImplementedError."""
+        return dit_grad.block_forward(self, x, t, dino_spatial_token, freqs_cis=freqs_cis)
 
 
 class _TimestepEmbedder(nn.Module):

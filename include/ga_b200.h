@@ -864,6 +864,91 @@ size_t ga_linear_bias_grad_workspace_bytes(int M, int N);
 int ga_linear_bias_grad_bf16(const void *g, float *db, int M, int N, void *workspace, size_t workspace_bytes,
                              void *stream);
 
+/*
+ * ---------------------------------------------------------------------------
+ * Part 14: the row kernels of a trainable image-to-3D DiT block (ImageCondDiTBlockPixelArtRMSNormClayLRM,
+ * gaussiananything_b200/dit_grad.py; csrc/dit_grad.cu).  With mod = scale_shift_table + t [B, 6 D] in the chunk order
+ * shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp, and b = r / rows_per_batch the batch item of row r:
+ *   RMSNorm-modulate   h = n w (1 + scale[b]) + shift[b],  n = x rstd,  rstd = (mean(x^2) + eps)^-1/2  (x fp32)
+ *     backward         dy0 = dh (1 + scale[b]),  dw = sum_r dy0 n,  dscale[b] = sum_{r in b} dh n w,
+ *                      dshift[b] = sum_{r in b} dh,  dx = dx_in + rstd (dy0 w - n mean(dy0 w n))
+ *                      (without modulation: scale = shift = 0 and no dscale, dshift)
+ *   q/k RMSNorm        per 64-column head: qn = bf16(n w), n = q rstd over the head's 64 values (q bf16)
+ *     backward         dq = bf16(rstd (dn - n mean(dn n))), dn = dqn w;  dw = sum over rows and heads of dqn n
+ *   gated residual     x_out = x + gate[b] a (a fp32, the GEMM's output), optionally followed in the same pass by
+ *                      h = bf16(RMSNorm-modulate(x_out))
+ *     backward         da = bf16(gate[b] dy),  dgate[b] = sum_{r in b} dy a
+ * All arithmetic is fp32; the only bf16 roundings are of the outputs named bf16 above (h, qn, dq, da).  rstd is
+ * recomputed from x (or q) in the backward, nothing is saved but the inputs.
+ * Layouts: row-major, fp32 rows of D columns (D % 4 == 0, D <= 1024) at pitch D; modulation chunks are [B, mod_ld]
+ * pointers already offset to their chunk (shift = mod + 0 D, ...); q/k matrices are bf16 [rows, ld] with head h of
+ * part p (p = 0: the q or first block, 1: the k block) at columns 64 (p heads + h) .. + 63, the "(K H D)" layout of a
+ * qkv or kv GEMM output.  Columns past parts * heads * 64 (v, padding) are never read or written.
+ * Determinism, no atomics: sums over rows are taken in chunks of 32 rows, a chunk never crossing a batch item.  The
+ * row kernels (norm and gate backward) run one CTA per chunk, warp w (0..7) adding rows w, w + 8, ... of the chunk in
+ * increasing order, the eight warp sums then added in warp order into partial p = b * ceil(rows_per_batch / 32) + c
+ * (ga_dit_grad_partials(R, rows_per_batch) partials in all).  The q/k backward runs one CTA per chunk of 32 rows
+ * (ga_dit_grad_partials(rows, rows) of them); its 32 slots of 8 lanes take the chunk's (row, head) items s, s + 32,
+ * ... in row-major order and the slot sums are added in slot order; partial [part, chunk, 64].  ga_dit_grad_reduce
+ * then adds partials in index order.  The same inputs give the same bits on any H100.
+ * Test bounds (tests/dit_grad_ref.py): a bf16-emulating fp64 reference rounds where these kernels and Parts 12 and 13
+ * round; the GPU results are held to 1.5 times its distance from fp64.  Timings: profiles/dit_block_grad_h100.md.
+ * ---------------------------------------------------------------------------
+ */
+/* Number of partials of a row sum over `rows` rows in batch items of rows_per_batch rows (0 when rows is not a
+ * positive multiple of rows_per_batch).  Host only. */
+int ga_dit_grad_partials(int rows, int rows_per_batch);
+/* Host only, no CUDA call: 0 when ga_dit_rmsnorm_bwd accepts the arguments, else GA_ERR_BADARG.  R a positive multiple
+ * of rows_per_batch >= 1; 4 <= D <= 1024, D % 4 == 0; R D < 2^31; dh, x, w, part_dw non-NULL; dx_in only with dx_out;
+ * with scale: mod_ld >= D, part_dshift and part_dscale non-NULL, part_ld >= D, both lds multiples of 4; without
+ * scale: part_dshift and part_dscale NULL.  Every pointer given 16-byte aligned. */
+int ga_dit_rmsnorm_bwd_validate(const float *dh, const float *x, const float *w, const float *scale, int mod_ld,
+                                const float *dx_in, const float *dx_out, const float *part_dw,
+                                const float *part_dshift, const float *part_dscale, int part_ld, int rows_per_batch,
+                                int R, int D);
+/* RMSNorm(-modulate) backward as above.  dh, x, dx fp32 [R, D]; scale [B, mod_ld] (NULL: no modulation); dx_out =
+ * dx_in + dRMSNorm (dx_in NULL: 0; dx_out NULL: dx is not formed; dx_in may be dx_out); partials part_dw [P, D] and,
+ * with scale, part_dshift / part_dscale [P, part_ld], P = ga_dit_grad_partials(R, rows_per_batch). */
+int ga_dit_rmsnorm_bwd(const float *dh, const float *x, const float *w, const float *scale, int mod_ld,
+                       const float *dx_in, float *dx_out, float *part_dw, float *part_dshift, float *part_dscale,
+                       int part_ld, int rows_per_batch, int R, int D, float eps, void *stream);
+/* Host only: as ga_dit_rmsnorm_bwd_validate for ga_dit_gate_bwd; dy, a, gate, part_dgate non-NULL and 16-byte
+ * aligned, da_bf16 non-NULL and 8-byte aligned, gate_ld and part_ld >= D and multiples of 4. */
+int ga_dit_gate_bwd_validate(const float *dy, const float *a, const float *gate, int gate_ld, const void *da_bf16,
+                             const float *part_dgate, int part_ld, int rows_per_batch, int R, int D);
+/* Gate backward: da bf16 [R, D] = bf16(gate[b] dy), part_dgate [P, part_ld] the chunk sums of dy a. */
+int ga_dit_gate_bwd(const float *dy, const float *a, const float *gate, int gate_ld, void *da_bf16, float *part_dgate,
+                    int part_ld, int rows_per_batch, int R, int D, void *stream);
+/* Host only: 0 when ga_dit_gate_residual accepts the arguments.  Rows as above; x, a, x_out non-NULL; a gate given
+ * with gate_ld >= D; w NULL: shift, scale and h_bf16 NULL too; w given: h_bf16 non-NULL (8-byte aligned), shift and
+ * scale both NULL or both given with mod_ld >= D; fp32 pointers 16-byte aligned, lds multiples of 4. */
+int ga_dit_gate_residual_validate(const float *x, const float *a, const float *gate, int gate_ld, const float *x_out,
+                                  const float *w, const float *shift, const float *scale, int mod_ld,
+                                  const void *h_bf16, int rows_per_batch, int R, int D);
+/* x_out [R, D] = x + gate[b] a (gate NULL: x + a); with w, also h_bf16 = RMSNorm(x_out) w [(1 + scale[b]) +
+ * shift[b]] (ga_rmsnorm_modulate's formula, on the fp32 x_out). */
+int ga_dit_gate_residual(const float *x, const float *a, const float *gate, int gate_ld, float *x_out, const float *w,
+                         const float *shift, const float *scale, int mod_ld, void *h_bf16, int rows_per_batch, int R,
+                         int D, float eps, void *stream);
+/* Host only: 0 when the q/k RMSNorm forward (backward = 0: dout, ld_dout and part_dw unused and dout, part_dw NULL)
+ * or backward (1; out is din) accepts the arguments.  rows, heads >= 1; parts 1 (w1 NULL) or 2 (w1 non-NULL); every
+ * ld >= 64 heads parts and a multiple of 8; in, out, dout, w0, w1, part_dw 16-byte aligned. */
+int ga_dit_qk_norm_validate(int backward, const void *in, int ld_in, const void *dout, int ld_dout, const void *out,
+                            int ld_out, const float *w0, const float *w1, const float *part_dw, int rows, int heads,
+                            int parts);
+/* q/k RMSNorm forward: out = bf16(n w) per head, w = w0 [64] for part 0 and w1 [64] for part 1.  out may be in. */
+int ga_dit_qk_norm_fwd_bf16(const void *in, int ld_in, void *out, int ld_out, const float *w0, const float *w1,
+                            int rows, int heads, int parts, float eps, void *stream);
+/* q/k RMSNorm backward: in = the pre-norm q/k, dout = the attention's dq/dk (bf16), din = the pre-norm gradient
+ * (bf16; din may be dout); part_dw fp32 [parts, ga_dit_grad_partials(rows, rows), 64]. */
+int ga_dit_qk_norm_bwd_bf16(const void *in, int ld_in, const void *dout, int ld_dout, void *din, int ld_din,
+                            const float *w0, const float *w1, float *part_dw, int rows, int heads, int parts,
+                            float eps, void *stream);
+/* Host only: 0 when part and out are non-NULL and groups, parts, cols >= 1. */
+int ga_dit_grad_reduce_validate(const float *part, const float *out, int groups, int parts, int cols);
+/* out [groups, cols] = sum over p = 0, 1, ..., parts - 1 (in that order, fp32) of part [groups, parts, cols]. */
+int ga_dit_grad_reduce(const float *part, float *out, int groups, int parts, int cols, void *stream);
+
 /* Measurement aid: when enabled, cudaEvents are recorded around every kernel
  * stage of the next forward/backward; ga_profile_read synchronises on them and
  * returns per-stage milliseconds: [0] preprocess, [1] binning, [2] render fwd,
