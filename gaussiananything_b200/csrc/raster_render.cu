@@ -509,10 +509,14 @@ cudaError_t ga_launch_render_fwd(const RasterDims &d, const RasterWs &w, const f
 // The records never leave the SM.  Tiles whose lists overflowed (and callers with list_k == 0) take the recompute
 // path of the same launch.
 // ---------------------------------------------------------------------------
-// Two CTAs per SM: ~104 KB of shared memory and up to 128 registers each.  Three (2048 records, 80 registers) were
+// Two CTAs per SM: ~88 KB of shared memory and up to 128 registers each.  Three (2048 records, 80 registers) were
 // measured slower on C2, 0.465 against 0.407 ms: the recurrence state that phase A carries across phase B does not
 // fit next to phase B's accumulators in 80 registers (176 B of spills).
-#define BWD_RECORDS 4096            /* window record buffer, 64 KB */
+// Records per window, C2 on an H100 SXM at 700 W (profiles/raster_bwd_phase_b_h100.md): 4096 gave render_bwd 0.407 ms,
+// 3072 0.378 ms, 3584 0.379 ms and 2048 0.395 ms.  With 3072, C2 needs a quarter more windows (tools/raster_rounds.py),
+// yet staging and phase A take 10-14 % fewer cycles per launch; the two CTAs then leave the SM 60 KB of L1 instead of
+// 28 KB, which is the likely cause (not measured).
+#define BWD_RECORDS 3072            /* window record buffer, 48 KB */
 #define BWD_TPI 2                   /* lanes per instance in phase B */
 
 struct BwdSmem {

@@ -6,6 +6,10 @@ and the totals of the forward's split mapping (csrc/raster_render.cu) beside tho
   phase 1: (instance, pixel) pairs inside the clipped cull boxes, packed 32 per warp iteration, per window of FWD_PAIRS
   phase 2: per warp and window, the largest number of box pairs of one of its pixels (an upper bound: only the pairs
            that reach alpha >= 1/255 are composited)
+and the backward's phase B: serial record iterations per window (the longest walk of one lane) when every instance
+gets two lanes, sorted by record count with 16 instances per warp (csrc/raster_render.cu), and when the window's
+records are spread evenly over the 256 lanes, for windows of 4096 and 3072 records.  A record is a box pixel in front of the pixel's last
+contributor, an upper bound on the forward's contributions.
 Cull boxes are approximated by the low-pass disc.  Counts, not timings.
     python tools/raster_rounds.py [tiles per view, or 0 for all] [views]"""
 import os
@@ -20,6 +24,28 @@ from tests.helpers import cameras, oracle_view, scene  # noqa: E402
 CHUNK, FWD_PAIRS = 256, 4096
 
 
+def windows(cc, limit):
+    """Splits a chunk's per-slot counts into windows of consecutive slots whose counts fit `limit`."""
+    incl = np.cumsum(cc)
+    t0, base = 0, 0
+    while t0 < len(cc):
+        t1 = t0 + int(((incl - base <= limit) & (np.arange(len(cc)) >= t0)).sum())
+        yield t0, t1
+        base, t0 = int(incl[t1 - 1]), t1
+
+
+def phase_b_pairs(c):
+    """Two lanes per instance, instances sorted by count, 16 per warp and 128 per round: the slowest warp's iterations."""
+    c = np.sort(c[c > 0])[::-1]
+    per_warp = np.zeros(8, np.int64)
+    for b0 in range(0, len(c), 128):
+        rnd = -(-c[b0:b0 + 128] // 2)
+        for w in range(8):
+            if 16 * w < len(rnd):
+                per_warp[w] += rnd[16 * w:16 * w + 16].max()
+    return int(per_warp.max())
+
+
 def main():
     ntiles = int(sys.argv[1]) if len(sys.argv) > 1 else 200
     nviews = int(sys.argv[2]) if len(sys.argv) > 2 else 1
@@ -28,6 +54,9 @@ def main():
     vs, ps, _, _ = cameras(6)
     tot = dict(gs32=0, gs16=0, gs8=0, lane=0, lane_sub32=0, lane_grp128=0, useful=0)
     split = dict(gs8_rounds=0, pairs=0, phase1_warp_iters=0, phase2_rounds=0, windows=0, chunks=0, max_chunk_pairs=0)
+    # phase B: (records per window, windows, serial iterations) per scheme; instances per window and records per instance
+    pb = {"pairs 4096": [4096, 0, 0], "pairs 3072": [3072, 0, 0], "even 4096": [4096, 0, 0], "even 3072": [3072, 0, 0]}
+    pb_records, pb_inst, pb_inst_max, pb_rec_max = 0, 0, 0, 0
     nw = 0
     for view in range(nviews):
         o = oracle_view(g, vs[view], ps[view], [1, 1, 1], H, W)
@@ -35,7 +64,7 @@ def main():
         tau = 2 * np.log(np.maximum(255 * opa, 1.0)) * 1.001 + 1e-3
         r2 = np.sqrt(0.5 * tau) + 0.51                  # the low-pass disc of K1's cull box (the 3-D part is tiny here)
         bx0, bx1, by0, by1 = xy[:, 0] - r2, xy[:, 0] + r2, xy[:, 1] - r2, xy[:, 1] + r2
-        ids, rng = o["ids"], o["ranges"]
+        ids, rng, last = o["ids"], o["ranges"], o["n_contrib"][0]
         tiles = np.arange(len(rng)) if ntiles <= 0 else np.random.default_rng(0).choice(len(rng), ntiles, replace=False)
         for t in tiles:
             a, b = rng[t]
@@ -83,9 +112,30 @@ def main():
                     per_pix = pix[:, c0 + t0:c0 + t1].sum(1)
                     split["phase2_rounds"] += sum(int(per_pix[wpx].max()) for wpx in warp_pix)
                     base, t0 = int(incl[t1 - 1]), t1
+            # backward: slot t of a chunk is list position hi - 1 - t, chunks from the tile's deepest contributor down
+            lc = last[oy:oy + 16, ox:ox + 16].reshape(256)
+            recs = (pix & (np.arange(len(sid))[None, :] < lc[:, None])).sum(0)
+            for hi in range(int(lc.max()), 0, -CHUNK):
+                cc = recs[max(0, hi - CHUNK):hi][::-1]
+                pb_records += int(cc.sum())
+                for key, v in pb.items():
+                    for t0, t1 in windows(cc, v[0]):
+                        w = cc[t0:t1]
+                        v[1] += 1
+                        v[2] += phase_b_pairs(w) if key.startswith("pairs") else -(-int(w.sum()) // 256)
+                        if key == "pairs 4096":
+                            pb_inst += int((w > 0).sum())
+                            pb_inst_max = max(pb_inst_max, int((w > 0).sum()))
+                            pb_rec_max = max(pb_rec_max, int(w.max()))
     print("rounds per warp (C2 scene, %s tiles x %d views): " % ("all" if ntiles <= 0 else ntiles, nviews)
           + ", ".join("%s %.1f" % (k, v / nw) for k, v in tot.items()))
     print("split forward totals (FWD_PAIRS %d): " % FWD_PAIRS + ", ".join("%s %d" % kv for kv in split.items()))
+    nwin = pb["pairs 4096"][1]
+    print("backward phase B (%d records; with 4096 records per window: %d windows, instances per window mean %.1f max %d, "
+          "records per instance mean %.1f max %d): " % (pb_records, nwin, pb_inst / nwin, pb_inst_max,
+                                                        pb_records / max(pb_inst, 1), pb_rec_max)
+          + ", ".join("%s: %d windows, serial iterations %.1f per window, %d in all" % (k, v[1], v[2] / v[1], v[2])
+                      for k, v in pb.items()))
 
 
 if __name__ == "__main__":
