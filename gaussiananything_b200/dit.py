@@ -133,6 +133,8 @@ class _XYZPosEmbed(nn.Module):
 
 
 class DiT_I23D_PCD_PixelArt_noclip(nn.Module):
+    xyz_cond = False        # True for the stage-2 models: context["fps-xyz"] conditions the tokens
+
     def __init__(self, input_size=32, patch_size=2, in_channels=4, hidden_size=1152, depth=28, num_heads=16,
                  mlp_ratio=4, class_dropout_prob=0.1, num_classes=1000, learn_sigma=True, mixing_logit_init=-3,
                  mixed_prediction=True, context_dim=False, pooling_ctx_dim=768, roll_out=False, vit_blk=None,
@@ -265,6 +267,8 @@ def _param_versions(model):
 
 
 class DiT_I23D_PCD_PixelArt_noclip_clay_stage2(DiT_I23D_PCD_PixelArt_noclip):
+    xyz_cond = True
+
     def __init__(self, *a, use_pe_cond=False, **kw):
         super().__init__(*a, **kw)
         self.has_caption = False
@@ -283,8 +287,16 @@ class DiT_I23D_PCD_PixelArt_noclip_clay_stage2(DiT_I23D_PCD_PixelArt_noclip):
 # --------------------------------------------------------------------------
 # engine: bf16 weight pack + workspaces + launch sequence (+ CUDA graph)
 # --------------------------------------------------------------------------
+_ATTN_SCALE = 1.0 / math.sqrt(64.0)        # softmax scale of head_dim 64
+
+
 class _DiTEngine:
+    """The image model's engine.  The text-to-3D engine (dit_t23d._T23DEngine) overrides only the class attributes
+    below, the final layer's modulation and the context K/V with its per-block context norm."""
     ctx_key, vec_key = "img_crossattn", "img_vector"          # the conditioner's output keys this model reads
+    block_order = ("cross_attn", "self_attn", "ffn")          # the sublayer methods each block launches, in order
+    vec_embedder = "pooled_vec_embedder"                      # the model's LayerNorm + Linear of the pooled vector
+    ca_modules = ("cross_attn_dino", "prenorm_ca_dino")       # a block's cross-attention and its pre-norm
 
     def __init__(self, model, device):
         self.L = _bind()
@@ -293,7 +305,7 @@ class _DiTEngine:
         self.D, self.H, self.depth = model.embed_dim, model.num_heads, model.depth
         self.Cin, self.Cout = model.in_channels, model.out_channels
         self.Dc = model.context_dim
-        self.stage2 = isinstance(model, DiT_I23D_PCD_PixelArt_noclip_clay_stage2)
+        self.stage2 = model.xyz_cond
         self.use_pe = self.stage2 and model.use_pe_cond
         self.use_graph = True
         self.tap_blocks = False            # tests: keep the residual stream after every block (s["taps"][l])
@@ -307,15 +319,20 @@ class _DiTEngine:
         self._graph = None
 
     # ---- weights
+    def _f32(self, t):
+        return t.detach().to(device=self.device, dtype=torch.float32).contiguous()
+
+    def _b16(self, t):
+        return t.detach().to(device=self.device, dtype=torch.bfloat16).contiguous()
+
     def _pack(self):
-        m, dev = self.m, self.device
-        f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()
-        b16 = lambda t: t.detach().to(device=dev, dtype=torch.bfloat16).contiguous()
+        m, dev, f32, b16 = self.m, self.device, self._f32, self._b16
+        vec = getattr(m, self.vec_embedder)
         w = {}
         w["t0_w"], w["t0_b"] = f32(m.t_embedder.mlp[0].weight), f32(m.t_embedder.mlp[0].bias)
         w["t2_w"], w["t2_b"] = f32(m.t_embedder.mlp[2].weight), f32(m.t_embedder.mlp[2].bias)
-        w["pv_ln_w"], w["pv_ln_b"] = f32(m.pooled_vec_embedder[0].weight), f32(m.pooled_vec_embedder[0].bias)
-        w["pv_w"], w["pv_b"] = f32(m.pooled_vec_embedder[1].weight), f32(m.pooled_vec_embedder[1].bias)
+        w["vec_ln_w"], w["vec_ln_b"] = f32(vec[0].weight), f32(vec[0].bias)
+        w["vec_w"], w["vec_b"] = f32(vec[1].weight), f32(vec[1].bias)
         w["ada_w"], w["ada_b"] = f32(m.adaLN_modulation[1].weight), f32(m.adaLN_modulation[1].bias)
         w["fc1_w"], w["fc1_b"] = f32(m.x_embedder.fc1.weight), f32(m.x_embedder.fc1.bias)
         w["fc2_w"], w["fc2_b"] = b16(m.x_embedder.fc2.weight), f32(m.x_embedder.fc2.bias)
@@ -324,24 +341,29 @@ class _DiTEngine:
             wx[:, :63] = f32(m.xyz_pos_embed.xyz_projection.weight)
             w["xyz_w"], w["xyz_b"] = wx.to(torch.bfloat16).contiguous(), f32(m.xyz_pos_embed.xyz_projection.bias)
         w["tables"] = torch.stack([f32(b.scale_shift_table) for b in m.blocks]).contiguous()      # [L,6,D]
-        w["table_f"] = f32(m.final_layer.scale_shift_table)
+        w.update(self._pack_final_modulation())
         w["fin_w"], w["fin_b"] = f32(m.final_layer.linear.weight), f32(m.final_layer.linear.bias)
-        blocks = []
-        for b in m.blocks:
-            ca, sa, mlp = b.cross_attn_dino, b.attn, b.mlp.mlp
-            blocks.append(dict(
-                pre_w=f32(b.prenorm_ca_dino.weight), n1_w=f32(b.norm1.weight), n2_w=f32(b.norm2.weight),
-                caq_w=b16(ca.to_q.weight), cakv_w=b16(torch.cat([ca.to_k.weight, ca.to_v.weight], 0)),
-                caq_n=f32(ca.q_norm.weight), cak_n=f32(ca.k_norm.weight),
-                cao_w=b16(ca.to_out[0].weight), cao_b=f32(ca.to_out[0].bias),
-                qkv_w=b16(sa.qkv.weight), qkv_b=f32(sa.qkv.bias), q_n=f32(sa.q_norm.weight), k_n=f32(sa.k_norm.weight),
-                proj_w=b16(sa.proj.weight), proj_b=f32(sa.proj.bias),
-                w1=b16(mlp[0].weight), b1=f32(mlp[1].bias), w2=b16(mlp[2].weight), b2=f32(mlp[3].bias),
-                # |q.k|/8 <= (sqrt(64) max|wq|)(sqrt(64) max|wk|)/8 for RMS-normalised q, k (+2% for bf16 rounding):
-                # lets the attention kernel skip the running maximum (ga_b200.h: score_bound)
-                ca_bound=8.16 * float(ca.q_norm.weight.detach().abs().max()) * float(ca.k_norm.weight.detach().abs().max()),
-                sa_bound=8.16 * float(sa.q_norm.weight.detach().abs().max()) * float(sa.k_norm.weight.detach().abs().max())))
-        self.w, self.wb = w, blocks
+        self.w, self.wb = w, [self._pack_block(b) for b in m.blocks]
+
+    def _pack_block(self, b):
+        f32, b16 = self._f32, self._b16
+        ca, pre = (getattr(b, n) for n in self.ca_modules)
+        sa, mlp = b.attn, b.mlp.mlp
+        # |q.k|/8 <= (sqrt(64) max|wq|)(sqrt(64) max|wk|)/8 for RMS-normalised q, k (+2% for bf16 rounding):
+        # lets the attention kernel skip the running maximum (ga_b200.h: score_bound)
+        bound = lambda a: 8.16 * float(a.q_norm.weight.detach().abs().max()) * float(a.k_norm.weight.detach().abs().max())
+        return dict(
+            pre_w=f32(pre.weight), n1_w=f32(b.norm1.weight), n2_w=f32(b.norm2.weight),
+            caq_w=b16(ca.to_q.weight), cakv_w=b16(torch.cat([ca.to_k.weight, ca.to_v.weight], 0)),
+            caq_n=f32(ca.q_norm.weight), cak_n=f32(ca.k_norm.weight),
+            cao_w=b16(ca.to_out[0].weight), cao_b=f32(ca.to_out[0].bias),
+            qkv_w=b16(sa.qkv.weight), qkv_b=f32(sa.qkv.bias), q_n=f32(sa.q_norm.weight), k_n=f32(sa.k_norm.weight),
+            proj_w=b16(sa.proj.weight), proj_b=f32(sa.proj.bias),
+            w1=b16(mlp[0].weight), b1=f32(mlp[1].bias), w2=b16(mlp[2].weight), b2=f32(mlp[3].bias),
+            ca_bound=bound(ca), sa_bound=bound(sa))
+
+    def _pack_final_modulation(self):
+        return {"table_f": self._f32(self.m.final_layer.scale_shift_table)}
 
     # ---- workspaces for a (B, N, M) problem
     def _alloc(self, B, N, M):
@@ -381,19 +403,69 @@ class _DiTEngine:
                          tok_pitch=self.Mp, rows_per_batch=M)
             gemm(s["ctx"], wb["cakv_w"], B * M, 2 * D, self.Dc, e, st)
 
+    def _final_modulation(self, st):
+        """modf [B, 2D] = final_layer.scale_shift_table + temb (T2IFinalLayer)."""
+        B, D = self._shape[0], self.D
+        _lib.check(self.L.ga_add_tables(_p(self.w["table_f"]), _p(self.s["temb"]), _p(self.s["modf"]), 1, B, 2 * D, D, st),
+                   "final modulation")
+
+    # ---- the block's sublayers: launches that update the residual stream xres.  l: the block's index, wb: its
+    # weights, ch: its six [B, D] modulation chunks (shift, scale and gate of the self-attention, then of the FFN)
+    def cross_attn(self, st, l, wb, ch):
+        """xres += CA(RMSNorm(xres; pre-norm)) against block l's cached context K/V: no modulation, no gate."""
+        L, s = self.L, self.s
+        B, N, M = self._shape
+        D, H, R = self.D, self.H, B * N
+        _lib.check(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["pre_w"]), None, None, 0, N, _p(s["h"]), R, D, 1e-5, st), "prenorm")
+        gemm(s["h"], wb["caq_w"], R, D, D,
+             epilogue(EPI_HEADS, q=s["q"], qn_w=wb["caq_n"], heads=H, first_part=0, tok_pitch=self.Np,
+                      rows_per_batch=N), st)
+        _lib.check(L.ga_attention_bf16(_p(s["q"]), _p(s["kc"][l]), _p(s["vtc"][l]), _p(s["ao"]), B, H, N, M, self.Np,
+                                       self.Mp, _ATTN_SCALE, wb["ca_bound"], st), "cross attention")
+        gemm(s["ao"], wb["cao_w"], R, D, D,
+             epilogue(EPI_RESID_GATE_F32, bias=wb["cao_b"], out=s["xres"], ld_out=D, rows_per_batch=N), st)
+
+    def self_attn(self, st, l, wb, ch):
+        """xres += gate_msa * SA(RMSNorm(xres) * (1 + scale_msa) + shift_msa)."""
+        L, s = self.L, self.s
+        B, N, M = self._shape
+        D, H, R = self.D, self.H, B * N
+        _lib.check(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["n1_w"]), _p(ch[0]), _p(ch[1]), 6 * D, N, _p(s["h"]), R, D,
+                                         1e-5, st), "norm1")
+        gemm(s["h"], wb["qkv_w"], R, 3 * D, D,
+             epilogue(EPI_HEADS, bias=wb["qkv_b"], q=s["q"], k=s["k"], vt=s["vt"], qn_w=wb["q_n"],
+                      kn_w=wb["k_n"], heads=H, first_part=0, tok_pitch=self.Np, rows_per_batch=N), st)
+        _lib.check(L.ga_attention_bf16(_p(s["q"]), _p(s["k"]), _p(s["vt"]), _p(s["ao"]), B, H, N, N, self.Np, self.Np,
+                                       _ATTN_SCALE, wb["sa_bound"], st), "self attention")
+        gemm(s["ao"], wb["proj_w"], R, D, D,
+             epilogue(EPI_RESID_GATE_F32, bias=wb["proj_b"], out=s["xres"], ld_out=D, gate=ch[2],
+                      gate_ld=6 * D, rows_per_batch=N), st)
+
+    def ffn(self, st, l, wb, ch):
+        """xres += gate_mlp * FFN(RMSNorm(xres) * (1 + scale_mlp) + shift_mlp)."""
+        L, s = self.L, self.s
+        B, N, M = self._shape
+        D, R = self.D, B * N
+        _lib.check(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["n2_w"]), _p(ch[3]), _p(ch[4]), 6 * D, N, _p(s["h"]), R, D,
+                                         1e-5, st), "norm2")
+        gemm(s["h"], wb["w1"], R, 4 * D, D, epilogue(EPI_GELU_BF16, bias=wb["b1"], out=s["hid"], ld_out=4 * D), st)
+        gemm(s["hid"], wb["w2"], R, D, 4 * D,
+             epilogue(EPI_RESID_GATE_F32, bias=wb["b2"], out=s["xres"], ld_out=D, gate=ch[5],
+                      gate_ld=6 * D, rows_per_batch=N), st)
+
     def _forward_launches(self, st, cfg_scale):
         L, s, w = self.L, self.s, self.w
         B, N, M = self._shape
-        D, H, R = self.D, self.H, B * N
-        # ---- prologue: timestep + pooled vector -> adaLN tables
+        D, R = self.D, B * N
+        # ---- prologue: timestep + pooled vector -> adaLN tables and the final layer's modulation
         _lib.check(L.ga_timestep_sinusoid(_p(s["t_in"]), _p(s["sinus"]), B, 256, st), "sinusoid")
         _lib.check(L.ga_linear_small(_p(s["sinus"]), _p(w["t0_w"]), _p(w["t0_b"]), _p(s["h1"]), B, D, 256, 0, 1, 0, st), "t0")
         _lib.check(L.ga_linear_small(_p(s["h1"]), _p(w["t2_w"]), _p(w["t2_b"]), _p(s["temb"]), B, D, D, 0, 0, 0, st), "t2")
-        _lib.check(L.ga_layernorm_rows(_p(s["vec_in"]), _p(w["pv_ln_w"]), _p(w["pv_ln_b"]), _p(s["vln"]), B, self.Dc, 1e-5, st), "ln")
-        _lib.check(L.ga_linear_small(_p(s["vln"]), _p(w["pv_w"]), _p(w["pv_b"]), _p(s["temb"]), B, D, self.Dc, 0, 0, 1, st), "pv")
+        _lib.check(L.ga_layernorm_rows(_p(s["vec_in"]), _p(w["vec_ln_w"]), _p(w["vec_ln_b"]), _p(s["vln"]), B, self.Dc, 1e-5, st), "ln")
+        _lib.check(L.ga_linear_small(_p(s["vln"]), _p(w["vec_w"]), _p(w["vec_b"]), _p(s["temb"]), B, D, self.Dc, 0, 0, 1, st), "vec")
         _lib.check(L.ga_linear_small(_p(s["temb"]), _p(w["ada_w"]), _p(w["ada_b"]), _p(s["t0"]), B, 6 * D, D, 1, 0, 0, st), "ada")
         _lib.check(L.ga_add_tables(_p(w["tables"]), _p(s["t0"]), _p(s["mod"]), self.depth, B, 6 * D, 6 * D, st), "tables")
-        _lib.check(L.ga_add_tables(_p(w["table_f"]), _p(s["temb"]), _p(s["modf"]), 1, B, 2 * D, D, st), "table_f")
+        self._final_modulation(st)
         # ---- token embedder
         concat = self.stage2 and not self.use_pe
         _lib.check(L.ga_embed_fc1(_p(s["x_in"]), self.Cin, _p(s["xyz_in"]) if concat else None, 3 if concat else 0,
@@ -404,37 +476,10 @@ class _DiTEngine:
             gemm(s["pe"], w["xyz_w"], R, D, 64,
                  epilogue(EPI_RESID_GATE_F32, bias=w["xyz_b"], out=s["xres"], ld_out=D, rows_per_batch=N), st)
         # ---- blocks
-        scale = 1.0 / math.sqrt(64.0)
         for l, wb in enumerate(self.wb):
-            mod = s["mod"][l]                       # [B, 6D]
-            ch = lambda j: mod[:, j * D:(j + 1) * D]
-            # cross attention (pre-norm, residual)
-            _lib.check(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["pre_w"]), None, None, 0, N, _p(s["h"]), R, D, 1e-5, st), "prenorm")
-            gemm(s["h"], wb["caq_w"], R, D, D,
-                 epilogue(EPI_HEADS, q=s["q"], qn_w=wb["caq_n"], heads=H, first_part=0, tok_pitch=self.Np,
-                          rows_per_batch=N), st)
-            _lib.check(L.ga_attention_bf16(_p(s["q"]), _p(s["kc"][l]), _p(s["vtc"][l]), _p(s["ao"]), B, H, N, M, self.Np,
-                                           self.Mp, scale, wb["ca_bound"], st), "cross attention")
-            gemm(s["ao"], wb["cao_w"], R, D, D,
-                 epilogue(EPI_RESID_GATE_F32, bias=wb["cao_b"], out=s["xres"], ld_out=D, rows_per_batch=N), st)
-            # gated self attention
-            _lib.check(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["n1_w"]), _p(ch(0)), _p(ch(1)), 6 * D, N, _p(s["h"]), R, D,
-                                             1e-5, st), "norm1")
-            gemm(s["h"], wb["qkv_w"], R, 3 * D, D,
-                 epilogue(EPI_HEADS, bias=wb["qkv_b"], q=s["q"], k=s["k"], vt=s["vt"], qn_w=wb["q_n"],
-                          kn_w=wb["k_n"], heads=H, first_part=0, tok_pitch=self.Np, rows_per_batch=N), st)
-            _lib.check(L.ga_attention_bf16(_p(s["q"]), _p(s["k"]), _p(s["vt"]), _p(s["ao"]), B, H, N, N, self.Np, self.Np,
-                                           scale, wb["sa_bound"], st), "self attention")
-            gemm(s["ao"], wb["proj_w"], R, D, D,
-                 epilogue(EPI_RESID_GATE_F32, bias=wb["proj_b"], out=s["xres"], ld_out=D, gate=ch(2),
-                          gate_ld=6 * D, rows_per_batch=N), st)
-            # gated FFN
-            _lib.check(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["n2_w"]), _p(ch(3)), _p(ch(4)), 6 * D, N, _p(s["h"]), R, D,
-                                             1e-5, st), "norm2")
-            gemm(s["h"], wb["w1"], R, 4 * D, D, epilogue(EPI_GELU_BF16, bias=wb["b1"], out=s["hid"], ld_out=4 * D), st)
-            gemm(s["hid"], wb["w2"], R, D, 4 * D,
-                 epilogue(EPI_RESID_GATE_F32, bias=wb["b2"], out=s["xres"], ld_out=D, gate=ch(5),
-                          gate_ld=6 * D, rows_per_batch=N), st)
+            ch = s["mod"][l].chunk(6, 1)
+            for sublayer in self.block_order:
+                getattr(self, sublayer)(st, l, wb, ch)
             if self.tap_blocks:
                 s["taps"][l].copy_(s["xres"])
         # ---- final layer (+ CFG combine)

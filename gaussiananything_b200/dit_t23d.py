@@ -9,8 +9,8 @@
 Same constructor arguments, attribute names and state_dict key layout (a reference checkpoint loads with
 strict=True), same `forward(x, timesteps, context)` / `forward_with_cfg(x, t, context, cfg_scale)` contracts, with
 context = {"caption_crossattn" [B,M,Dc], "caption_vector" [B,Dc]} (+ "fps-xyz" [B,N,3] for stage 2).  The engine is
-the image DiT's (dit._DiTEngine: bf16 weight pack, workspaces, CUDA graph, cached cross-attention K/V) with the text
-block's launch sequence:
+the image DiT's (dit._DiTEngine: bf16 weight pack, workspaces, sublayer launches, CUDA graph, cached cross-attention
+K/V) in the text block's order and with its modules:
 
   t = t_embedder(t) + cap_embedder(caption_vector);  t0 = adaLN_modulation(t);  mod = scale_shift_table + t0
   x += gate_msa * SA(RMSNorm(x) * (1 + scale_msa) + shift_msa)
@@ -20,14 +20,12 @@ block's launch sequence:
 
 Precision as in dit.py: bf16 tensor-core operands, fp32 accumulation, residual stream, norms and output.
 """
-import math
-
 import torch
 import torch.nn as nn
 
 from . import _lib, dit
 from ._launch import epilogue, gemm, ptr as _p
-from ._lib import EPI_F32, EPI_GELU_BF16, EPI_HEADS, EPI_RESID_GATE_F32
+from ._lib import EPI_HEADS
 from .dit import _CrossAttn, _FusedMLP, _Mlp, _SelfAttn, _TimestepEmbedder, _Weight, _XYZPosEmbed
 
 
@@ -120,6 +118,8 @@ class DiT_PCD_PixelArt(dit.DiT_I23D_PCD_PixelArt_noclip):
 
 
 class DiT_PCD_PixelArt_tofeat(DiT_PCD_PixelArt):
+    xyz_cond = True
+
     def __init__(self, *a, use_pe_cond=True, **kw):
         super().__init__(*a, **kw)
         self.use_pe_cond = use_pe_cond
@@ -135,49 +135,25 @@ class DiT_PCD_PixelArt_tofeat(DiT_PCD_PixelArt):
 
 
 class _T23DEngine(dit._DiTEngine):
-    """dit._DiTEngine with the text block: per-block context RMSNorm before the cached K/V, SA -> CA -> FFN,
-    FinalLayer."""
+    """dit._DiTEngine with the text block: SA -> CA -> FFN, a per-block context RMSNorm before the cached K/V, and
+    FinalLayer's modulation."""
     ctx_key, vec_key = "caption_crossattn", "caption_vector"
+    block_order = ("self_attn", "cross_attn", "ffn")
+    vec_embedder = "cap_embedder"
+    ca_modules = ("cross_attn", "prenorm_ca_text")
 
-    def _pack(self):
-        m, dev = self.m, self.device
-        # set here because the base constructor's stage-2 test names the image model's class
-        self.stage2 = isinstance(m, DiT_PCD_PixelArt_tofeat)
-        self.use_pe = self.stage2 and m.use_pe_cond
-        f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()
-        b16 = lambda t: t.detach().to(device=dev, dtype=torch.bfloat16).contiguous()
-        w = {}
-        w["t0_w"], w["t0_b"] = f32(m.t_embedder.mlp[0].weight), f32(m.t_embedder.mlp[0].bias)
-        w["t2_w"], w["t2_b"] = f32(m.t_embedder.mlp[2].weight), f32(m.t_embedder.mlp[2].bias)
-        w["cap_ln_w"], w["cap_ln_b"] = f32(m.cap_embedder[0].weight), f32(m.cap_embedder[0].bias)
-        w["cap_w"], w["cap_b"] = f32(m.cap_embedder[1].weight), f32(m.cap_embedder[1].bias)
-        w["ada_w"], w["ada_b"] = f32(m.adaLN_modulation[1].weight), f32(m.adaLN_modulation[1].bias)
-        w["fc1_w"], w["fc1_b"] = f32(m.x_embedder.fc1.weight), f32(m.x_embedder.fc1.bias)
-        w["fc2_w"], w["fc2_b"] = b16(m.x_embedder.fc2.weight), f32(m.x_embedder.fc2.bias)
-        if self.use_pe:
-            wx = torch.zeros(self.D, 64, device=dev, dtype=torch.float32)
-            wx[:, :63] = f32(m.xyz_pos_embed.xyz_projection.weight)
-            w["xyz_w"], w["xyz_b"] = wx.to(torch.bfloat16).contiguous(), f32(m.xyz_pos_embed.xyz_projection.bias)
-        w["tables"] = torch.stack([f32(b.scale_shift_table) for b in m.blocks]).contiguous()      # [L,6,D]
-        w["fin_ada_w"] = f32(m.final_layer.adaLN_modulation[1].weight)
-        w["fin_ada_b"] = f32(m.final_layer.adaLN_modulation[1].bias)
-        w["fin_w"], w["fin_b"] = f32(m.final_layer.linear.weight), f32(m.final_layer.linear.bias)
-        blocks = []
-        for b in m.blocks:
-            ca, sa, mlp = b.cross_attn, b.attn, b.mlp.mlp
-            blocks.append(dict(
-                n1_w=f32(b.norm1.weight), n2_w=f32(b.norm2.weight), pre_w=f32(b.prenorm_ca_text.weight),
-                y_w=f32(b.attention_y_norm.weight),
-                caq_w=b16(ca.to_q.weight), cakv_w=b16(torch.cat([ca.to_k.weight, ca.to_v.weight], 0)),
-                caq_n=f32(ca.q_norm.weight), cak_n=f32(ca.k_norm.weight),
-                cao_w=b16(ca.to_out[0].weight), cao_b=f32(ca.to_out[0].bias),
-                qkv_w=b16(sa.qkv.weight), qkv_b=f32(sa.qkv.bias), q_n=f32(sa.q_norm.weight), k_n=f32(sa.k_norm.weight),
-                proj_w=b16(sa.proj.weight), proj_b=f32(sa.proj.bias),
-                w1=b16(mlp[0].weight), b1=f32(mlp[1].bias), w2=b16(mlp[2].weight), b2=f32(mlp[3].bias),
-                # score bounds of the RMS-normalised q, k (dit._DiTEngine._pack)
-                ca_bound=8.16 * float(ca.q_norm.weight.detach().abs().max()) * float(ca.k_norm.weight.detach().abs().max()),
-                sa_bound=8.16 * float(sa.q_norm.weight.detach().abs().max()) * float(sa.k_norm.weight.detach().abs().max())))
-        self.w, self.wb = w, blocks
+    def _pack_block(self, b):
+        return dict(super()._pack_block(b), y_w=self._f32(b.attention_y_norm.weight))
+
+    def _pack_final_modulation(self):
+        lin = self.m.final_layer.adaLN_modulation[1]
+        return {"fin_ada_w": self._f32(lin.weight), "fin_ada_b": self._f32(lin.bias)}
+
+    def _final_modulation(self, st):
+        """modf [B, 2D] = final_layer.adaLN_modulation(temb) = Linear(SiLU(temb)) (FinalLayer)."""
+        B, D, s, w = self._shape[0], self.D, self.s, self.w
+        _lib.check(self.L.ga_linear_small(_p(s["temb"]), _p(w["fin_ada_w"]), _p(w["fin_ada_b"]), _p(s["modf"]), B, 2 * D, D,
+                                          1, 0, 0, st), "final modulation")
 
     def _context_kv(self, st, c32):
         """Per block: RMSNorm(context; attention_y_norm) -> bf16 -> the K/V GEMM, once per context tensor."""
@@ -189,72 +165,6 @@ class _T23DEngine(dit._DiTEngine):
             e = epilogue(EPI_HEADS, k=s["kc"][l], vt=s["vtc"][l], kn_w=wb["cak_n"], heads=H, first_part=1,
                          tok_pitch=self.Mp, rows_per_batch=M)
             gemm(s["ctx"], wb["cakv_w"], B * M, 2 * D, self.Dc, e, st)
-
-    def _forward_launches(self, st, cfg_scale):
-        L, s, w = self.L, self.s, self.w
-        B, N, M = self._shape
-        D, H, R = self.D, self.H, B * N
-        # ---- prologue: t = t_embedder(t) + cap_embedder(caption_vector) -> adaLN tables and the final modulation
-        _lib.check(L.ga_timestep_sinusoid(_p(s["t_in"]), _p(s["sinus"]), B, 256, st), "sinusoid")
-        _lib.check(L.ga_linear_small(_p(s["sinus"]), _p(w["t0_w"]), _p(w["t0_b"]), _p(s["h1"]), B, D, 256, 0, 1, 0, st), "t0")
-        _lib.check(L.ga_linear_small(_p(s["h1"]), _p(w["t2_w"]), _p(w["t2_b"]), _p(s["temb"]), B, D, D, 0, 0, 0, st), "t2")
-        _lib.check(L.ga_layernorm_rows(_p(s["vec_in"]), _p(w["cap_ln_w"]), _p(w["cap_ln_b"]), _p(s["vln"]), B, self.Dc, 1e-5,
-                                       st), "cap ln")
-        _lib.check(L.ga_linear_small(_p(s["vln"]), _p(w["cap_w"]), _p(w["cap_b"]), _p(s["temb"]), B, D, self.Dc, 0, 0, 1, st),
-                   "cap")
-        _lib.check(L.ga_linear_small(_p(s["temb"]), _p(w["ada_w"]), _p(w["ada_b"]), _p(s["t0"]), B, 6 * D, D, 1, 0, 0, st), "ada")
-        _lib.check(L.ga_add_tables(_p(w["tables"]), _p(s["t0"]), _p(s["mod"]), self.depth, B, 6 * D, 6 * D, st), "tables")
-        _lib.check(L.ga_linear_small(_p(s["temb"]), _p(w["fin_ada_w"]), _p(w["fin_ada_b"]), _p(s["modf"]), B, 2 * D, D, 1, 0,
-                                     0, st), "final ada")
-        # ---- token embedder
-        concat = self.stage2 and not self.use_pe
-        _lib.check(L.ga_embed_fc1(_p(s["x_in"]), self.Cin, _p(s["xyz_in"]) if concat else None, 3 if concat else 0,
-                                  _p(w["fc1_w"]), _p(w["fc1_b"]), _p(s["e1"]), R, D, st), "embed_fc1")
-        gemm(s["e1"], w["fc2_w"], R, D, D, epilogue(EPI_F32, bias=w["fc2_b"], out=s["xres"], ld_out=D), st)
-        if self.use_pe:
-            _lib.check(L.ga_xyz_posenc(_p(s["xyz_in"]), _p(s["pe"]), R, st), "xyz_pe")
-            gemm(s["pe"], w["xyz_w"], R, D, 64,
-                 epilogue(EPI_RESID_GATE_F32, bias=w["xyz_b"], out=s["xres"], ld_out=D, rows_per_batch=N), st)
-        # ---- blocks
-        scale = 1.0 / math.sqrt(64.0)
-        for l, wb in enumerate(self.wb):
-            mod = s["mod"][l]                       # [B, 6D]
-            ch = lambda j: mod[:, j * D:(j + 1) * D]
-            # gated self attention
-            _lib.check(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["n1_w"]), _p(ch(0)), _p(ch(1)), 6 * D, N, _p(s["h"]), R, D,
-                                             1e-5, st), "norm1")
-            gemm(s["h"], wb["qkv_w"], R, 3 * D, D,
-                 epilogue(EPI_HEADS, bias=wb["qkv_b"], q=s["q"], k=s["k"], vt=s["vt"], qn_w=wb["q_n"],
-                          kn_w=wb["k_n"], heads=H, first_part=0, tok_pitch=self.Np, rows_per_batch=N), st)
-            _lib.check(L.ga_attention_bf16(_p(s["q"]), _p(s["k"]), _p(s["vt"]), _p(s["ao"]), B, H, N, N, self.Np, self.Np,
-                                           scale, wb["sa_bound"], st), "self attention")
-            gemm(s["ao"], wb["proj_w"], R, D, D,
-                 epilogue(EPI_RESID_GATE_F32, bias=wb["proj_b"], out=s["xres"], ld_out=D, gate=ch(2),
-                          gate_ld=6 * D, rows_per_batch=N), st)
-            # cross attention on the caption tokens (pre-norm, ungated residual)
-            _lib.check(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["pre_w"]), None, None, 0, N, _p(s["h"]), R, D, 1e-5, st),
-                       "prenorm_ca_text")
-            gemm(s["h"], wb["caq_w"], R, D, D,
-                 epilogue(EPI_HEADS, q=s["q"], qn_w=wb["caq_n"], heads=H, first_part=0, tok_pitch=self.Np,
-                          rows_per_batch=N), st)
-            _lib.check(L.ga_attention_bf16(_p(s["q"]), _p(s["kc"][l]), _p(s["vtc"][l]), _p(s["ao"]), B, H, N, M, self.Np,
-                                           self.Mp, scale, wb["ca_bound"], st), "cross attention")
-            gemm(s["ao"], wb["cao_w"], R, D, D,
-                 epilogue(EPI_RESID_GATE_F32, bias=wb["cao_b"], out=s["xres"], ld_out=D, rows_per_batch=N), st)
-            # gated FFN
-            _lib.check(L.ga_rmsnorm_modulate(_p(s["xres"]), _p(wb["n2_w"]), _p(ch(3)), _p(ch(4)), 6 * D, N, _p(s["h"]), R, D,
-                                             1e-5, st), "norm2")
-            gemm(s["h"], wb["w1"], R, 4 * D, D, epilogue(EPI_GELU_BF16, bias=wb["b1"], out=s["hid"], ld_out=4 * D), st)
-            gemm(s["hid"], wb["w2"], R, D, 4 * D,
-                 epilogue(EPI_RESID_GATE_F32, bias=wb["b2"], out=s["xres"], ld_out=D, gate=ch(5),
-                          gate_ld=6 * D, rows_per_batch=N), st)
-            if self.tap_blocks:
-                s["taps"][l].copy_(s["xres"])
-        # ---- FinalLayer (+ CFG combine)
-        _lib.check(L.ga_final_layer(_p(s["xres"]), _p(s["modf"]), _p(w["fin_w"]), _p(w["fin_b"]), _p(s["y"]), R, D,
-                                    self.Cout, N, 1e-6, st), "final layer")
-        if cfg_scale is not None:
-            _lib.check(L.ga_cfg_combine(_p(s["y"]), _p(s["y_cfg"]), (B // 2) * N * self.Cout, cfg_scale, st), "cfg")
 
 
 # --------------------------------------------------------------------------
