@@ -152,6 +152,14 @@ ABI = {
     "ga_dit_qk_norm_bwd_bf16": (i32, [vp, i32, vp, i32, vp, i32, vp, vp, vp, i32, i32, i32, f32, vp]),
     "ga_dit_grad_reduce_validate": (i32, [vp, vp, i32, i32, i32]),
     "ga_dit_grad_reduce": (i32, [vp, vp, i32, i32, i32, vp]),
+    "ga_dit_final_layer_bwd_validate": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32]),
+    "ga_dit_final_layer_bwd": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp]),
+    "ga_dit_embed_fc1_bwd_validate": (i32, [vp, i32, vp, i32, vp, vp, vp, vp, vp, vp, i32, i32]),
+    "ga_dit_embed_fc1_bwd": (i32, [vp, i32, vp, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp]),
+    "ga_dit_linear_small_bwd_validate": (i32, [vp, i32, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32]),
+    "ga_dit_linear_small_bwd": (i32, [vp, i32, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, vp]),
+    "ga_dit_layernorm_rows_bwd_validate": (i32, [vp, vp, vp, vp, vp, vp, i32, i32]),
+    "ga_dit_layernorm_rows_bwd": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, f32, vp]),
     "ga_profile_enable": (i32, [i32]),
     "ga_profile_read": (i32, [C.POINTER(f32), i32]),
     "ga_b200_version": (C.c_char_p, []),

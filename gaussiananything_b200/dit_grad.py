@@ -27,11 +27,12 @@ import math
 import torch
 
 from . import _lib
-from ._launch import ptr, stream
+from ._launch import epilogue, gemm, ptr, stream
+from ._lib import EPI_RESID_GATE_F32
 from .attention import _stride_table
 from .mlp import _bgrad, _dgrad, _fc1, _forward_linear, _pack, _wgrad
 
-__all__ = ["block_forward"]
+__all__ = ["block_forward", "model_forward"]
 
 _BF16, _F32 = torch.bfloat16, torch.float32
 _EPS = 1e-5
@@ -355,3 +356,351 @@ def block_forward(block, x, t, context, freqs_cis=None):
     with torch.cuda.device(x.device):
         y, _ = _forward(x, t, context, params, keep=False)
     return y.view(x.shape).to(x.dtype)
+
+
+# ---- the whole model: stem -> blocks -> head (include/ga_b200.h Part 15) ---------------------------------------------
+#
+# model_forward(model, x, timesteps, context) is DiT_I23D_PCD_PixelArt_noclip.forward (the reference's
+# dit/dit_i23d.py:511-567, stage 2 :707-750) with a backward, in three autograd pieces:
+#   stem   (x, img_vector, the stem parameters) -> (xres [B, N, D] the residual stream, t0 [B, 6 D], temb [B, D])
+#   blocks _DiTBlock per block, each fed the same t0, so autograd adds their dt
+#   head   (xres, temb, the final layer's parameters) -> y [B, N, out_channels]
+# The stem's backward gets dt0 from the blocks and dtemb from the head.  timesteps and context["fps-xyz"] are
+# constants.  The forward runs the launches of the inference engine (dit._DiTEngine._forward_launches) with the same
+# precision: the B-row stem in fp32, the token embedder's GEMMs on bf16 operands.
+
+_SMALL_ROWS = 16                                            # ga_linear_small's row limit
+
+
+def _linear_small(x, W, b, y, act_in=0, accumulate=0):
+    """y [B, N] (+)= act(x) W^T + b over 16-row chunks, any B (fp32 ga_linear_small)."""
+    B, K = x.shape
+    N = W.shape[0]
+    for r0 in range(0, B, _SMALL_ROWS):
+        n = min(_SMALL_ROWS, B - r0)
+        _lib.check(_lib.lib().ga_linear_small(_at(x, r0 * K), ptr(W), ptr(b), _at(y, r0 * N), n, N, K, act_in, 0,
+                                              accumulate, stream(x.device)), "ga_linear_small")
+
+
+def _linear_small_bwd(x, act_in, W, dy, want_w, want_b, want_x, dx_in=None):
+    """(dW, db, dx) of y = act(x) W^T + b for dy [B, N]; dx = dx_in + act'(x) (dy W).  None where not wanted."""
+    B, K = x.shape
+    N = W.shape[0]
+    L, dev = _lib.lib(), x.device
+    dW = torch.empty((N, K), dtype=_F32, device=dev) if want_w else None
+    db = torch.empty(N, dtype=_F32, device=dev) if want_b else None
+    dx = part = None
+    if want_x:
+        dx = torch.empty((B, K), dtype=_F32, device=dev)
+        part = torch.empty((L.ga_dit_grad_partials(N, N), B, K), dtype=_F32, device=dev)
+    if want_w or want_b or want_x:
+        _lib.check(L.ga_dit_linear_small_bwd(ptr(x), act_in, ptr(W), ptr(dy), ptr(dW), ptr(db), ptr(part),
+                                             ptr(dx_in if want_x else None), ptr(dx), B, N, K, stream(dev)),
+                   "ga_dit_linear_small_bwd")
+    return dW, db, dx
+
+
+def stem_parameters(model):
+    """The stem's parameters in the order the autograd function takes them."""
+    t, v, a, e = model.t_embedder.mlp, model.pooled_vec_embedder, model.adaLN_modulation[1], model.x_embedder
+    p = (t[0].weight, t[0].bias, t[2].weight, t[2].bias, v[0].weight, v[0].bias, v[1].weight, v[1].bias,
+         a.weight, a.bias, e.fc1.weight, e.fc1.bias, e.fc2.weight, e.fc2.bias)
+    if _uses_pe(model):
+        p += (model.xyz_pos_embed.xyz_projection.weight, model.xyz_pos_embed.xyz_projection.bias)
+    return p
+
+
+def head_parameters(model):
+    f = model.final_layer
+    return (f.scale_shift_table, f.linear.weight, f.linear.bias)
+
+
+def _uses_pe(model):
+    return bool(model.xyz_cond and model.use_pe_cond)
+
+
+def _stem_forward(x, vec, t, xyz, params, keep):
+    """(xres fp32 [B N, D], t0 [B, 6 D], temb [B, D], the saved state or None)."""
+    (t0_w, t0_b, t2_w, t2_b, ln_w, ln_b, v_w, v_b, a_w, a_b, f1_w, f1_b, f2_w, f2_b) = params[:14]
+    use_pe = len(params) == 16
+    B, N, Cin = x.shape
+    D, Dc, R = t2_w.shape[0], vec.shape[-1], B * N
+    dev = x.device
+    L, st = _lib.lib(), stream(dev)
+    f = [_f32(p) for p in (t0_w, t0_b, t2_w, t2_b, ln_w, ln_b, v_w, v_b, a_w, a_b, f1_w, f1_b, f2_b)]
+    t0_wf, t0_bf, t2_wf, t2_bf, ln_wf, ln_bf, v_wf, v_bf, a_wf, a_bf, f1_wf, f1_bf, f2_bf = f
+    f2_wb = _pack(f2_w)
+    tf = t.detach().to(_F32).reshape(-1).expand(B).contiguous() if t.numel() == 1 else _f32(t).view(B)
+    sinus = torch.empty((B, 256), dtype=_F32, device=dev)
+    _lib.check(L.ga_timestep_sinusoid(ptr(tf), ptr(sinus), B, 256, st), "ga_timestep_sinusoid")
+    a1 = torch.empty((B, D), dtype=_F32, device=dev)                   # t_embedder's pre-SiLU activation
+    _linear_small(sinus, t0_wf, t0_bf, a1)
+    temb = torch.empty((B, D), dtype=_F32, device=dev)
+    _linear_small(a1, t2_wf, t2_bf, temb, act_in=1)
+    vf = _f32(vec).view(B, Dc)
+    vln = torch.empty((B, Dc), dtype=_F32, device=dev)
+    _lib.check(L.ga_layernorm_rows(ptr(vf), ptr(ln_wf), ptr(ln_bf), ptr(vln), B, Dc, 1e-5, st), "ga_layernorm_rows")
+    _linear_small(vln, v_wf, v_bf, temb, accumulate=1)
+    t0 = torch.empty((B, 6 * D), dtype=_F32, device=dev)
+    _linear_small(temb, a_wf, a_bf, t0, act_in=1)
+    # token embedder (+ the xyz conditioning of stage 2)
+    xf = _f32(x).view(R, Cin)
+    xyzf = _f32(xyz).view(R, 3) if xyz is not None else None
+    concat = xyz is not None and not use_pe
+    e1 = torch.empty((R, D), dtype=_BF16, device=dev)
+    _lib.check(L.ga_embed_fc1(ptr(xf), Cin, ptr(xyzf) if concat else None, 3 if concat else 0, ptr(f1_wf), ptr(f1_bf),
+                              ptr(e1), R, D, st), "ga_embed_fc1")
+    xres = _forward_linear(e1, f2_wb, f2_bf, _F32)
+    pe = xyz_wb = None
+    if use_pe:
+        pe = torch.empty((R, 64), dtype=_BF16, device=dev)
+        _lib.check(L.ga_xyz_posenc(ptr(xyzf), ptr(pe), R, st), "ga_xyz_posenc")
+        xyz_wb = torch.zeros((D, 64), dtype=_BF16, device=dev)           # K padded 63 -> 64, the padded column 0
+        xyz_wb[:, :63] = params[14].detach()
+        gemm(pe, xyz_wb, R, D, 64, epilogue(EPI_RESID_GATE_F32, bias=_f32(params[15]), out=xres, ld_out=D,
+                                            rows_per_batch=N), st)
+    if not keep:
+        return xres, t0, temb, None
+    saved = (sinus, a1, vf, vln, temb, xf, e1, f2_wb, t0_wf, t2_wf, ln_wf, v_wf, a_wf, f1_wf, f1_bf)
+    saved += ((xyzf,) if xyz is not None else ()) + ((pe,) if use_pe else ())
+    return xres, t0, temb, saved
+
+
+class _DiTStem(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, vec, t, xyz, *params):
+        with torch.cuda.device(x.device):
+            xres, t0, temb, saved = _stem_forward(x, vec, t, xyz, params, keep=True)
+        ctx.save_for_backward(*saved, *params)
+        ctx.meta = (x.shape, x.dtype, vec.shape, vec.dtype, xyz is not None, len(params))
+        return xres.view(x.shape[0], x.shape[1], -1), t0, temb
+
+    @staticmethod
+    def backward(ctx, dxres, dt0, dtemb):
+        if torch.is_grad_enabled():
+            raise RuntimeError("dit_grad: double backward (create_graph=True) is not supported")
+        with torch.cuda.device(dxres.device):
+            return _stem_backward(ctx, dxres, dt0, dtemb)
+
+
+def _stem_backward(ctx, dxres, dt0, dtemb):
+    x_shape, x_dtype, v_shape, v_dtype, stage2, nparam = ctx.meta
+    use_pe = nparam == 16
+    saved = ctx.saved_tensors
+    params = saved[-nparam:]
+    sinus, a1, vf, vln, temb, xf, e1, f2_wb, t0_wf, t2_wf, ln_wf, v_wf, a_wf, f1_wf, f1_bf = saved[:15]
+    xyzf = saved[15] if stage2 else None
+    pe = saved[16] if use_pe else None
+    need = ctx.needs_input_grad
+    nx, nvec = need[0], need[1]
+    n = need[4:] + (False, False)
+    (n_t0w, n_t0b, n_t2w, n_t2b, n_lnw, n_lnb, n_vw, n_vb, n_aw, n_ab, n_f1w, n_f1b, n_f2w, n_f2b, n_xw, n_xb) = n[:16]
+    B, N, Cin = x_shape
+    D, R = temb.shape[1], B * N
+    dev = temb.device
+    L, st = _lib.lib(), stream(dev)
+    grads = [None] * (4 + nparam)
+    # ---- token embedder: xres = fc2(e1) (+ xyz projection)
+    fc1_side = nx or n_f1w or n_f1b
+    if fc1_side or n_f2w or n_f2b or n_xw or n_xb:
+        g = torch.empty((R, D), dtype=_BF16, device=dev)
+        _lib.check(L.ga_f32_to_bf16(ptr(dxres.to(_F32).contiguous()), ptr(g), R * D, st), "ga_f32_to_bf16")
+        if n_xw:
+            grads[4 + 14] = _wgrad(g, pe)[:, :63].contiguous()         # the padded column carries no parameter
+        if n_f2w:
+            grads[4 + 12] = _wgrad(g, e1)
+        if n_f2b or n_xb:
+            db = _bgrad(g)                               # fc2 and the xyz projection share their output's bias sum
+            if n_f2b:
+                grads[4 + 13] = db
+            if n_xb:
+                grads[4 + 15] = db.clone() if n_f2b else db              # one tensor per .grad
+        if fc1_side:
+            de1 = _dgrad(g, f2_wb, f32=True)
+            concat = stage2 and not use_pe
+            K = Cin + (3 if concat else 0)
+            P = L.ga_dit_grad_partials(R, R)
+            pw, pb = (torch.empty((P, D * K), dtype=_F32, device=dev), torch.empty((P, D), dtype=_F32, device=dev))
+            dxin = torch.empty((R, Cin), dtype=_F32, device=dev) if nx else None
+            _lib.check(L.ga_dit_embed_fc1_bwd(ptr(xf), Cin, ptr(xyzf) if concat else None, 3 if concat else 0,
+                                              ptr(f1_wf), ptr(f1_bf), ptr(de1), ptr(pw), ptr(pb), ptr(dxin), R, D, st),
+                       "ga_dit_embed_fc1_bwd")
+            if n_f1w:
+                grads[4 + 10] = _reduce(pw, 1, D * K).view(D, K)
+            if n_f1b:
+                grads[4 + 11] = _reduce(pb, 1, D)[0]
+            if nx:
+                grads[0] = dxin.view(x_shape).to(x_dtype)
+    # ---- vector path: t0 = ada(silu(temb)), temb = t2(silu(a1)) + vec1(LN(vec)), a1 = t0(sinus)
+    up_t = n_t0w or n_t0b or n_t2w or n_t2b
+    up_v = nvec or n_lnw or n_lnb or n_vw or n_vb
+    dt0 = dt0.to(_F32).contiguous()
+    dtemb = dtemb.to(_F32).contiguous()
+    grads[4 + 8], grads[4 + 9], dtemb = _linear_small_bwd(temb, 1, a_wf, dt0, n_aw, n_ab, up_t or up_v, dx_in=dtemb)
+    if up_t:
+        grads[4 + 2], grads[4 + 3], da1 = _linear_small_bwd(a1, 1, t2_wf, dtemb, n_t2w, n_t2b, n_t0w or n_t0b)
+        if n_t0w or n_t0b:
+            grads[4 + 0], grads[4 + 1], _ = _linear_small_bwd(sinus, 0, t0_wf, da1, n_t0w, n_t0b, False)
+    if up_v:
+        grads[4 + 6], grads[4 + 7], dvln = _linear_small_bwd(vln, 0, v_wf, dtemb, n_vw, n_vb, nvec or n_lnw or n_lnb)
+        if nvec or n_lnw or n_lnb:
+            Dc = vf.shape[1]
+            dvec = torch.empty_like(vf) if nvec else None
+            dw = torch.empty(Dc, dtype=_F32, device=dev) if n_lnw else None
+            db = torch.empty(Dc, dtype=_F32, device=dev) if n_lnb else None
+            _lib.check(L.ga_dit_layernorm_rows_bwd(ptr(vf), ptr(ln_wf), ptr(dvln), ptr(dvec), ptr(dw), ptr(db), B, Dc,
+                                                   1e-5, st), "ga_dit_layernorm_rows_bwd")
+            grads[4 + 4], grads[4 + 5] = dw, db
+            if nvec:
+                grads[1] = dvec.view(v_shape).to(v_dtype)
+    for i, p in enumerate(params):
+        g = grads[4 + i]
+        if g is not None:
+            grads[4 + i] = g.view(p.shape).to(p.dtype)
+    return tuple(grads)
+
+
+def _head_forward(xres, temb, params, N, keep):
+    table, W, b = params
+    R, D = xres.shape
+    B, Cout = temb.shape[0], W.shape[0]
+    dev = xres.device
+    L, st = _lib.lib(), stream(dev)
+    tf, Wf, bf = _f32(table), _f32(W), _f32(b)
+    tembf = temb.detach().to(_F32).contiguous()
+    modf = torch.empty((B, 2 * D), dtype=_F32, device=dev)
+    _lib.check(L.ga_add_tables(ptr(tf), ptr(tembf), ptr(modf), 1, B, 2 * D, D, st), "ga_add_tables")
+    y = torch.empty((R, Cout), dtype=_F32, device=dev)
+    _lib.check(L.ga_final_layer(ptr(xres), ptr(modf), ptr(Wf), ptr(bf), ptr(y), R, D, Cout, N, 1e-6, st),
+               "ga_final_layer")
+    return y, ((xres, modf, Wf) if keep else None)
+
+
+class _DiTHead(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, xres, temb, *params):
+        B, N, D = xres.shape
+        xf = xres.detach().to(_F32).contiguous().view(B * N, D)
+        with torch.cuda.device(xres.device):
+            y, saved = _head_forward(xf, temb, params, N, keep=True)
+        ctx.save_for_backward(*saved, *params)
+        ctx.meta = (xres.shape, xres.dtype, temb.dtype)
+        return y.view(B, N, -1)
+
+    @staticmethod
+    def backward(ctx, gy):
+        if torch.is_grad_enabled():
+            raise RuntimeError("dit_grad: double backward (create_graph=True) is not supported")
+        with torch.cuda.device(gy.device):
+            return _head_backward(ctx, gy)
+
+
+def _head_backward(ctx, gy):
+    xf, modf, Wf, table, W, b = ctx.saved_tensors
+    (B, N, D), x_dtype, t_dtype = ctx.meta
+    nx, nt, n_tab, n_w, n_b = ctx.needs_input_grad
+    R, Cout = B * N, W.shape[0]
+    dev = xf.device
+    L, st = _lib.lib(), stream(dev)
+    P = L.ga_dit_grad_partials(R, N)
+    dy = gy.reshape(R, Cout).to(_F32).contiguous()
+    dx = torch.empty((R, D), dtype=_F32, device=dev) if nx else None
+    pmod = torch.empty((P, 2 * D), dtype=_F32, device=dev) if (nt or n_tab) else None
+    pw = torch.empty((P, Cout * D), dtype=_F32, device=dev) if (n_w or n_b) else None
+    pb = torch.empty((P, Cout), dtype=_F32, device=dev) if (n_w or n_b) else None
+    _lib.check(L.ga_dit_final_layer_bwd(ptr(xf), ptr(modf), ptr(Wf), ptr(dy), ptr(dx), ptr(pmod), ptr(pw), ptr(pb), N,
+                                        R, D, Cout, 1e-6, st), "ga_dit_final_layer_bwd")
+    grads = [None] * 5
+    if nx:
+        grads[0] = dx.view(B, N, D).to(x_dtype)
+    if nt or n_tab:
+        dmod = _reduce(pmod, B, 2 * D)                                   # [B, 2 D]: d shift | d scale
+        if nt:
+            grads[1] = _reduce(dmod, B, D).to(t_dtype)                   # mod = table + temb: dtemb = dshift + dscale
+        if n_tab:
+            grads[2] = _reduce(dmod, 1, 2 * D).view(table.shape).to(table.dtype)
+    if n_w:
+        grads[3] = _reduce(pw, 1, Cout * D).view(W.shape).to(W.dtype)
+    if n_b:
+        grads[4] = _reduce(pb, 1, Cout)[0].to(b.dtype)
+    return tuple(grads)
+
+
+def _check_model(model, x, timesteps, context):
+    from .dit import DiT_I23D_PCD_PixelArt_noclip, ImageCondDiTBlockPixelArtRMSNormClayLRM
+    what = type(model).__name__
+    if not isinstance(model, DiT_I23D_PCD_PixelArt_noclip):
+        raise TypeError("model_forward: %s is not an image-to-3D point DiT" % what)
+    if not all(type(b) is ImageCondDiTBlockPixelArtRMSNormClayLRM for b in model.blocks):
+        raise NotImplementedError("model_forward: %s has other blocks than ImageCondDiTBlockPixelArtRMSNormClayLRM "
+                                  "(the text-to-3D DiT is not trainable here)" % what)
+    if model.enable_rope or model.freqs_cis is not None:
+        raise NotImplementedError("%s: RoPE is not supported" % what)
+    D, heads = model.embed_dim, model.num_heads
+    if D % heads or D // heads != 64:
+        raise NotImplementedError("%s: head_dim %s is not supported (64 only)" % (what, D / heads))
+    Cout, Dc = model.out_channels, model.pooled_vec_embedder[0].weight.shape[0]
+    if Cout > 16:
+        raise NotImplementedError("%s: out_channels %d > 16 (the final layer's limit)" % (what, Cout))
+    if D > 1024 or D % 8 or Dc > 1024 or Dc % 8:
+        raise NotImplementedError("%s: hidden size %d or pooled width %d is not a multiple of 8 up to 1024"
+                                  % (what, D, Dc))
+    if not isinstance(context, dict) or "img_crossattn" not in context or "img_vector" not in context:
+        raise ValueError("%s: context must be a dict with img_crossattn and img_vector" % what)
+    ctx, vec = context["img_crossattn"], context["img_vector"]
+    xyz = context.get("fps-xyz") if model.xyz_cond else None
+    if model.xyz_cond and xyz is None:
+        raise ValueError("%s: the stage-2 model needs context['fps-xyz']" % what)
+    for name, v in (("x", x), ("timesteps", timesteps), ("img_vector", vec), ("fps-xyz", xyz)):
+        if v is None and name == "fps-xyz":
+            continue
+        if not isinstance(v, torch.Tensor):
+            raise TypeError("%s: %s must be a tensor" % (what, name))
+        if v.dtype not in (torch.float32, torch.bfloat16, torch.float16):
+            raise TypeError("%s: %s must be fp32, bf16 or fp16, got %s" % (what, name, v.dtype))
+    for name, v in (("timesteps", timesteps), ("context['fps-xyz']", xyz)):
+        if v is not None and v.requires_grad:
+            raise ValueError("%s: %s is a constant of the model and gets no gradient; pass it detached" % (what, name))
+    if x.dim() != 3 or x.shape[2] != model.in_channels or x.shape[0] < 1 or x.shape[1] < 1:
+        raise ValueError("%s: x must be [B, N, %d], got %s" % (what, model.in_channels, tuple(x.shape)))
+    B, N = x.shape[:2]
+    K = model.in_channels + (3 if model.xyz_cond and not model.use_pe_cond else 0)
+    if K > 16:
+        raise NotImplementedError("%s: the token embedder's %d inputs > 16" % (what, K))
+    if timesteps.numel() not in (1, B):
+        raise ValueError("%s: timesteps must hold 1 or B = %d values, got %s" % (what, B, tuple(timesteps.shape)))
+    if vec.numel() != B * Dc:
+        raise ValueError("%s: img_vector must be [%d, %d], got %s" % (what, B, Dc, tuple(vec.shape)))
+    if xyz is not None and xyz.numel() != B * N * 3:
+        raise ValueError("%s: fps-xyz must be [%d, %d, 3], got %s" % (what, B, N, tuple(xyz.shape)))
+    stem, head = stem_parameters(model), head_parameters(model)
+    tensors = (x, timesteps, ctx, vec) + ((xyz,) if xyz is not None else ()) + stem + head
+    if not all(v.is_cuda for v in tensors):
+        raise RuntimeError("%s needs CUDA tensors (there is no CPU fallback)" % what)
+    if any(v.device != x.device for v in tensors):
+        raise ValueError("%s: inputs and parameters are on different devices" % what)
+    return ctx, vec, xyz, stem, head
+
+
+def model_forward(model, x, timesteps=None, context=None):
+    """DiT_I23D_PCD_PixelArt_noclip(_clay_stage2).forward with a backward: x [B, N, in_channels], timesteps [B] (or
+    one value), context {img_crossattn [B, M, Dc], img_vector [B, Dc], fps-xyz [B, N, 3] for stage 2}.  Returns y
+    [B, N, out_channels] fp32.  Gradients reach x, img_crossattn, img_vector and every parameter the forward reads;
+    timesteps and fps-xyz are constants.  functools.partial(model_forward, model) is a model for
+    Transport.training_losses.  The model's inference engine (model(...)) is not touched."""
+    ctx, vec, xyz, stem, head = _check_model(model, x, timesteps, context)
+    B, N = x.shape[:2]
+    grad = torch.is_grad_enabled()
+    with torch.cuda.device(x.device):
+        if grad and any(v.requires_grad for v in (x, vec) + stem):
+            xres, t0, temb = _DiTStem.apply(x, vec, timesteps, xyz, *stem)
+        else:
+            xres, t0, temb, _ = _stem_forward(x, vec, timesteps, xyz, stem, keep=False)
+            xres = xres.view(B, N, -1)
+        h = xres
+        for blk in model.blocks:
+            h = block_forward(blk, h, t0, ctx)
+        if grad and any(v.requires_grad for v in (h, temb) + head):
+            return _DiTHead.apply(h, temb, *head)
+        y, _ = _head_forward(h.detach().to(_F32).contiguous().view(B * N, -1), temb, head, N, keep=False)
+        return y.view(B, N, -1)

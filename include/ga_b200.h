@@ -949,6 +949,73 @@ int ga_dit_grad_reduce_validate(const float *part, const float *out, int groups,
 /* out [groups, cols] = sum over p = 0, 1, ..., parts - 1 (in that order, fp32) of part [groups, parts, cols]. */
 int ga_dit_grad_reduce(const float *part, float *out, int groups, int parts, int cols, void *stream);
 
+/*
+ * ---------------------------------------------------------------------------
+ * Part 15: the backwards of the image-to-3D DiT outside its blocks (DiT_I23D_PCD_PixelArt_noclip and its stage-2
+ * model, gaussiananything_b200/dit_grad.py model_forward; csrc/dit_model_grad.cu).  The forward runs on the Part 2
+ * launches the inference engine uses:
+ *   stem     sinus = timestep_embedding(t, 256); a1 = sinus W0^T + b0; temb = silu(a1) W2^T + b2
+ *            + (LayerNorm(vec) Wv^T + bv); t0 = silu(temb) Wa^T + ba [B, 6 D]            (fp32, ga_linear_small)
+ *   tokens   e1 = bf16(gelu_tanh([xyz | x] W1^T + b1)); xres = e1 Wf2^T + bf2 (+ bf16(posenc(xyz)) Wxyz^T + bxyz)
+ *   head     y = (LN(xres) (1 + scale[b]) + shift[b]) Wf^T + bf,  [shift | scale] = table + temb  (eps 1e-6)
+ * Its backward: fc2's and the xyz projection's dW and db and fc2's dgrad are Part 13 GEMMs on bf16(dxres); the
+ * kernels below do the rest in fp32.  As in Part 14 nothing uses atomics: sums over the R token rows are written as
+ * one partial per chunk of 32 rows of one batch item (ga_dit_grad_partials(R, rows_per_batch) of them), rows added in
+ * a stated order, and ga_dit_grad_reduce adds the partials in index order; sums over the B stem rows are taken in
+ * row order.  The same inputs give the same bits on any H100.  Every entry point checks its arguments with its
+ * host-only *_validate first (0, or GA_ERR_BADARG).
+ * Test bounds (tests/dit_model_grad_ref.py): the GPU gradients are held to 1.5 times a bf16-emulating fp64
+ * reference's distance from fp64.  Timings: profiles/dit_train_h100.md.
+ * ---------------------------------------------------------------------------
+ */
+/* Host only: R a positive multiple of rows_per_batch; 4 <= D <= 1024, D % 4 == 0; 1 <= Cout <= 16; R D < 2^31;
+ * x, mod, W non-NULL; dy non-NULL; part_dw and part_db both NULL or both given; x, mod, W, dx, part_dmod, part_dw
+ * 16-byte aligned, dy and part_db 4-byte aligned. */
+int ga_dit_final_layer_bwd_validate(const float *x, const float *mod, const float *W, const float *dy,
+                                    const float *dx, const float *part_dmod, const float *part_dw,
+                                    const float *part_db, int rows_per_batch, int R, int D, int Cout);
+/* Final-layer backward: x fp32 [R, D] (the residual stream), mod [B, 2 D] = [shift | scale], W [Cout, D], dy
+ * [R, Cout].  With n = LN(x) recomputed and dh = dy W: dx [R, D] = rstd (dn - mean(dn) - n mean(dn n)),
+ * dn = dh (1 + scale[b]) (NULL: not formed); part_dmod [P, 2 D] = the chunk sums of [dh | dh n] (NULL: not formed);
+ * part_dw [P, Cout, D] and part_db [P, Cout] = the chunk sums of dy h and dy, h = n (1 + scale[b]) + shift[b], rows
+ * in increasing order.  P = ga_dit_grad_partials(R, rows_per_batch). */
+int ga_dit_final_layer_bwd(const float *x, const float *mod, const float *W, const float *dy, float *dx,
+                           float *part_dmod, float *part_dw, float *part_db, int rows_per_batch, int R, int D,
+                           int Cout, float eps, void *stream);
+/* Host only: R >= 1; 1 <= D <= 1024; Cx >= 1, C2 >= 0, Cx + C2 <= 16; R D < 2^31; xin2 given iff C2 > 0; xin, W1,
+ * b1, de1, part_dw1, part_db1 non-NULL; every pointer 4-byte aligned. */
+int ga_dit_embed_fc1_bwd_validate(const float *xin, int Cx, const float *xin2, int C2, const float *W1,
+                                  const float *b1, const float *de1, const float *part_dw1, const float *part_db1,
+                                  const float *dxin, int R, int D);
+/* Token-embedder fc1 backward (ga_embed_fc1's layer, K = C2 + Cx inputs [xin2 | xin]): v recomputed in fp32, dv =
+ * de1 gelu_tanh'(v) with de1 fp32 [R, D]; part_dw1 [P, D, K] and part_db1 [P, D] the chunk sums of dv [xin2 | xin]
+ * and dv over rows in increasing order (P = ga_dit_grad_partials(R, R)); dxin [R, Cx] = dv W1[:, C2:] (NULL: not
+ * formed; the xin2 columns get no gradient). */
+int ga_dit_embed_fc1_bwd(const float *xin, int Cx, const float *xin2, int C2, const float *W1, const float *b1,
+                         const float *de1, float *part_dw1, float *part_db1, float *dxin, int R, int D, void *stream);
+/* Host only: rows, N >= 1; K >= 4, K % 4 == 0; act_in 0 or 1; N K < 2^31 and P rows K < 2^31; x, W non-NULL and
+ * 16-byte aligned; dy non-NULL; dW 16-byte aligned; dx given: part non-NULL and 16-byte aligned; dx NULL: part and
+ * dx_in NULL; dy, db, dx, dx_in 4-byte aligned. */
+int ga_dit_linear_small_bwd_validate(const float *x, int act_in, const float *W, const float *dy, const float *dW,
+                                     const float *db, const float *part, const float *dx_in, const float *dx,
+                                     int rows, int N, int K);
+/* Backward of ga_linear_small's y = act(x) W^T + b for any number of rows: x [rows, K], W [N, K], dy [rows, N], act
+ * SiLU when act_in.  dW [N, K] = sum over b = 0, 1, ... of dy[b]^T act(x[b]); db [N] likewise; dx [rows, K] = dx_in +
+ * act'(x) (dy W) (dx_in NULL: 0; dx_in may be dx), dy W summed over chunks of 32 rows of W (P =
+ * ga_dit_grad_partials(N, N) partials [P, rows, K] in part, rows of a chunk in increasing order) then over the
+ * chunks in order.  Any output may be NULL.  Byte floor: W read once and dW written once, 8 N K bytes, plus 8 P rows K
+ * bytes of partials when dx is formed. */
+int ga_dit_linear_small_bwd(const float *x, int act_in, const float *W, const float *dy, float *dW, float *db,
+                            float *part, const float *dx_in, float *dx, int rows, int N, int K, void *stream);
+/* Host only: R >= 1; 4 <= D <= 1024, D % 4 == 0; R D < 2^31; x, w, dy non-NULL; every pointer 16-byte aligned. */
+int ga_dit_layernorm_rows_bwd_validate(const float *x, const float *w, const float *dy, const float *dx,
+                                       const float *dw, const float *db, int R, int D);
+/* Backward of ga_layernorm_rows with affine w (the pooled vector's LayerNorm): n = (x - mean) rstd, dn = dy w;
+ * dx [R, D] = rstd (dn - mean(dn) - n mean(dn n)); dw = sum_r dy n, db = sum_r dy, rows in increasing order (one
+ * CTA).  Any output may be NULL. */
+int ga_dit_layernorm_rows_bwd(const float *x, const float *w, const float *dy, float *dx, float *dw, float *db,
+                              int R, int D, float eps, void *stream);
+
 /* Measurement aid: when enabled, cudaEvents are recorded around every kernel
  * stage of the next forward/backward; ga_profile_read synchronises on them and
  * returns per-stage milliseconds: [0] preprocess, [1] binning, [2] render fwd,
