@@ -22,6 +22,7 @@ import sys
 import torch
 
 from . import _lib
+from ._launch import ptr, stream
 
 __all__ = ["memory_efficient_attention", "install_shims"]
 
@@ -52,10 +53,6 @@ def _stride_table(tensors):
     for t in tensors:
         vals += _strides(t) if t is not None else [0, 0, 0]
     return (C.c_int64 * 24)(*vals)
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr() if t is not None else None)
 
 
 def _check_args(query, key, value, attn_bias, p):
@@ -135,13 +132,26 @@ def _forward(qp, kp, vp, scale):
     dev = qp.device
     o = torch.empty((B, Nq, H, Dv), dtype=_BF16, device=dev)
     lse = torch.empty((B * H, Nq), dtype=torch.float32, device=dev)
-    L = _lib.lib()
     with torch.cuda.device(dev):
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(L.ga_attention_fwd_lse_bf16(_ptr(qp), _ptr(kp), _ptr(vp), _ptr(o), _ptr(lse), B, H, Nq, Nk, D, Dv,
-                                               _stride_table((qp, kp, vp, o)), float(scale), C.c_void_p(stream)),
+        _lib.check(_lib.lib().ga_attention_fwd_lse_bf16(ptr(qp), ptr(kp), ptr(vp), ptr(o), ptr(lse), B, H, Nq, Nk, D,
+                                                        Dv, _stride_table((qp, kp, vp, o)), float(scale), stream(dev)),
                    "ga_attention_fwd_lse_bf16")
     return o, lse
+
+
+def _backward(qp, kp, vp, o, lse, g, dq, dk, dv, scale):
+    """Writes the gradients dq, dk, dv (each may be None) of prepared [B, N, H, d] tensors, given _forward's o and lse
+    and the output gradient g, into those [B, N, H, d] buffers."""
+    B, Nq, H, D = qp.shape
+    Nk, Dv = kp.shape[1], vp.shape[3]
+    dev = qp.device
+    delta = torch.empty((B * H, Nq), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().ga_attention_bwd_bf16(ptr(qp), ptr(kp), ptr(vp), ptr(o), ptr(lse), ptr(g), ptr(delta),
+                                                    ptr(dq), ptr(dk), ptr(dv), B, H, Nq, Nk, D, Dv,
+                                                    _stride_table((qp, kp, vp, o, g, dq, dk, dv)), float(scale),
+                                                    stream(dev)),
+                   "ga_attention_bwd_bf16")
 
 
 class _MemEffAttention(torch.autograd.Function):
@@ -164,23 +174,13 @@ class _MemEffAttention(torch.autograd.Function):
             raise RuntimeError("memory_efficient_attention: double backward (create_graph=True) is not supported")
         qp, kp, vp, o, lse = ctx.saved_tensors
         need_q, need_k, need_v = ctx.needs_input_grad[:3]
-        B, Nq, H, D = qp.shape
-        Nk, Dv = kp.shape[1], vp.shape[3]
         g = grad_out.unsqueeze(2) if grad_out.dim() == 3 else grad_out
         g = _prepare(g)
         # the gradients are written with the strides of the tensors the kernels read (the inputs' own when bf16)
         dq = _grad_buffer(qp) if need_q else None
         dk = _grad_buffer(kp) if need_k else None
         dv = _grad_buffer(vp) if need_v else None
-        delta = torch.empty((B * H, Nq), dtype=torch.float32, device=qp.device)
-        L = _lib.lib()
-        with torch.cuda.device(qp.device):
-            stream = torch.cuda.current_stream(qp.device).cuda_stream
-            _lib.check(L.ga_attention_bwd_bf16(_ptr(qp), _ptr(kp), _ptr(vp), _ptr(o), _ptr(lse), _ptr(g), _ptr(delta),
-                                               _ptr(dq), _ptr(dk), _ptr(dv), B, H, Nq, Nk, D, Dv,
-                                               _stride_table((qp, kp, vp, o, g, dq, dk, dv)), ctx.scale,
-                                               C.c_void_p(stream)),
-                       "ga_attention_bwd_bf16")
+        _backward(qp, kp, vp, o, lse, g, dq, dk, dv, ctx.scale)
         oq, ok, ov = ctx.orig
         return (_grad_like(dq, oq) if need_q else None, _grad_like(dk, ok) if need_k else None,
                 _grad_like(dv, ov) if need_v else None, None)

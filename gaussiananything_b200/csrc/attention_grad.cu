@@ -22,8 +22,10 @@
 // (sequence, head) on CUDA cores, bf16 operands staged in shared memory, everything else fp32.
 #include "../../include/ga_b200.h"
 #include "device_once.cuh"
+#include "row_common.cuh"
 #include "sm90_ptx.cuh"
 
+using namespace ga_row;
 using namespace sm90;
 
 namespace {
@@ -68,30 +70,6 @@ __device__ __forceinline__ long long head_off(long long bh, int heads, long long
     return b * sb + (bh - b * heads) * sh;
 }
 
-__device__ __forceinline__ void cpa16(uint32_t dst, const void *src, bool valid)
-{
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
-}
-__device__ __forceinline__ void cpa_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
-template <int N> __device__ __forceinline__ void cpa_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
-
-__device__ __forceinline__ uint32_t pack_bf16(float a, float b)
-{
-    __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<uint32_t *>(&h);
-}
-
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
-
-__device__ __forceinline__ uint8_t *align1024(uint8_t *p)
-{
-    return reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(p) + 1023) & ~uintptr_t(1023));
-}
-
-// byte offset of 16-byte piece `chunk` of row `row` in a 64 x 64 tile with 128-byte swizzle (the K-major layout
-// wgmma_desc_k_sw128 describes)
-__device__ __forceinline__ uint32_t sw_off(int row, int chunk) { return row * 128 + ((chunk ^ (row & 7)) << 4); }
-
 // rows [n0, n0 + 64) x columns [0, 64) of one head into a swizzled tile; rows >= N and columns >= d are zeros
 __device__ __forceinline__ void load_tile(uint8_t *s, const Tens &t, long long base, int n0, int N, int d)
 {
@@ -99,7 +77,7 @@ __device__ __forceinline__ void load_tile(uint8_t *s, const Tens &t, long long b
     for (int i = 0; i < 4; i++) {
         const int idx = threadIdx.x + kThreads * i, row = idx >> 3, ch = idx & 7;
         const bool ok = n0 + row < N && ch * 8 < d;
-        cpa16(smem_u32(s) + sw_off(row, ch), ok ? t.p + base + (long long)(n0 + row) * t.sn + ch * 8 : t.p, ok);
+        cp_async16(smem_u32(s) + sw128_off(row, ch), ok ? t.p + base + (long long)(n0 + row) * t.sn + ch * 8 : t.p, ok);
     }
 }
 
@@ -111,12 +89,12 @@ __device__ __forceinline__ void transpose_tile(uint8_t *dst, const uint8_t *src)
 #pragma unroll
     for (int i = 0; i < 2; i++) {
         const int idx = threadIdx.x + kThreads * i, r0 = 2 * (idx & 31), ch = idx >> 5;
-        const uint4 va = *reinterpret_cast<const uint4 *>(src + sw_off(r0, ch));
-        const uint4 vb = *reinterpret_cast<const uint4 *>(src + sw_off(r0 + 1, ch));
+        const uint4 va = *reinterpret_cast<const uint4 *>(src + sw128_off(r0, ch));
+        const uint4 vb = *reinterpret_cast<const uint4 *>(src + sw128_off(r0 + 1, ch));
         const uint16_t *ea = reinterpret_cast<const uint16_t *>(&va), *eb = reinterpret_cast<const uint16_t *>(&vb);
 #pragma unroll
         for (int e = 0; e < 8; e++)
-            *reinterpret_cast<uint32_t *>(dst + sw_off(8 * ch + e, r0 >> 3) + (r0 & 7) * 2) =
+            *reinterpret_cast<uint32_t *>(dst + sw128_off(8 * ch + e, r0 >> 3) + (r0 & 7) * 2) =
                 (uint32_t)ea[e] | ((uint32_t)eb[e] << 16);
     }
 }
@@ -189,14 +167,14 @@ __device__ __forceinline__ void store_rows(const OutTens &t, long long base, int
 // every thread
 __device__ __forceinline__ void tiles_ready()
 {
-    cpa_wait<1>();
-    fence_async_smem();
+    cp_async_wait<1>();
+    fence_proxy_async();
     __syncthreads();
 }
 // shared-memory stores (the transposed tiles) made visible to wgmma and to every thread
 __device__ __forceinline__ void stores_ready()
 {
-    fence_async_smem();
+    fence_proxy_async();
     __syncthreads();
 }
 
@@ -214,7 +192,7 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_lse_kernel(const AttnArgs a
     load_tile(sQ, a.q, bq, q0, a.Nq, a.dqk);
     load_tile(sK, a.k, bk, 0, a.Nk, a.dqk);
     load_tile(sV, a.v, bv, 0, a.Nk, a.dvv);
-    cpa_commit();
+    cp_async_commit();
 
     float o[32];
     zero(o);
@@ -225,7 +203,7 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_lse_kernel(const AttnArgs a
             load_tile(sK + st * TB, a.k, bk, (j + 1) * BC, a.Nk, a.dqk);
             load_tile(sV + st * TB, a.v, bv, (j + 1) * BC, a.Nk, a.dvv);
         }
-        cpa_commit();
+        cp_async_commit();
         tiles_ready();
         transpose_tile(sVt, sV + (j & 1) * TB);
         stores_ready();
@@ -275,7 +253,7 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_lse_kernel(const AttnArgs a
         keep_live(pa);
         __syncthreads();
     }
-    cpa_wait<0>();
+    cp_async_wait<0>();
 
     float inv[2];
 #pragma unroll
@@ -348,7 +326,7 @@ __global__ void __launch_bounds__(kThreads) attn_dkdv_kernel(const AttnArgs a)
     if (kDK) load_tile(sV, a.v, bv, k0, a.Nk, a.dvv);
     load_tile(sQ, a.q, bq, 0, a.Nq, a.dqk);
     load_tile(sG, a.dout, bg, 0, a.Nq, a.dvv);
-    cpa_commit();
+    cp_async_commit();
     load_rowstats(sL, sD, a, bh, 0, kDK);
 
     float dk[32], dv[32];
@@ -360,7 +338,7 @@ __global__ void __launch_bounds__(kThreads) attn_dkdv_kernel(const AttnArgs a)
             load_tile(sQ + st * TB, a.q, bq, (i + 1) * BC, a.Nq, a.dqk);
             load_tile(sG + st * TB, a.dout, bg, (i + 1) * BC, a.Nq, a.dvv);
         }
-        cpa_commit();
+        cp_async_commit();
         tiles_ready();
         if (i + 1 < a.nqb) load_rowstats(sL + ((i + 1) & 1) * BC, sD + ((i + 1) & 1) * BC, a, bh, (i + 1) * BC, kDK);
         const uint8_t *q_t = sQ + (i & 1) * TB, *g_t = sG + (i & 1) * TB;
@@ -405,7 +383,7 @@ __global__ void __launch_bounds__(kThreads) attn_dkdv_kernel(const AttnArgs a)
         if (kDK) keep_live(da);
         __syncthreads();
     }
-    cpa_wait<0>();
+    cp_async_wait<0>();
     if (kDK && a.dk.p)
         store_rows(a.dk, head_off(bh, a.heads, a.dk.sb, a.dk.sh), k0 + 16 * warp, a.Nk, a.dqk, dk, a.scale);
     if (a.dv.p) store_rows(a.dv, head_off(bh, a.heads, a.dv.sb, a.dv.sh), k0 + 16 * warp, a.Nk, a.dvv, dv, 1.f);
@@ -426,7 +404,7 @@ __global__ void __launch_bounds__(kThreads) attn_dq_kernel(const AttnArgs a)
     load_tile(sG, a.dout, bg, q0, a.Nq, a.dvv);
     load_tile(sK, a.k, bk, 0, a.Nk, a.dqk);
     load_tile(sV, a.v, bv, 0, a.Nk, a.dvv);
-    cpa_commit();
+    cp_async_commit();
 
     float lse[2], dlt[2];
 #pragma unroll
@@ -443,7 +421,7 @@ __global__ void __launch_bounds__(kThreads) attn_dq_kernel(const AttnArgs a)
             load_tile(sK + st * TB, a.k, bk, (j + 1) * BC, a.Nk, a.dqk);
             load_tile(sV + st * TB, a.v, bv, (j + 1) * BC, a.Nk, a.dvv);
         }
-        cpa_commit();
+        cp_async_commit();
         tiles_ready();
         const uint8_t *k_t = sK + (j & 1) * TB, *v_t = sV + (j & 1) * TB;
         transpose_tile(sKt, k_t);
@@ -476,7 +454,7 @@ __global__ void __launch_bounds__(kThreads) attn_dq_kernel(const AttnArgs a)
         keep_live(da);
         __syncthreads();
     }
-    cpa_wait<0>();
+    cp_async_wait<0>();
     store_rows(a.dq, head_off(bh, a.heads, a.dq.sb, a.dq.sh), q0 + 16 * warp, a.Nq, a.dqk, dq, a.scale);
 }
 

@@ -58,15 +58,6 @@ struct ConvArgs {
 constexpr int kEpiNone = 0, kEpiRelu = 1, kEpiMask = 2, kEpiLrelu = 3, kEpiLreluGrad = 4, kEpiStats = 5,
               kEpiBnGrad = 6;
 
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid)
-{
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
-template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
-// cp.async writes through the generic proxy, wgmma reads through the async proxy
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
-
 // Per-channel sums over the CTA's 128 rows of two values per fragment element: lanes of equal l % 4 by an xor
 // butterfly (16 rows per warp), then the eight warps in order.  red: 8 * BN float2 of shared memory.  Thread t < BN
 // gets column t's sums.  Every thread of the CTA calls it.
@@ -105,7 +96,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const ConvA
 {
     using Cfg = ConvCfg<BN>;
     extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t *smem = align1024(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int wg = warp >> 2, wi = warp & 3;
     const int m0 = blockIdx.x * CBM, n0 = blockIdx.y * BN;
@@ -142,6 +133,8 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const ConvA
             const int tap = kin ? k / a.Cin : 0;
             const int c = k - tap * a.Cin;
             const int ky = tap / KS, kx = tap - ky * KS;
+            // sw128_off(r, chunk) written out so that sa + r * 128 is added first: calling it reorders the additions
+            // and changes these kernels' register allocation
 #pragma unroll
             for (int i = 0; i < 4; i++) {
                 const int r = (tid >> 3) + 32 * i;

@@ -17,8 +17,10 @@
 //   warp 8    : TMA producer (Q once, K and V double buffered).
 #include "../../include/ga_b200.h"
 #include "device_once.cuh"
+#include "row_common.cuh"
 #include "sm90_ptx.cuh"
 
+using namespace ga_row;
 using namespace sm90;
 
 int ga_make_tmap_bf16(CUtensorMap *map, const void *ptr, uint64_t rows, uint64_t cols, uint64_t ld_elems,
@@ -34,11 +36,6 @@ constexpr int kSmemAttn = kQBytes + 2 * kKBytes + 2 * kVBytes + 1024;
 constexpr int kConsumerWarps = 8;
 constexpr int kAttnThreads = 32 * kConsumerWarps + 32;
 
-__device__ __forceinline__ uint32_t pack2(float a, float b)
-{
-    __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<uint32_t *>(&h);
-}
 __device__ __forceinline__ float ex2_fast(float x)
 {
     float r;
@@ -67,7 +64,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant
 {
     extern __shared__ uint8_t smem_raw[];
     __shared__ uint64_t q_full, k_full[2], k_empty[2], v_full[2], v_empty[2];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t *smem = align1024(smem_raw);
     uint8_t *sQ = smem;
     uint8_t *sK = sQ + kQBytes;
     uint8_t *sV = sK + 2 * kKBytes;
@@ -185,7 +182,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant
             const float p0 = ex2_fast(fmaf(s_acc[i], scale_log2, -m_use[hf]));
             const float p1 = ex2_fast(fmaf(s_acc[i + 1], scale_log2, -m_use[hf]));
             l_run[hf] += p0 + p1;
-            pa[i >> 3][(i >> 1) & 3] = pack2(p0, p1);
+            pa[i >> 3][(i >> 1) & 3] = pack_bf16(p0, p1);
         }
         // O += P V_j, then (under the same wait) S = Q K_{j+1}^T
         const int sv = j & 1;
@@ -223,7 +220,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant
             __nv_bfloat16 *dst = out + ((size_t)b * Nq + q) * (size_t)(heads * HD) + h * HD + 2 * c;
 #pragma unroll
             for (int jj = 0; jj < HD / 8; jj++)
-                *reinterpret_cast<uint32_t *>(dst + 8 * jj) = pack2(o_acc[4 * jj + 2 * hf] * inv, o_acc[4 * jj + 2 * hf + 1] * inv);
+                *reinterpret_cast<uint32_t *>(dst + 8 * jj) = pack_bf16(o_acc[4 * jj + 2 * hf] * inv, o_acc[4 * jj + 2 * hf + 1] * inv);
         }
     }
 }

@@ -13,8 +13,10 @@
 // ring for the next tile while the consumers run the epilogue of this one.
 #include "../../include/ga_b200.h"
 #include "device_once.cuh"
+#include "row_common.cuh"
 #include "sm90_ptx.cuh"
 
+using namespace ga_row;
 using namespace sm90;
 
 namespace {
@@ -48,12 +50,6 @@ __device__ __forceinline__ float gelu_erf(float v)
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(p));
     const float erf_abs = 1.0f - r;
     return 0.5f * v * (1.0f + copysignf(erf_abs, v));
-}
-
-__device__ __forceinline__ uint32_t pack_bf16(float a, float b)
-{
-    __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<uint32_t *>(&h);
 }
 
 // ---- epilogue ---------------------------------------------------------------
@@ -358,7 +354,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
     using Cfg = GemmCfg<BN>;
     extern __shared__ uint8_t smem_raw[];
     __shared__ uint64_t full_bar[Cfg::kStages], empty_bar[Cfg::kStages];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t *smem = align1024(smem_raw);
     uint8_t *smem_a = smem, *smem_b = smem + Cfg::kStages * Cfg::kABytes;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;

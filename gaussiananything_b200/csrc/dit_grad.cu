@@ -7,21 +7,11 @@
 // cross a batch item), adding within a chunk in a fixed order, and ga_dit_grad_reduce adds the partials in index
 // order.  The number of partials depends on the shapes alone.
 #include "../../include/ga_b200.h"
-#include <cuda_bf16.h>
-#include <cuda_runtime.h>
+#include "row_common.cuh"
+
+using namespace ga_row;
 
 namespace {
-
-constexpr int kChunkRows = 32;          // rows per partial
-constexpr int kWarps = 8;               // warps per CTA of the row kernels
-constexpr int kMaxD = 1024;             // widest row kept in registers (8 float4 per lane)
-
-__device__ __forceinline__ float warp_sum(float v)
-{
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 
 __device__ __forceinline__ float sum8(float v)       // over the 8 lanes of an aligned lane group
 {
@@ -29,56 +19,6 @@ __device__ __forceinline__ float sum8(float v)       // over the 8 lanes of an a
     v += __shfl_xor_sync(0xffffffffu, v, 2);
     v += __shfl_xor_sync(0xffffffffu, v, 4);
     return v;
-}
-
-__device__ __forceinline__ float4 ld4(const float *p, int i) { return __ldg(reinterpret_cast<const float4 *>(p) + i); }
-__device__ __forceinline__ float dot4(float4 a, float4 b) { return a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w; }
-__device__ __forceinline__ float4 mul4(float4 a, float4 b) { return make_float4(a.x * b.x, a.y * b.y, a.z * b.z, a.w * b.w); }
-__device__ __forceinline__ void add4(float4 &a, float4 b) { a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w; }
-
-__device__ __forceinline__ uint2 pack4(float4 v)
-{
-    __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
-    return make_uint2(*reinterpret_cast<uint32_t *>(&a), *reinterpret_cast<uint32_t *>(&b));
-}
-
-__device__ __forceinline__ void unpack8(uint4 u, float (&f)[8])
-{
-    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-        const float2 p = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&w[i]));
-        f[2 * i] = p.x;
-        f[2 * i + 1] = p.y;
-    }
-}
-
-__device__ __forceinline__ uint4 pack8(const float (&f)[8])
-{
-    uint32_t w[4];
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-        __nv_bfloat162 h = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
-        w[i] = *reinterpret_cast<uint32_t *>(&h);
-    }
-    return make_uint4(w[0], w[1], w[2], w[3]);
-}
-
-// The CTA's sum of acc (float4 index lane + 32 u of each warp), warps added in warp order, written to out[0, D).
-__device__ __forceinline__ void cta_colsum(float4 (*red)[kMaxD / 4], const float4 (&acc)[8], float *out, int n4)
-{
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-#pragma unroll
-    for (int u = 0; u < 8; u++)
-        if (lane + 32 * u < n4) red[warp][lane + 32 * u] = acc[u];
-    __syncthreads();
-    for (int i = threadIdx.x; i < n4; i += blockDim.x) {
-        float4 s = red[0][i];
-#pragma unroll
-        for (int w = 1; w < kWarps; w++) add4(s, red[w][i]);
-        reinterpret_cast<float4 *>(out)[i] = s;
-    }
-    __syncthreads();
 }
 
 // One CTA per chunk (b, c): rows b N + 32 c + i, i < 32, warp w taking i = w, w + 8, ... in increasing order.
@@ -334,21 +274,34 @@ qk_norm_bwd_kernel(const __nv_bfloat16 *__restrict__ in, int ld_in, const __nv_b
     }
 }
 
-// out[g, c] = sum over p in increasing order of part[g parts + p, c]
-__global__ void grad_reduce_kernel(const float *__restrict__ part, float *__restrict__ out, int groups, int parts,
-                                   int cols)
+// out[g, c] = part[g parts, c] + part[g parts + 1, c] + ... in increasing order (ga_launch_partial_sum), one thread
+// per output element; T is float or float4, four columns added one by one
+template <typename T>
+__global__ void partial_sum_kernel(const T *__restrict__ part, T *__restrict__ out, long long n, int parts,
+                                   long long cols)
 {
     const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-    if (i >= (long long)groups * cols) return;
-    const int g = (int)(i / cols), c = (int)(i - (long long)g * cols);
-    const float *src = part + (size_t)g * parts * cols + c;
-    float s = src[0];
-    for (int p = 1; p < parts; p++) s += src[(size_t)p * cols];
+    if (i >= n) return;
+    const long long g = i / cols, c = i - g * cols;
+    const T *src = part + g * parts * cols + c;
+    const auto add = [](T &a, const T &b) {
+        if constexpr (sizeof(T) == sizeof(float4)) add4(a, b);
+        else a += b;
+    };
+    T s = src[0];
+    int p = 1;
+    // sixteen loads in flight before their additions (which stay in order): with a few thousand columns the sum is
+    // bound by load latency
+    for (; p + 16 <= parts; p += 16) {
+        T v[16];
+#pragma unroll
+        for (int u = 0; u < 16; u++) v[u] = src[(p + u) * cols];
+#pragma unroll
+        for (int u = 0; u < 16; u++) add(s, v[u]);
+    }
+    for (; p < parts; p++) add(s, src[p * cols]);
     out[i] = s;
 }
-
-bool mis16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
-bool mis8(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 7) != 0; }
 
 bool bad_rows(int R, int rows_per_batch, int D)
 {
@@ -356,6 +309,22 @@ bool bad_rows(int R, int rows_per_batch, int D)
 }
 
 }  // namespace
+
+cudaError_t ga_launch_partial_sum(const float *part, float *out, long long groups, int parts, long long cols,
+                                  cudaStream_t s)
+{
+    // float4 only when a quarter of the columns still gives each of the H100's 132 SMs a CTA: narrower sums (the
+    // DiT partials, bias chunks) are latency-bound and run faster with one thread per column
+    const bool vec = cols % 4 == 0 && cols / 4 >= 132 * 256 && !mis16(part) && !mis16(out);
+    const long long w = vec ? cols / 4 : cols, n = groups * w;
+    const unsigned blocks = (unsigned)((n + 255) / 256);
+    if (vec)
+        partial_sum_kernel<<<blocks, 256, 0, s>>>(reinterpret_cast<const float4 *>(part), reinterpret_cast<float4 *>(out),
+                                                  n, parts, w);
+    else
+        partial_sum_kernel<<<blocks, 256, 0, s>>>(part, out, n, parts, w);
+    return cudaGetLastError();
+}
 
 extern "C" int ga_dit_grad_partials(int rows, int rows_per_batch)
 {
@@ -501,7 +470,5 @@ extern "C" int ga_dit_grad_reduce(const float *part, float *out, int groups, int
 {
     const int rc = ga_dit_grad_reduce_validate(part, out, groups, parts, cols);
     if (rc) return rc;
-    const long long n = (long long)groups * cols;
-    grad_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(part, out, groups, parts, cols);
-    return (int)cudaGetLastError();
+    return (int)ga_launch_partial_sum(part, out, groups, parts, cols, (cudaStream_t)stream);
 }

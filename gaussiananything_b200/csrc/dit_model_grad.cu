@@ -6,68 +6,14 @@
 // cross a batch item, ga_dit_grad_partials counts them), added within a chunk in a fixed order, and reduced by
 // ga_dit_grad_reduce in index order.  Sums over the B rows of the stem are taken in row order.
 #include "../../include/ga_b200.h"
-#include <cuda_bf16.h>
-#include <cuda_runtime.h>
+#include "row_common.cuh"
+
+using namespace ga_row;
 
 namespace {
 
-constexpr int kChunkRows = 32;          // rows per partial (ga_dit_grad_partials)
-constexpr int kWarps = 8;               // warps per CTA
-constexpr int kMaxD = 1024;             // widest row kept in registers (8 float4 per lane)
 constexpr int kMaxCout = 16;            // ga_final_layer's output width limit
 constexpr int kMaxK = 16;               // fc1's input width limit (x channels + xyz)
-
-__device__ __forceinline__ float warp_sum(float v)
-{
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
-__device__ __forceinline__ float4 ld4(const float *p, int i) { return __ldg(reinterpret_cast<const float4 *>(p) + i); }
-__device__ __forceinline__ float dot4(float4 a, float4 b) { return a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w; }
-__device__ __forceinline__ float sum4(float4 a) { return a.x + a.y + a.z + a.w; }
-__device__ __forceinline__ float4 mul4(float4 a, float4 b) { return make_float4(a.x * b.x, a.y * b.y, a.z * b.z, a.w * b.w); }
-__device__ __forceinline__ float4 scale4(float4 a, float s) { return make_float4(a.x * s, a.y * s, a.z * s, a.w * s); }
-__device__ __forceinline__ void add4(float4 &a, float4 b) { a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w; }
-__device__ __forceinline__ void fma4(float4 &a, float s, float4 b)
-{
-    a.x = fmaf(s, b.x, a.x); a.y = fmaf(s, b.y, a.y); a.z = fmaf(s, b.z, a.z); a.w = fmaf(s, b.w, a.w);
-}
-__device__ __forceinline__ float4 zero4() { return make_float4(0.f, 0.f, 0.f, 0.f); }
-
-__device__ __forceinline__ float silu(float x) { return x / (1.0f + __expf(-x)); }
-__device__ __forceinline__ float silu_grad(float x)
-{
-    const float s = 1.0f / (1.0f + __expf(-x));
-    return s * (1.0f + x * (1.0f - s));
-}
-__device__ __forceinline__ float4 silu4(float4 v) { return make_float4(silu(v.x), silu(v.y), silu(v.z), silu(v.w)); }
-
-// d/dv of 0.5 v (1 + tanh(k0 (v + k1 v^3))), ga_embed_fc1's activation
-__device__ __forceinline__ float gelu_tanh_grad(float v)
-{
-    const float k0 = 0.7978845608028654f, k1 = 0.044715f;
-    const float th = tanhf(k0 * (v + k1 * v * v * v));
-    return 0.5f * (1.0f + th) + 0.5f * v * (1.0f - th * th) * k0 * (1.0f + 3.0f * k1 * v * v);
-}
-
-// The CTA's sum of acc (float4 index lane + 32 u of each warp), warps added in warp order, written to out[0, D).
-__device__ __forceinline__ void cta_colsum(float4 (*red)[kMaxD / 4], const float4 (&acc)[8], float *out, int n4)
-{
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-#pragma unroll
-    for (int u = 0; u < 8; u++)
-        if (lane + 32 * u < n4) red[warp][lane + 32 * u] = acc[u];
-    __syncthreads();
-    for (int i = threadIdx.x; i < n4; i += blockDim.x) {
-        float4 s = red[0][i];
-#pragma unroll
-        for (int w = 1; w < kWarps; w++) add4(s, red[w][i]);
-        reinterpret_cast<float4 *>(out)[i] = s;
-    }
-    __syncthreads();
-}
 
 // ---- final layer ----------------------------------------------------------------------------------------------------
 // One CTA per chunk (b, c) of rows b N + 32 c + i.  Phase 1, warp w taking rows i = w, w + 8, ...: n = LN(x), dh =
@@ -393,7 +339,6 @@ layernorm_rows_bwd_kernel(const float *__restrict__ x, const float *__restrict__
     if (db) reinterpret_cast<float4 *>(db)[q] = ab;
 }
 
-bool mis16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
 bool mis4(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 3) != 0; }
 
 }  // namespace

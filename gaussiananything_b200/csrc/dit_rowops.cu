@@ -5,24 +5,12 @@
 // Math follows /root/reference/dit/dit_i23d.py:511-567,707-750,
 // /root/reference/dit/dit_models_xformers.py:62-128 and /root/reference/dit/norm.py.
 #include "../../include/ga_b200.h"
-#include <cuda_bf16.h>
-#include <cuda_runtime.h>
+#include "row_common.cuh"
 #include <cstdlib>
 
-namespace {
+using namespace ga_row;
 
-__device__ __forceinline__ float warp_sum(float v)
-{
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-__device__ __forceinline__ float silu(float x) { return x / (1.0f + __expf(-x)); }
-__device__ __forceinline__ float gelu_tanh(float x)
-{
-    const float u = 0.7978845608028654f * (x + 0.044715f * x * x * x);
-    return 0.5f * x * (1.0f + tanhf(u));
-}
+namespace {
 
 // out_bf16[r, :] = RMSNorm(x[r, :]) * w  [* (1 + scale[b]) + shift[b]]      one warp per row; the row is kept in
 // registers (D <= 1024: 8 float4 per lane) so x is read once.

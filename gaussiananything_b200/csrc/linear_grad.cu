@@ -20,8 +20,10 @@
 // depend on the card.  Each range writes an fp32 partial; a second kernel adds them in split order.
 #include "../../include/ga_b200.h"
 #include "device_once.cuh"
+#include "row_common.cuh"
 #include "sm90_ptx.cuh"
 
+using namespace ga_row;
 using namespace sm90;
 
 int ga_make_tmap_bf16(CUtensorMap *map, const void *ptr, uint64_t rows, uint64_t cols, uint64_t ld_elems,
@@ -51,12 +53,6 @@ struct GradArgs {
     int splits;
     long long split_stride;         // elements between partials
 };
-
-__device__ __forceinline__ uint32_t pack_bf16(float a, float b)
-{
-    __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<uint32_t *>(&h);
-}
 
 // d/dz of z Phi(z): Phi(z) + z phi(z), fp32
 __device__ __forceinline__ float gelu_grad(float z)
@@ -137,7 +133,7 @@ linear_grad_gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_
 {
     extern __shared__ uint8_t smem_raw[];
     __shared__ uint64_t full_bar[kStages], empty_bar[kStages];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t *smem = align1024(smem_raw);
     uint8_t *smem_a = smem, *smem_b = smem + kStages * kABytes;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -212,19 +208,6 @@ linear_grad_gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_
     }
 }
 
-// dw = sum over s of ws[s], in split order (float4 lanes; N K is a multiple of 64)
-__global__ void split_sum_kernel(const float4 *__restrict__ ws, float4 *__restrict__ dw, long long n4, int splits)
-{
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
-        float4 v = ws[i];
-        for (int s = 1; s < splits; s++) {
-            const float4 w = ws[s * n4 + i];
-            v.x += w.x; v.y += w.y; v.z += w.z; v.w += w.w;
-        }
-        dw[i] = v;
-    }
-}
-
 // Column sums of g bf16 [M, N], one block per (64 columns, chunk of kColRows rows): warp w adds rows w, w + 8, ...
 // of the chunk in order, lane l columns 2 l, 2 l + 1; the warp sums are added in warp order into out[chunk, :].
 __global__ void __launch_bounds__(32 * kColWarps)
@@ -254,16 +237,6 @@ colsum_chunk_kernel(const __nv_bfloat16 *__restrict__ g, float *__restrict__ out
     }
 }
 
-// db[c] = sum over chunks, in chunk order, of part[chunk, c]
-__global__ void colsum_final_kernel(const float *__restrict__ part, float *__restrict__ db, int chunks, int N)
-{
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= N) return;
-    float s = part[c];
-    for (int k = 1; k < chunks; k++) s += part[(long long)k * N + c];
-    db[c] = s;
-}
-
 int wgrad_splits(int M, int N, int K)
 {
     const long long tiles = (long long)((N + BM - 1) / BM) * ((K + BN - 1) / BN);
@@ -275,8 +248,6 @@ int wgrad_splits(int M, int N, int K)
 }
 
 int col_chunks(int M) { return (M + kColRows - 1) / kColRows; }
-
-bool misaligned(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
 
 template <int KIND, int EPI>
 int launch_grad_gemm(const CUtensorMap &ta, const CUtensorMap &tb, const GradArgs &a, cudaStream_t s)
@@ -324,19 +295,19 @@ extern "C" int ga_linear_grad_validate(int op, const void *a, const void *b, con
     if (op != GA_LINEAR_BGRAD && (K < 8 || K % 8)) return GA_ERR_BADARG;
     const long long wide = (op == GA_LINEAR_BGRAD || N >= K) ? N : K;
     if ((long long)M * wide >= (1LL << 31)) return GA_ERR_BADARG;
-    if (!a || misaligned(a) || !out || misaligned(out)) return GA_ERR_BADARG;
+    if (!a || mis16(a) || !out || mis16(out)) return GA_ERR_BADARG;
     size_t need = 0;
     switch (op) {
     case GA_LINEAR_FC1:
-        if (!b || misaligned(b) || !aux || misaligned(aux) || out_f32 != 0) return GA_ERR_BADARG;
+        if (!b || mis16(b) || !aux || mis16(aux) || out_f32 != 0) return GA_ERR_BADARG;
         if (block_n != 64 && block_n != 128 && block_n != 192 && block_n != 256) return GA_ERR_BADARG;
         return 0;
     case GA_LINEAR_DGRAD:
-        if (!b || misaligned(b) || (out_f32 != 0 && out_f32 != 1)) return GA_ERR_BADARG;
-        if (aux && (misaligned(aux) || out_f32)) return GA_ERR_BADARG;
+        if (!b || mis16(b) || (out_f32 != 0 && out_f32 != 1)) return GA_ERR_BADARG;
+        if (aux && (mis16(aux) || out_f32)) return GA_ERR_BADARG;
         return 0;
     case GA_LINEAR_WGRAD:
-        if (!b || misaligned(b) || out_f32 != 1) return GA_ERR_BADARG;
+        if (!b || mis16(b) || out_f32 != 1) return GA_ERR_BADARG;
         need = ga_linear_wgrad_workspace_bytes(M, N, K);
         break;
     default:
@@ -344,7 +315,7 @@ extern "C" int ga_linear_grad_validate(int op, const void *a, const void *b, con
         need = ga_linear_bias_grad_workspace_bytes(M, N);
         break;
     }
-    if (workspace_bytes < need || (need > 0 && (!workspace || misaligned(workspace)))) return GA_ERR_BADARG;
+    if (workspace_bytes < need || (need > 0 && (!workspace || mis16(workspace)))) return GA_ERR_BADARG;
     return 0;
 }
 
@@ -380,11 +351,7 @@ extern "C" int ga_linear_wgrad_bf16(const void *g, const void *x, float *dw, int
     cudaStream_t s = (cudaStream_t)stream;
     rc = launch_grad_gemm<kWgrad, kEpiF32>(ta, tb, a, s);
     if (rc || S == 1) return rc;
-    const long long n4 = (long long)N * K / 4;
-    const long long blocks = (n4 + 255) / 256;
-    split_sum_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, s>>>(
-        reinterpret_cast<const float4 *>(workspace), reinterpret_cast<float4 *>(dw), n4, S);
-    return (int)cudaGetLastError();
+    return (int)ga_launch_partial_sum(reinterpret_cast<const float *>(workspace), dw, 1, S, (long long)N * K, s);
 }
 
 extern "C" int ga_linear_bias_grad_bf16(const void *g, float *db, int M, int N, void *workspace, size_t workspace_bytes,
@@ -398,6 +365,6 @@ extern "C" int ga_linear_bias_grad_bf16(const void *g, float *db, int M, int N, 
     float *part = chunks > 1 ? reinterpret_cast<float *>(workspace) : db;
     colsum_chunk_kernel<<<(unsigned)((long long)chunks * col_blocks), 32 * kColWarps, 0, s>>>(
         reinterpret_cast<const __nv_bfloat16 *>(g), part, M, N, col_blocks);
-    if (chunks > 1) colsum_final_kernel<<<(N + 255) / 256, 256, 0, s>>>(part, db, chunks, N);
-    return (int)cudaGetLastError();
+    if (chunks == 1) return (int)cudaGetLastError();
+    return (int)ga_launch_partial_sum(part, db, 1, chunks, N, s);
 }

@@ -95,6 +95,26 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr)
 }
 __device__ __forceinline__ void warp_sync_smem() { asm volatile("bar.warp.sync 0xffffffff;\n" ::: "memory"); }
 
+// ---------------------------------------------------------------- cp.async and shared-memory layout
+// 16 bytes from global to shared memory; zeros when !valid (src must still be a valid address)
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid)
+{
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
+template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
+// cp.async writes through the generic proxy, wgmma reads through the async proxy
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
+
+// dynamic shared memory rounded up to the 1024-byte alignment of 128-byte-swizzled tiles (kernels reserve 1024 extra)
+__device__ __forceinline__ uint8_t *align1024(uint8_t *p)
+{
+    return reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(p) + 1023) & ~uintptr_t(1023));
+}
+// byte offset of 16-byte piece `chunk` of row `row` in a tile of 128-byte rows with 128-byte swizzle (the K-major
+// layout wgmma_desc_k_sw128 describes)
+__device__ __forceinline__ uint32_t sw128_off(int row, int chunk) { return row * 128 + ((chunk ^ (row & 7)) << 4); }
+
 // ---------------------------------------------------------------- register budget of warp-specialised kernels
 template <uint32_t kRegs> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(kRegs)); }
 template <uint32_t kRegs> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(kRegs)); }

@@ -4,6 +4,9 @@
 // with the posterior.  The 1x1 convolutions, linears and attentions run on the Part 2 GEMM / attention entry points.
 #include "../../include/ga_b200.h"
 #include "conv_igemm.cuh"
+#include "row_common.cuh"
+
+using namespace ga_row;
 
 namespace {
 
@@ -240,11 +243,6 @@ __global__ void heads32_kernel(const __nv_bfloat16 *__restrict__ qkv, const floa
 // logvar = 20 tanh(logvar / 20), std = exp(logvar / 2), latent = mean + std * eps.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int kHeadThreads = 256;
-
-__device__ __forceinline__ float gelu_tanh(float x)
-{
-    return 0.5f * x * (1.f + tanhf(0.7978845608028654f * (x + 0.044715f * x * x * x)));
-}
 
 __device__ __forceinline__ float block_sum(float v, float *red)
 {

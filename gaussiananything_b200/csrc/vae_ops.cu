@@ -10,21 +10,16 @@
 // /root/reference/vit/vision_transformer.py:215-303; the checker is oracle/vae_decoder_oracle.py.
 #include "../../include/ga_b200.h"
 #include "device_once.cuh"
-#include <cuda_bf16.h>
-#include <cuda_runtime.h>
+#include "row_common.cuh"
+
+using namespace ga_row;
 
 namespace {
 
-__device__ __forceinline__ float wsum(float v)
-{
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 // Warp sums of N values at once (N a power of two <= 32): at every butterfly step a lane keeps one half of its values
 // and hands the other half to its partner, so N totals cost N - 1 + log2(32 / N) shuffles instead of 5 N.  Lane l ends
 // up with the total of value index (l >> log2(32 / N)) & (N - 1); the additions are the ones the plain butterfly makes,
-// in the same order, so the totals are bit-identical to wsum().
+// in the same order, so the totals are bit-identical to warp_sum().
 template <int N>
 __device__ __forceinline__ float packed_wsum(float (&v)[N], int lane)
 {
@@ -42,7 +37,6 @@ __device__ __forceinline__ float packed_wsum(float (&v)[N], int lane)
     for (; o > 0; o >>= 1) v[0] += __shfl_xor_sync(0xffffffffu, v[0], o);
     return v[0];
 }
-__device__ __forceinline__ float silu_f(float x) { return x / (1.0f + __expf(-x)); }
 
 // one warp per row, row cached in registers (D % 4 == 0, D <= 1024)
 __global__ void __launch_bounds__(256)
@@ -63,7 +57,7 @@ layernorm_modulate_kernel(const float *__restrict__ x, const float *__restrict__
         c[u] = i < n4 ? x4[i] : make_float4(0.f, 0.f, 0.f, 0.f);
         s += (c[u].x + c[u].y) + (c[u].z + c[u].w);
     }
-    const float mean = wsum(s) / (float)D;
+    const float mean = warp_sum(s) / (float)D;
     float v = 0.f;
 #pragma unroll
     for (int u = 0; u < 8; u++) {
@@ -72,7 +66,7 @@ layernorm_modulate_kernel(const float *__restrict__ x, const float *__restrict__
             v += d0 * d0 + d1 * d1 + d2 * d2 + d3 * d3;
         }
     }
-    const float rs = rsqrtf(wsum(v) / (float)D + eps);
+    const float rs = rsqrtf(warp_sum(v) / (float)D + eps);
     const int b = r / rows_per_batch;
     const float4 *w4 = reinterpret_cast<const float4 *>(w), *b4 = reinterpret_cast<const float4 *>(bias);
     const float4 *sh4 = shift ? reinterpret_cast<const float4 *>(shift + (size_t)b * mod_ld) : nullptr;
@@ -139,7 +133,7 @@ thin_linear_kernel(const float *__restrict__ x, const float *__restrict__ ln_w, 
             float s = 0.f;
 #pragma unroll
             for (int u = 0; u < 8; u++) s += (c[q][u].x + c[q][u].y) + (c[q][u].z + c[q][u].w);
-            mean[q] = wsum(s) / (float)D;
+            mean[q] = warp_sum(s) / (float)D;
             float v = 0.f;
 #pragma unroll
             for (int u = 0; u < 8; u++) {
@@ -148,7 +142,7 @@ thin_linear_kernel(const float *__restrict__ x, const float *__restrict__ ln_w, 
                     v += d0 * d0 + d1 * d1 + d2 * d2 + d3 * d3;
                 }
             }
-            rs[q] = rsqrtf(wsum(v) / (float)D + eps);
+            rs[q] = rsqrtf(warp_sum(v) / (float)D + eps);
         }
     }
     float acc[THIN_ROWS][16];
@@ -173,7 +167,7 @@ thin_linear_kernel(const float *__restrict__ x, const float *__restrict__ ln_w, 
                     h[q].x = (h[q].x - mean[q]) * rs[q] * ww.x + bb.x; h[q].y = (h[q].y - mean[q]) * rs[q] * ww.y + bb.y;
                     h[q].z = (h[q].z - mean[q]) * rs[q] * ww.z + bb.z; h[q].w = (h[q].w - mean[q]) * rs[q] * ww.w + bb.w;
                 }
-                if (apply_silu) { h[q].x = silu_f(h[q].x); h[q].y = silu_f(h[q].y); h[q].z = silu_f(h[q].z); h[q].w = silu_f(h[q].w); }
+                if (apply_silu) { h[q].x = silu(h[q].x); h[q].y = silu(h[q].y); h[q].z = silu(h[q].z); h[q].w = silu(h[q].w); }
             }
 #pragma unroll
             for (int k = 0; k < 16; k++) {
@@ -191,7 +185,7 @@ thin_linear_kernel(const float *__restrict__ x, const float *__restrict__ ln_w, 
 #pragma unroll
         for (int k = 0; k < 16; k++) {
             if (k < C) {
-                const float t = wsum(acc[q][k]);
+                const float t = warp_sum(acc[q][k]);
                 if (lane == 0 && r0 + q < R) y[(size_t)(r0 + q) * C + k] = t + (bias ? bias[k] : 0.f);
             }
         }
@@ -242,8 +236,8 @@ micro_attention_kernel(const __nv_bfloat16 *__restrict__ qkv, const float *__res
             if (i0 + u < L) {
                 const int i = i0 + u;
                 const float2 q = __bfloat1622float2(rq[u]), k = __bfloat1622float2(rk[u]), v = __bfloat1622float2(rv[u]);
-                const float nq = rsqrtf(wsum(q.x * q.x + q.y * q.y) * (1.0f / 64.0f) + eps);
-                const float nk = rsqrtf(wsum(k.x * k.x + k.y * k.y) * (1.0f / 64.0f) + eps);
+                const float nq = rsqrtf(warp_sum(q.x * q.x + q.y * q.y) * (1.0f / 64.0f) + eps);
+                const float nk = rsqrtf(warp_sum(k.x * k.x + k.y * k.y) * (1.0f / 64.0f) + eps);
                 sq[i * kMicroPitch + 2 * lane] = q.x * nq * wq0; sq[i * kMicroPitch + 2 * lane + 1] = q.y * nq * wq1;
                 sk[i * kMicroPitch + 2 * lane] = k.x * nk * wk0; sk[i * kMicroPitch + 2 * lane + 1] = k.y * nk * wk1;
                 sv[i * kMicroPitch + 2 * lane] = v.x; sv[i * kMicroPitch + 2 * lane + 1] = v.y;
@@ -466,7 +460,7 @@ __global__ void surfel_cascade_pack_kernel(const float *__restrict__ res, int re
 __global__ void silu_to_bf16_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ y, size_t n)
 {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) y[i] = __float2bfloat16(silu_f(x[i]));
+    if (i < n) y[i] = __float2bfloat16(silu(x[i]));
 }
 
 inline int last_err() { return (int)cudaGetLastError(); }

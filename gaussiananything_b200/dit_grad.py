@@ -29,7 +29,7 @@ import torch
 from . import _lib
 from ._launch import epilogue, gemm, ptr, stream
 from ._lib import EPI_RESID_GATE_F32
-from .attention import _stride_table
+from .attention import _backward as _attention_bwd, _forward as _attention
 from .mlp import _bgrad, _dgrad, _fc1, _forward_linear, _pack, _wgrad
 
 __all__ = ["block_forward", "model_forward"]
@@ -88,23 +88,6 @@ def _reduce(part, groups, cols):
     return out
 
 
-def _attention(q, k, v, B, H, N, M):
-    o = torch.empty((B, N, H, 64), dtype=_BF16, device=q.device)
-    lse = torch.empty((B * H, N), dtype=_F32, device=q.device)
-    _lib.check(_lib.lib().ga_attention_fwd_lse_bf16(ptr(q), ptr(k), ptr(v), ptr(o), ptr(lse), B, H, N, M, 64, 64,
-                                                    _stride_table((q, k, v, o)), _SCALE, stream(q.device)),
-               "ga_attention_fwd_lse_bf16")
-    return o, lse
-
-
-def _attention_bwd(q, k, v, o, lse, g, dq, dk, dv, B, H, N, M):
-    delta = torch.empty((B * H, N), dtype=_F32, device=q.device)
-    _lib.check(_lib.lib().ga_attention_bwd_bf16(ptr(q), ptr(k), ptr(v), ptr(o), ptr(lse), ptr(g), ptr(delta),
-                                                ptr(dq), ptr(dk), ptr(dv), B, H, N, M, 64, 64,
-                                                _stride_table((q, k, v, o, g, dq, dk, dv)), _SCALE, stream(q.device)),
-               "ga_attention_bwd_bf16")
-
-
 def _gate_residual(x, a, gate, x_out, w=None, shift=None, scale=None, h=None, N=1, D=1):
     R = x.shape[0]
     _lib.check(_lib.lib().ga_dit_gate_residual(ptr(x), ptr(a), gate, 6 * D, ptr(x_out), ptr(w), shift, scale, 6 * D,
@@ -138,14 +121,14 @@ def _forward(x, t, ctx, params, keep):
     kv = _forward_linear(ctxb, wkv, None, _BF16)                       # [B M, 2 D]: k | v
     qcn = _qk_norm(qc, D, caqn_f, None, R, H, 1)
     kcn = _qk_norm(kv, 2 * D, cakn_f, None, RM, H, 1)
-    o_ca, lse_ca = _attention(qcn.view(B, N, H, 64), kcn.view(B, M, H, 64), _heads(kv, B, M, 2, 1), B, H, N, M)
+    o_ca, lse_ca = _attention(qcn.view(B, N, H, 64), kcn.view(B, M, H, 64), _heads(kv, B, M, 2, 1), _SCALE)
     a1 = _forward_linear(o_ca.view(R, D), wo, o_bf, _F32)
     x1, h1 = torch.empty_like(xf), torch.empty_like(h0)
     _gate_residual(xf, a1, None, x1, n1_f, ch(0), ch(1), h1, N, D)
     # gated self-attention
     qkv = _forward_linear(h1, wqkv, qkv_bf, _BF16)                      # [B N, 3 D]: q | k | v
     qkn = _qk_norm(qkv, 3 * D, qn_f, kn_f, R, H, 2)
-    o_sa, lse_sa = _attention(_heads(qkn, B, N, 2, 0), _heads(qkn, B, N, 2, 1), _heads(qkv, B, N, 3, 2), B, H, N, N)
+    o_sa, lse_sa = _attention(_heads(qkn, B, N, 2, 0), _heads(qkn, B, N, 2, 1), _heads(qkv, B, N, 3, 2), _SCALE)
     a2 = _forward_linear(o_sa.view(R, D), wp, p_bf, _F32)
     x2, h2 = torch.empty_like(xf), torch.empty_like(h0)
     _gate_residual(x1, a2, ch(2), x2, n2_f, ch(3), ch(4), h2, N, D)
@@ -247,8 +230,7 @@ def _backward(ctx, gy):
             do = _dgrad(da2, wp).view(B, N, H, 64)
             dqkv = torch.empty((R, 3 * D), dtype=_BF16, device=dev)
             _attention_bwd(_heads(qkn, B, N, 2, 0), _heads(qkn, B, N, 2, 1), _heads(qkv, B, N, 3, 2), o_sa, lse_sa,
-                           do, _heads(dqkv, B, N, 3, 0), _heads(dqkv, B, N, 3, 1), _heads(dqkv, B, N, 3, 2),
-                           B, H, N, N)
+                           do, _heads(dqkv, B, N, 3, 0), _heads(dqkv, B, N, 3, 1), _heads(dqkv, B, N, 3, 2), _SCALE)
             pqk = _qk_norm_bwd(qkv, 3 * D, dqkv, 3 * D, qn_f, kn_f, R, H, 2)
             if n_qn or n_kn:
                 dqk = _reduce(pqk, 2, 64)
@@ -275,7 +257,7 @@ def _backward(ctx, gy):
             _attention_bwd(qcn.view(B, N, H, 64), kcn.view(B, M, H, 64), _heads(kv, B, M, 2, 1), o_ca, lse_ca, do,
                            dq.view(B, N, H, 64) if q_side else None,
                            _heads(dkv, B, M, 2, 0) if kv_side else None,
-                           _heads(dkv, B, M, 2, 1) if kv_side else None, B, H, N, M)
+                           _heads(dkv, B, M, 2, 1) if kv_side else None, _SCALE)
             if q_side:
                 pq = _qk_norm_bwd(qc, D, dq, D, caqn_f, None, R, H, 1)
                 if n_cqn:

@@ -20,26 +20,18 @@ Deployed configuration only: the files' size == reso_encoder == reso == 512, cam
 reference's (PostProcess.paired_post_process_chunk with split_chunk_size 16: no shuffle, the first 8 views go to the
 encoder, the last 8 are the held-out ones).
 """
-import ctypes as C
 import os
 
 import numpy as np
 import torch
 
 from . import _lib
+from ._launch import ptr, stream
 
 SIZE = 512
 CHUNK_FILES = ("raw_img.jpg", "normal.png", "alpha.jpg", "depth.npz", "c.npy")
 PSNR_CAP = 100.0                         # dB reported where the squared error is exactly zero
 METRIC_BLOCKS = 64                       # GA_RECON_METRICS_BLOCKS of include/ga_b200.h
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr() if t is not None else 0)
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 def read_chunk(path):
@@ -160,8 +152,8 @@ def pack(chunk, views=None, device="cuda", with_targets=True):
              "depth": torch.empty(V, 1, h, w, device=dev), "mask": torch.empty(V, 1, h, w, device=dev)}
     with torch.cuda.device(dev):
         _lib.check(_lib.lib().ga_gbuffer_pack(
-            _p(raw), _p(normal), _p(alpha), _p(depth), _p(c), n, h, w, _p(vi), V, _p(enc),
-            *[_p(t[k] if t else None) for k in ("img", "alpha", "depth", "mask")], _stream(dev)), "ga_gbuffer_pack")
+            ptr(raw), ptr(normal), ptr(alpha), ptr(depth), ptr(c), n, h, w, ptr(vi), V, ptr(enc),
+            *[ptr(t[k] if t else None) for k in ("img", "alpha", "depth", "mask")], stream(dev)), "ga_gbuffer_pack")
     if t is not None:
         t["normal"] = enc[:, 3:6]
     return enc, t, c[vi.long()]
@@ -194,9 +186,9 @@ def metric_table(render_out, targets):
     table = torch.empty(V, 8, device=dev)
     ti, td, ta, tm = (targets[k].contiguous() for k in ("img", "depth", "alpha", "mask"))
     with torch.cuda.device(dev):
-        _lib.check(_lib.lib().ga_recon_metrics(_p(img), _p(dep), _p(alp), _p(nrm), _p(ti), _p(td), _p(ta), _p(tm), _p(tn),
-                                               tn.stride(0) if V > 1 else 3 * H * W, V, H, W, _p(partial), _p(table),
-                                               _stream(dev)), "ga_recon_metrics")
+        _lib.check(_lib.lib().ga_recon_metrics(ptr(img), ptr(dep), ptr(alp), ptr(nrm), ptr(ti), ptr(td), ptr(ta), ptr(tm), ptr(tn),
+                                               tn.stride(0) if V > 1 else 3 * H * W, V, H, W, ptr(partial), ptr(table),
+                                               stream(dev)), "ga_recon_metrics")
     return table
 
 

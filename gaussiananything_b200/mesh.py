@@ -19,6 +19,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._launch import ptr, stream
 from .mc_table import TRI_TABLE
 
 AABB = np.array([-0.45, -0.45, -0.45, 0.45, 0.45, 0.45]).reshape(2, 3) * 1.1
@@ -141,10 +142,6 @@ class TriangleMesh:
         return self._v, self._t, self._c
 
 
-def _ptr(t):
-    return C.c_void_p(t.data_ptr())
-
-
 def _check_cuda(x, name, dtype, dev=None):
     if not isinstance(x, torch.Tensor) or not x.is_cuda:
         raise RuntimeError("%s must be a CUDA tensor (no CPU fallback)" % name)
@@ -165,7 +162,7 @@ class _Status:
         self.event.record(torch.cuda.current_stream(dev))
 
     def args(self):
-        return _ptr(self.dev_words), C.c_void_p(self.host.data_ptr()), C.c_void_p(self.event.cuda_event)
+        return ptr(self.dev_words), C.c_void_p(self.host.data_ptr()), C.c_void_p(self.event.cuda_event)
 
     def read(self):
         self.event.synchronize()
@@ -197,7 +194,7 @@ def fuse(rgb, depth, alpha, setup, alpha_thres=ALPHA_THRES, stages=None):
         raise ValueError("fuse: the setup was made for %d views of %dx%d" % (len(setup["cams_f"]), setup["H"],
                                                                            setup["W"]))
     rgb, depth, alpha = rgb.contiguous(), depth.contiguous(), alpha.contiguous()
-    s = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    s = stream(dev)
     mark = stages or (lambda name: None)
     f64 = dict(dtype=torch.float64, device=dev)
     trunc = torch.tensor(setup["depth_trunc"], **f64)
@@ -209,15 +206,15 @@ def fuse(rgb, depth, alpha, setup, alpha_thres=ALPHA_THRES, stages=None):
     n_box = int(np.prod(box_h[3:].astype(np.int64)))
     st = _Status(dev)
     texels = torch.empty(V, H, W, 2, dtype=torch.int32, device=dev)
-    _lib.check(lib.ga_mesh_prepare(_ptr(rgb), _ptr(depth), _ptr(alpha), V, H, W, _ptr(trunc), float(alpha_thres),
-                                   _ptr(texels), s), "ga_mesh_prepare")
+    _lib.check(lib.ga_mesh_prepare(ptr(rgb), ptr(depth), ptr(alpha), V, H, W, ptr(trunc), float(alpha_thres),
+                                   ptr(texels), s), "ga_mesh_prepare")
     mark("prepare")
     table = torch.empty(n_box, (V + 31) // 32, dtype=torch.int32, device=dev)
     pool = torch.empty(n_box, dtype=torch.int32, device=dev)
     slot = torch.empty(n_box, dtype=torch.int32, device=dev)
     work = _work(n_box, dev)
-    _lib.check(lib.ga_mesh_touch(_ptr(texels), V, H, W, _ptr(cams_d), _ptr(volume), _ptr(box), n_box, _ptr(table),
-                                 _ptr(pool), _ptr(slot), _ptr(work), *st.args(), s), "ga_mesh_touch")
+    _lib.check(lib.ga_mesh_touch(ptr(texels), V, H, W, ptr(cams_d), ptr(volume), ptr(box), n_box, ptr(table),
+                                 ptr(pool), ptr(slot), ptr(work), *st.args(), s), "ga_mesh_touch")
     words = st.read()
     if words[1]:
         raise RuntimeError("extract_mesh_bounded: a depth point lies outside the volume box %s" % (box_h.tolist(),))
@@ -225,25 +222,25 @@ def fuse(rgb, depth, alpha, setup, alpha_thres=ALPHA_THRES, stages=None):
     mark("touch")
     nvox = n_units * 4096
     voxels = torch.empty(5, max(nvox, 1), dtype=torch.float32, device=dev)
-    _lib.check(lib.ga_mesh_integrate(_ptr(texels), V, H, W, _ptr(cams_f), _ptr(volume), _ptr(box), _ptr(table),
-                                     _ptr(pool), n_units, _ptr(voxels), s), "ga_mesh_integrate")
+    _lib.check(lib.ga_mesh_integrate(ptr(texels), V, H, W, ptr(cams_f), ptr(volume), ptr(box), ptr(table),
+                                     ptr(pool), n_units, ptr(voxels), s), "ga_mesh_integrate")
     mark("integrate")
     tri_table = torch.tensor(TRI_TABLE, device=dev)
     cube = torch.empty(2, max(nvox, 1), dtype=torch.uint8, device=dev)
     vert_off = torch.empty(max(nvox, 1), dtype=torch.int32, device=dev)
     tri_off = torch.empty(max(nvox, 1), dtype=torch.int32, device=dev)
     work = _work(nvox, dev)
-    _lib.check(lib.ga_mesh_cubes_count(_ptr(voxels), n_units, _ptr(pool), _ptr(slot), _ptr(box), _ptr(tri_table),
-                                       _ptr(cube), _ptr(vert_off), _ptr(tri_off), _ptr(work), *st.args(), s),
+    _lib.check(lib.ga_mesh_cubes_count(ptr(voxels), n_units, ptr(pool), ptr(slot), ptr(box), ptr(tri_table),
+                                       ptr(cube), ptr(vert_off), ptr(tri_off), ptr(work), *st.args(), s),
                "ga_mesh_cubes_count")
     words = st.read()
     nv, nt = words[2], words[3]
     verts = torch.empty(nv, 3, **f64)
     cols = torch.empty(nv, 3, **f64)
     tris = torch.empty(nt, 3, dtype=torch.int32, device=dev)
-    _lib.check(lib.ga_mesh_cubes_emit(_ptr(voxels), n_units, _ptr(pool), _ptr(slot), _ptr(box), _ptr(volume),
-                                      _ptr(tri_table), _ptr(cube), _ptr(vert_off), _ptr(tri_off), _ptr(verts),
-                                      _ptr(cols), _ptr(tris), s), "ga_mesh_cubes_emit")
+    _lib.check(lib.ga_mesh_cubes_emit(ptr(voxels), n_units, ptr(pool), ptr(slot), ptr(box), ptr(volume),
+                                      ptr(tri_table), ptr(cube), ptr(vert_off), ptr(tri_off), ptr(verts),
+                                      ptr(cols), ptr(tris), s), "ga_mesh_cubes_emit")
     mark("marching_cubes")
     state = dict(texels=texels, table=table, pool=pool[:n_units], slot=slot, voxels=voxels[:, :nvox],
                  cube=cube[:, :nvox], n_units=n_units)
@@ -288,8 +285,8 @@ def _clusters(v, t):
     sizes = torch.empty(max(nt, 1), dtype=torch.int32, device=dev)
     work = _work(nt, dev)
     st = _Status(dev)
-    s = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-    _lib.check(lib.ga_mesh_clusters(_ptr(t), nt, _ptr(hash_), slots, _ptr(label), _ptr(sizes), _ptr(work),
+    s = stream(dev)
+    _lib.check(lib.ga_mesh_clusters(ptr(t), nt, ptr(hash_), slots, ptr(label), ptr(sizes), ptr(work),
                                     *st.args(), s), "ga_mesh_clusters")
     nc = st.read()[4]
     return label[:nt], sizes[:nc]
@@ -313,9 +310,9 @@ def post_process_mesh(mesh, cluster_to_keep=None):
     out_t = torch.empty_like(t)
     work = _work(nv + nt, dev)
     st = _Status(dev)
-    s = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-    _lib.check(lib.ga_mesh_filter(_ptr(v), _ptr(c), nv, _ptr(t), nt, _ptr(label), _ptr(sizes), n_min, _ptr(out_v),
-                                  _ptr(out_c), _ptr(out_t), _ptr(work), *st.args(), s), "ga_mesh_filter")
+    s = stream(dev)
+    _lib.check(lib.ga_mesh_filter(ptr(v), ptr(c), nv, ptr(t), nt, ptr(label), ptr(sizes), n_min, ptr(out_v),
+                                  ptr(out_c), ptr(out_t), ptr(work), *st.args(), s), "ga_mesh_filter")
     w = st.read()
     return TriangleMesh(out_v[:w[5]], out_t[:w[6]], out_c[:w[5]])
 

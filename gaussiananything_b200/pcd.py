@@ -15,7 +15,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .gbuffer import _p, _stream, read_chunk, to_device
+from ._launch import ptr, stream
+from .gbuffer import read_chunk, to_device
 
 ALPHA_MIN = 255          # save_pcd_from_depth's alpha_mask == 1 on the 8-bit alpha.jpg
 MIN_DEPTH = 1.05         # its depth < 1.05 outlier filter
@@ -61,8 +62,8 @@ def sample_farthest_points(points, lengths=None, K=50, random_start_point=False,
     ws = torch.empty(L.ga_fps_ex_workspace_bytes(B, N, Kmax), dtype=torch.uint8, device=dev)
     ld = None if lengths is None else lens.to(dev, torch.int32)
     with torch.cuda.device(dev):
-        _lib.check(L.ga_fps_ex(_p(pts), _p(ld), B, N, Kmax, _p(start.to(dev)), _p(idx), _p(xyz), _p(ws), ws.numel(),
-                               _stream(dev)), "ga_fps_ex")
+        _lib.check(L.ga_fps_ex(ptr(pts), ptr(ld), B, N, Kmax, ptr(start.to(dev)), ptr(idx), ptr(xyz), ptr(ws), ws.numel(),
+                               stream(dev)), "ga_fps_ex")
     if int(Ks.min()) < Kmax:                                   # per-cloud K: FPS is prefix-stable, so cut and pad
         cut = torch.arange(Kmax)[None] >= Ks[:, None]
         cut = cut.to(dev)
@@ -95,9 +96,9 @@ def chunk_surface_points(chunk, views=None, alpha_min=ALPHA_MIN, min_depth=MIN_D
     L = _lib.lib()
     scratch = torch.empty(L.ga_chunk_surface_points_scratch_bytes(V, h, w), dtype=torch.uint8, device=dev)
     with torch.cuda.device(dev):
-        _lib.check(L.ga_chunk_surface_points(_p(d["alpha"]), _p(d["depth"]), _p(d["c"]), n, h, w, _p(vi), V,
-                                             int(alpha_min), float(min_depth), _p(pts), _p(count), _p(scratch),
-                                             scratch.numel(), _stream(dev)), "ga_chunk_surface_points")
+        _lib.check(L.ga_chunk_surface_points(ptr(d["alpha"]), ptr(d["depth"]), ptr(d["c"]), n, h, w, ptr(vi), V,
+                                             int(alpha_min), float(min_depth), ptr(pts), ptr(count), ptr(scratch),
+                                             scratch.numel(), stream(dev)), "ga_chunk_surface_points")
     return pts[:int(count)]
 
 

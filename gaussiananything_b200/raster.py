@@ -10,16 +10,9 @@ import ctypes as C
 import torch
 
 from . import _lib
+from ._launch import ptr, stream
 
 _capacity_hint = {}
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr())
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 LIST_K = 32          # per-pixel contribution-list capacity used when the caller will ask for gradients
@@ -124,9 +117,9 @@ def _forward_on_device(lib, dev, gauss13, viewmats, projmats, bg, B, P, V, H, W,
         # num_rendered back) is copied to pinned memory right after the tile scan, so this wait returns while the
         # GPU is still scattering, sorting and compositing -- no bubble in the stream
         _lib.check(lib.ga_raster_forward_ex(
-            _ptr(gauss13), B, P, V, _ptr(viewmats), _ptr(projmats), _ptr(bg), H, W, float(scale_modifier),
-            _ptr(color), _ptr(allmap), _ptr(radii), _ptr(ws), L.total_bytes, max_instances, list_k,
-            C.c_void_p(host_status.data_ptr()), C.c_void_p(ev.cuda_event), _stream(dev)),
+            ptr(gauss13), B, P, V, ptr(viewmats), ptr(projmats), ptr(bg), H, W, float(scale_modifier),
+            ptr(color), ptr(allmap), ptr(radii), ptr(ws), L.total_bytes, max_instances, list_k,
+            C.c_void_p(host_status.data_ptr()), C.c_void_p(ev.cuda_event), stream(dev)),
             "ga_raster_forward_ex")
         ev.synchronize()
         status = host_status.clone()
@@ -163,12 +156,12 @@ def backward_raw(state, grad_color, grad_allmap):
     with torch.cuda.device(dev):
         pool_key, scratch = _take_scratch(dev, nbytes)
         grad = torch.empty(B, P, 13, device=dev, dtype=torch.float32)
-        rc = lib.ga_raster_backward_ex(_ptr(state["gauss13"]), B, P, V, _ptr(state["viewmats"]),
-                                    _ptr(state["projmats"]), _ptr(state["bg"]), H, W,
-                                    state["scale_modifier"], _ptr(state["radii"]),
-                                    _ptr(grad_color), _ptr(grad_allmap),
-                                    _ptr(state["ws"]), state["L"].total_bytes, state["max_instances"], state.get("list_k", 0),
-                                    _ptr(scratch), nbytes, _ptr(grad), _stream(dev))
+        rc = lib.ga_raster_backward_ex(ptr(state["gauss13"]), B, P, V, ptr(state["viewmats"]),
+                                    ptr(state["projmats"]), ptr(state["bg"]), H, W,
+                                    state["scale_modifier"], ptr(state["radii"]),
+                                    ptr(grad_color), ptr(grad_allmap),
+                                    ptr(state["ws"]), state["L"].total_bytes, state["max_instances"], state.get("list_k", 0),
+                                    ptr(scratch), nbytes, ptr(grad), stream(dev))
     if len(_scratch_pool[pool_key]) < 2:
         _scratch_pool[pool_key].append(scratch)          # reused by later calls on the same stream: stream-ordered, safe
     _lib.check(rc, "ga_raster_backward_ex")
@@ -216,8 +209,8 @@ class _RenderPost(torch.autograd.Function):
         normal = torch.empty(B, V, 3, H, W, device=dev)
         dist = torch.empty(B, V, 1, H, W, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(lib.ga_render_post_forward(_ptr(color), _ptr(allmap), _ptr(vm), B * V, H, W, _ptr(image),
-                                                  _ptr(alpha), _ptr(depth), _ptr(normal), _ptr(dist), _stream(dev)),
+            _lib.check(lib.ga_render_post_forward(ptr(color), ptr(allmap), ptr(vm), B * V, H, W, ptr(image),
+                                                  ptr(alpha), ptr(depth), ptr(normal), ptr(dist), stream(dev)),
                        "ga_render_post_forward")
         ctx.save_for_backward(color, allmap, vm)
         return image, alpha, depth, normal, dist
@@ -232,10 +225,10 @@ class _RenderPost(torch.autograd.Function):
         g_color = torch.empty_like(color)
         g_allmap = torch.empty_like(allmap)
         null = C.c_void_p(0)
-        ptrs = [null if g is None else _ptr(g) for g in gs]
+        ptrs = [null if g is None else ptr(g) for g in gs]
         with torch.cuda.device(dev):
-            _lib.check(lib.ga_render_post_backward(_ptr(color), _ptr(allmap), _ptr(vm), B * V, H, W, *ptrs, _ptr(g_color),
-                                                   _ptr(g_allmap), _stream(dev)), "ga_render_post_backward")
+            _lib.check(lib.ga_render_post_backward(ptr(color), ptr(allmap), ptr(vm), B * V, H, W, *ptrs, ptr(g_color),
+                                                   ptr(g_allmap), stream(dev)), "ga_render_post_backward")
         return g_color, g_allmap, None
 
 

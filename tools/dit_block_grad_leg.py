@@ -76,7 +76,7 @@ def row_kernel_bytes(B, N, M, D):
         "gate_residual_kernel": 2 * 14 * R * D + 12 * R * D,
         "qk_norm_fwd_kernel": 4 * D * (3 * R + RM),      # bf16 in and out: CA q, CA k, SA q|k
         "qk_norm_bwd_kernel": 6 * D * (3 * R + RM),      # pre-norm, dq/dk read, gradient written
-        "grad_reduce_kernel": 4 * 9 * P * D,             # the norm and modulation partials
+        "partial_sum_kernel": 4 * 9 * P * D,             # the norm and modulation partials
     }
 
 

@@ -156,7 +156,7 @@ def main():
     ap.add_argument("--skip-torch-4m", action="store_true", help="leave out the torch loop on 4M points")
     args = ap.parse_args()
     from gaussiananything_b200 import _lib, gbuffer, pcd
-    from gaussiananything_b200.gbuffer import _p, _stream
+    from gaussiananything_b200._launch import ptr as _p, stream as _stream
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
     name, watts, mhz = card()
