@@ -463,6 +463,12 @@ extern "C" int ga_conv4x4_out_size(int H, int stride)
     return H >= 2 && o > 0 ? o : GA_ERR_BADARG;
 }
 
+// the kernels read and write float2 and __nv_bfloat162 through these pointers
+static inline bool misaligned(const void *p, uintptr_t bytes)
+{
+    return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) != 0;
+}
+
 static int conv4x4_args(ConvArgs &a, const void *x, int n, int H, int W, int Cin, const void *w_packed, int k_pitch,
                         const float *bias, int Cout, int stride, float *out_f32, void *out_bf16)
 {
@@ -478,7 +484,7 @@ extern "C" int ga_conv4x4_lrelu_bf16(const void *x, int n, int H, int W, int Cin
     ConvArgs a;
     const int rc = conv4x4_args(a, x, n, H, W, Cin, w_packed, k_pitch, bias, Cout, stride, nullptr, out_bf16);
     if (rc) return rc;
-    if (!out_bf16) return GA_ERR_BADARG;
+    if (!out_bf16 || misaligned(out_bf16, 4)) return GA_ERR_BADARG;
     cudaStream_t s = (cudaStream_t)stream;
     return Cout % 128 == 0 ? launch_conv<4, 128, kEpiLrelu>(a, s) : launch_conv<4, 64, kEpiLrelu>(a, s);
 }
@@ -487,7 +493,7 @@ extern "C" int ga_conv4x4_stats(const void *x, int n, int H, int W, int Cin, con
                                 int Cout, int stride, float *z, void *partial, void *stream)
 {
     ConvArgs a;
-    if (!z || (reinterpret_cast<uintptr_t>(partial) & 7)) return GA_ERR_BADARG;
+    if (!z || misaligned(z, 8) || misaligned(partial, 8)) return GA_ERR_BADARG;
     const int rc = conv4x4_args(a, x, n, H, W, Cin, w_packed, k_pitch, nullptr, Cout, stride, z, nullptr);
     if (rc) return rc;
     a.partial = reinterpret_cast<float2 *>(partial);
@@ -503,6 +509,7 @@ extern "C" int ga_disc_bn_forward(const float *z, const void *partial, int64_t M
 {
     if (!z || !gamma || !beta || !running_mean || !running_var || !mean_out || !rstd_out || !a_out) return GA_ERR_BADARG;
     if (M <= 0 || C <= 0 || C % 2 || (training && (!partial || M < 2))) return GA_ERR_BADARG;
+    if (misaligned(z, 8) || misaligned(partial, 8) || misaligned(a_out, 4)) return GA_ERR_BADARG;
     if (M > ((int64_t)1 << 31) / CBM * CBM) return GA_ERR_SIZE;
     cudaStream_t s = (cudaStream_t)stream;
     const int nb = (int)((M + CBM - 1) / CBM);
@@ -537,6 +544,9 @@ extern "C" int ga_disc_conv5_backward(const float *g5, int n, int H, int W, cons
     if (!g5 || !w5 || !a4 || !z4 || !mean4 || !rstd4 || !gy4 || !bn_partial || (!dw_partial) != (!dw5))
         return GA_ERR_BADARG;
     if (n <= 0 || H < 2 || W < 2) return GA_ERR_BADARG;
+    if (misaligned(a4, 4) || misaligned(z4, 8) || misaligned(gy4, 8) || misaligned(bn_partial, 8) ||
+        misaligned(dw_partial, 8))
+        return GA_ERR_BADARG;
     const int nb = ga_disc_conv5_partials(n, H, W);
     cudaStream_t s = (cudaStream_t)stream;
     disc_conv5_backward_kernel<<<nb, kC5 / 2, 0, s>>>(g5, n, H, W, w5, reinterpret_cast<const __nv_bfloat16 *>(a4), z4,
@@ -567,6 +577,8 @@ extern "C" int ga_disc_dgrad(const void *g, int n, int H, int W, int Cg, const v
     if (Hg <= 0 || Wg <= 0 || !act || (reinterpret_cast<uintptr_t>(act) & 3)) return GA_ERR_BADARG;
     const bool bn = z != nullptr;
     if (bn ? (!mean || !rstd || !gy_out || !partial || out_bf16) : (!out_bf16 || gy_out)) return GA_ERR_BADARG;
+    if (misaligned(z, 8) || misaligned(gy_out, 8) || misaligned(partial, 8) || misaligned(out_bf16, 4))
+        return GA_ERR_BADARG;
     cudaStream_t s = (cudaStream_t)stream;
     const int ncls = stride == 1 ? 1 : 4;
     int part_off = 0;
@@ -609,6 +621,9 @@ extern "C" int ga_disc_bn_backward(const float *gy, const float *z, int64_t M, i
 {
     if (!gy || !z || !mean || !rstd || !gamma || !partial || !k_scratch || !dz_bf16) return GA_ERR_BADARG;
     if (M <= 0 || C <= 0 || C % 2 || n_partial <= 0) return GA_ERR_BADARG;
+    if (misaligned(gy, 8) || misaligned(z, 8) || misaligned(partial, 8) || misaligned(k_scratch, 8) ||
+        misaligned(dz_bf16, 4))
+        return GA_ERR_BADARG;
     cudaStream_t s = (cudaStream_t)stream;
     float2 *k = reinterpret_cast<float2 *>(k_scratch);
     bn_grad_finalize_kernel<<<C, kFinThreads, 0, s>>>(reinterpret_cast<const float2 *>(partial), n_partial, M, C,
@@ -636,6 +651,7 @@ extern "C" int ga_disc_wgrad(const void *dy, const void *x, int n, int H, int W,
     const int64_t P = (int64_t)n * Ho * Wo;
     if (P >= (int64_t)1 << 31 || (int64_t)n * H * W >= (int64_t)1 << 31) return GA_ERR_SIZE;
     if (!workspace || workspace_bytes < ga_disc_wgrad_workspace_bytes(n, Ho, Wo, Co, Cin)) return GA_ERR_WORKSPACE;
+    if (misaligned(workspace, 8)) return GA_ERR_BADARG;
     static GaPerDevice attr_set;
     if (ga_first_use_on_device(attr_set)) {
         cudaError_t e = cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmem);

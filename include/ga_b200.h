@@ -669,6 +669,12 @@ int ga_chunk_surface_points(const uint8_t *alpha, const float *depth, const floa
  * and the logits fp32; conv 5's weights fp32.  disc_ops.cu is compiled without FMA contraction: every operation of
  * the non-GEMM kernels below is rounded to fp32 on its own, in the order written.  No atomics: the same inputs give
  * the same bits.
+ * Alignment (GA_ERR_BADARG otherwise): the bf16 NHWC inputs of the convolutions and g1 of ga_disc_input_backward
+ * 16 bytes; every fp32 tensor read or written as float2 8 bytes (z of ga_conv4x4_stats; z and partial of
+ * ga_disc_bn_forward; z4, gy4, bn_partial and dw_partial of ga_disc_conv5_backward; z, gy_out and partial of
+ * ga_disc_dgrad; gy, z, partial and k_scratch of ga_disc_bn_backward; the workspace of ga_disc_wgrad); every bf16
+ * tensor read or written in pairs 4 bytes (the bf16 outputs of ga_conv4x4_lrelu_bf16, ga_disc_bn_forward,
+ * ga_disc_dgrad and ga_disc_bn_backward; act of ga_disc_dgrad; a4 of ga_disc_conv5_backward).
  * BatchNorm statistics: each conv CTA (128 output pixels) writes its channel mean m_b (fp32 sum / count) and
  * M2_b = sum (z - m_b)^2 (fp32, from the accumulator registers); the finalize merges them in fp64 with Chan's rule
  * (mean += d n_b / n, M2 += M2_b + d^2 n_a n_b / n), so no E[z^2] - mean^2 cancellation: thread t of 128 merges CTAs
