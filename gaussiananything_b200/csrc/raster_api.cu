@@ -3,6 +3,7 @@
 #include "raster_common.cuh"
 
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+static_assert(GA_ROW_F == GA_RASTER_ROW_FLOATS && GA_GRAD_F <= GA_RASTER_GRAD_FLOATS, "gradient row sizes");
 
 // ---- optional per-stage timing (bench.py's roofline leg) -------------------
 static int g_profile = 0;
@@ -141,13 +142,15 @@ extern "C" int ga_raster_forward_ex(const float *gauss13, int batch, int P, int 
     return 0;
 }
 
-// Backward scratch = gradient accumulators [NV*P][18]; the per-(pixel, surfel) records stay in shared memory
-static size_t bwd_acc_bytes(int batch, int P, int views) { return align_up((size_t)batch * views * P * GA_GRAD_F * sizeof(float), 256); }
+// Backward scratch: the per-surfel gradient rows [batch][P][GA_ROW_F] (raster_common.cuh) at its start; the
+// per-(pixel, surfel) records stay in shared memory.  The size asked for stays that of one GA_RASTER_GRAD_FLOATS row
+// per (view, surfel), which callers size their buffers by; only the leading rows are used.
+static size_t bwd_scratch_bytes(int batch, int P, int views) { return align_up((size_t)batch * views * P * GA_RASTER_GRAD_FLOATS * sizeof(float), 256); }
 
 extern "C" size_t ga_raster_backward_scratch_bytes(int batch, int P, int views)
 {
     if (batch <= 0 || P <= 0 || views <= 0) return 0;
-    return bwd_acc_bytes(batch, P, views);
+    return bwd_scratch_bytes(batch, P, views);
 }
 
 extern "C" int ga_raster_backward_ex(const float *gauss13, int batch, int P, int views,
@@ -168,19 +171,19 @@ extern "C" int ga_raster_backward_ex(const float *gauss13, int batch, int P, int
     GaRasterLayout L;
     ga_raster_layout_ex(batch, P, views, H, W, max_instances, list_k, &L);
     if (workspace_bytes < L.total_bytes) return GA_ERR_WORKSPACE;
-    const size_t need = bwd_acc_bytes(batch, P, views);                 // a larger buffer is accepted; the rest is unused
-    if (scratch_bytes < need) return GA_ERR_WORKSPACE;
+    if (scratch_bytes < bwd_scratch_bytes(batch, P, views)) return GA_ERR_WORKSPACE;   // a larger buffer is accepted
+    if ((uintptr_t)scratch % 16) return GA_ERR_BADARG;                   // the rows are read as float4
     RasterWs w;
     carve(L, d, const_cast<void *>(workspace), &w);
     cudaStream_t s = (cudaStream_t)stream;
     cudaError_t e;
-    float *grad_acc = (float *)scratch;
+    float *grad_rows = (float *)scratch;
     prof(4, s);
-    if ((e = cudaMemsetAsync(grad_acc, 0, need, s)) != cudaSuccess) return (int)e;
-    if ((e = ga_launch_render_bwd(d, w, bg, dL_dcolor, dL_dallmap, grad_acc, s)) != cudaSuccess) return (int)e;
-    prof(5, s);
-    if ((e = ga_launch_preprocess_bwd(d, w, gauss13, viewmats, projmats, radii, grad_acc, grad_gauss13, s)) != cudaSuccess)
+    if ((e = cudaMemsetAsync(grad_rows, 0, (size_t)batch * P * GA_ROW_F * sizeof(float), s)) != cudaSuccess) return (int)e;
+    if ((e = ga_launch_render_bwd(d, w, bg, viewmats, projmats, dL_dcolor, dL_dallmap, grad_rows, s)) != cudaSuccess)
         return (int)e;
+    prof(5, s);
+    if ((e = ga_launch_preprocess_bwd(d, gauss13, grad_rows, grad_gauss13, s)) != cudaSuccess) return (int)e;
     prof(6, s);
     return 0;
 }

@@ -14,12 +14,19 @@
 #define GA_CUTOFF 3.0f
 #define GA_REC_F 24
 #define GA_GRAD_F 18
+#define GA_ROW_F 16
 
 // record float offsets (6 x float4):
 //  q0 = Tu.x Tu.y Tu.z Tv.x | q1 = Tv.y Tv.z Tw.x Tw.y | q2 = Tw.z xy.x xy.y opacity
-//  q3 = n.x n.y n.z r        | q4 = bbox x0 x1 y0 y1    | q5 = g b - -
-// gradient accumulator float offsets:
+//  q3 = n.x n.y n.z r        | q4 = bbox x0 x1 y0 y1    | q5 = g b sign -
+// sign: +1 or -1, the factor K1 applied to the view-space normal so that it faces the camera.
+// Per-(tile, instance) gradient components that the backward's phase B sums over a surfel's records (GA_GRAD_F):
 //  0-8 dL/dT (Tu,Tv,Tw) | 9-10 dL/dmean2D | 11-13 dL/dnormal | 14 dL/dopacity | 15-17 dL/drgb
+// Per-surfel gradient row, summed over the views of the batch item (GA_ROW_F), [batch][P][16]:
+//  0-8 dL/dM, entry 3r+k = row r (0: scale-x axis, 1: scale-y axis, 2: position) and world axis k | 9-11 dL/dR column
+//  2 (the normal) | 12 dL/dopacity | 13-15 dL/drgb
+// The map from the 18 components to the row is linear and depends only on the view and on the record, so the
+// backward applies it to each (tile, instance) partial sum before it adds the partial to the row.
 
 struct RasterDims {
     int batch, P, views, NV;   // NV = batch*views images
@@ -81,10 +88,10 @@ cudaError_t ga_launch_binning(const RasterDims &d, const RasterWs &w, cudaStream
                               cudaEvent_t status_event);
 cudaError_t ga_launch_render_fwd(const RasterDims &d, const RasterWs &w, const float *bg,
                                  float *out_color, float *out_allmap, cudaStream_t s);
+// grad_rows: [batch][P][GA_ROW_F], zeroed by the caller; render_bwd adds into it and preprocess_bwd reads it
 cudaError_t ga_launch_render_bwd(const RasterDims &d, const RasterWs &w, const float *bg,
+                                 const float *viewmats, const float *projmats,
                                  const float *dL_dcolor, const float *dL_dallmap,
-                                 float *grad_acc, cudaStream_t s);
-cudaError_t ga_launch_preprocess_bwd(const RasterDims &d, const RasterWs &w, const float *gauss13,
-                                     const float *viewmats, const float *projmats,
-                                     const int32_t *radii, const float *grad_acc,
+                                 float *grad_rows, cudaStream_t s);
+cudaError_t ga_launch_preprocess_bwd(const RasterDims &d, const float *gauss13, const float *grad_rows,
                                      float *grad_gauss13, cudaStream_t s);

@@ -26,8 +26,7 @@ __device__ __forceinline__ void quat_to_rotmat(const float *q, float R[3][3])
     R[2][2] = 1.f - 2.f * (x * x + y * y);
 }
 
-// T = (Tu, Tv, Tw): the surfel's ray-splat transform for one view.  K1 stores it in the record and K5 recomputes it
-// from the same inputs with the same operations (so with the same bits) instead of reading it back.
+// T = (Tu, Tv, Tw): the surfel's ray-splat transform for one view, stored in the record.
 __device__ __forceinline__ void surfel_transmat(const float R[3][3], float sx, float sy, float px, float py, float pz,
                                                 const float *pm, int W, int H, float Tu[3], float Tv[3], float Tw[3])
 {
@@ -118,6 +117,9 @@ __device__ __forceinline__ void preprocess_one(const RasterDims &d, const Raster
                     rec[9] = cx; rec[10] = cy; rec[11] = opa;
                     rec[12] = nx; rec[13] = ny; rec[14] = nz; rec[15] = g[10];
                     rec[20] = g[11]; rec[21] = g[12];
+                    // the backward's normal sign, cosv > 0 ? 1 : -1; a surfel with cosv == 0 gets no tiles, so the
+                    // sign of every instance the backward reads is this one
+                    rec[22] = mult;
                     // ---- conservative cull box: a pixel outside can never reach
                     // alpha >= 1/255, i.e. needs min(rho3d, rho2d) <= tau = 2 ln(255 o).
                     float bx0 = 1e30f, bx1 = -1e30f, by0 = 1e30f, by1 = -1e30f;
@@ -198,95 +200,33 @@ cudaError_t ga_launch_preprocess(const RasterDims &d, const RasterWs &w, const f
 }
 
 // ---------------------------------------------------------------------------
-// K5: per-surfel backward, summed over the views of the batch item.
-// grad_acc: [NV*P][18] (layout in raster_common.cuh); grad_gauss13 [batch][P][13].
+// K5: per-surfel backward from the surfel's gradient row.
+// grad_rows: [batch][P][16], already summed over the views of the batch item by render_bwd, which also applied each
+// view's chain rule through T = (Tu, Tv, Tw) and the normal (layout in raster_common.cuh).  What is left depends on
+// the surfel alone.  A surfel with radii <= 0 in a view got no tiles there from K1 (its rectangle is empty), so that
+// view added nothing to its row.  grad_gauss13 [batch][P][13].
 // ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-preprocess_bwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ gauss13,
-                      const float *__restrict__ viewmats, const float *__restrict__ projmats,
-                      const int32_t *__restrict__ radii, const float *__restrict__ grad_acc,
-                      float *__restrict__ grad_gauss13)
+// One surfel: its 13 inputs at g (shared memory) are replaced by its 13 gradient columns; row = its gradient row.
+__device__ __forceinline__ void preprocess_bwd_one(const RasterDims &d, float *g, const float4 *row)
 {
-    const int b = blockIdx.y;
-    const int i = blockIdx.x * 256 + threadIdx.x;
-    if (i >= d.P) return;
-    const float *g = gauss13 + ((size_t)b * d.P + i) * 13;
     float q[4] = {g[6], g[7], g[8], g[9]};
     float R[3][3];
     quat_to_rotmat(q, R);
     const float sx = d.scale_modifier * g[4], sy = d.scale_modifier * g[5];
-    const float px = g[0], py = g[1], pz = g[2];
-    const float hw = 0.5f * d.W, hh = 0.5f * d.H, cw = 0.5f * (d.W - 1), ch = 0.5f * (d.H - 1);
-    float gm[3] = {0, 0, 0}, gs[2] = {0, 0}, dR[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}};
-    float gop = 0.f, gcol[3] = {0, 0, 0};
-    for (int v = 0; v < d.views; v++) {
-        const int view = b * d.views + v;
-        const size_t vi = (size_t)view * d.P + i;
-        if (!(radii[vi] > 0)) continue;
-        const float *ga = grad_acc + vi * GA_GRAD_F;
-        const float *vm = viewmats + view * 16, *pm = projmats + view * 16;
-        float G[3][3];
+    const float4 r0 = row[0], r1 = row[1], r2 = row[2], r3 = row[3];
+    const float dM[3][3] = {{r0.x, r0.y, r0.z}, {r0.w, r1.x, r1.y}, {r1.z, r1.w, r2.x}};
+    const float dtn[3] = {r2.y, r2.z, r2.w};
+    float gm[3], gs[2] = {0, 0}, dR[3][3];
 #pragma unroll
-        for (int c = 0; c < 3; c++)
-#pragma unroll
-            for (int r = 0; r < 3; r++) G[c][r] = ga[3 * c + r];
-        const float gmx = ga[9], gmy = ga[10];
-        if (gmx != 0.f || gmy != 0.f) {
-            const float t[3] = {9.f, 9.f, -1.f};
-            float Tu[3], Tv[3], Tw[3];
-            surfel_transmat(R, sx, sy, px, py, pz, pm, d.W, d.H, Tu, Tv, Tw);
-            float dd = 0.f;
-#pragma unroll
-            for (int r = 0; r < 3; r++) dd += t[r] * Tw[r] * Tw[r];
-            float f[3], dL_dd = 0.f;
-#pragma unroll
-            for (int r = 0; r < 3; r++) f[r] = t[r] / dd;
-#pragma unroll
-            for (int r = 0; r < 3; r++) {
-                G[0][r] += gmx * f[r] * Tw[r];
-                G[1][r] += gmy * f[r] * Tw[r];
-                G[2][r] += gmx * f[r] * Tu[r] + gmy * f[r] * Tv[r];
-                dL_dd += (gmx * Tu[r] * Tw[r] + gmy * Tv[r] * Tw[r]) * f[r];
-            }
-            dL_dd *= (-1.0f / dd);
-#pragma unroll
-            for (int r = 0; r < 3; r++) G[2][r] += dL_dd * t[r] * Tw[r] * 2.0f;
-        }
-        float dM[3][3];
-#pragma unroll
-        for (int k = 0; k < 3; k++) {
-            float an0 = pm[4 * k + 0] * hw + pm[4 * k + 3] * cw;
-            float an1 = pm[4 * k + 1] * hh + pm[4 * k + 3] * ch;
-            float an2 = pm[4 * k + 3];
-#pragma unroll
-            for (int r = 0; r < 3; r++) dM[r][k] = an0 * G[0][r] + an1 * G[1][r] + an2 * G[2][r];
-        }
-        // dual-visible sign (recomputed exactly like K1)
-        float vx = ((vm[0] * px + vm[4] * py) + vm[8] * pz) + vm[12];
-        float vy = ((vm[1] * px + vm[5] * py) + vm[9] * pz) + vm[13];
-        float vz = ((vm[2] * px + vm[6] * py) + vm[10] * pz) + vm[14];
-        float nx = (vm[0] * R[0][2] + vm[4] * R[1][2]) + vm[8] * R[2][2];
-        float ny = (vm[1] * R[0][2] + vm[5] * R[1][2]) + vm[9] * R[2][2];
-        float nz = (vm[2] * R[0][2] + vm[6] * R[1][2]) + vm[10] * R[2][2];
-        float cosv = -((vx * nx + vy * ny) + vz * nz);
-        const float mult = cosv > 0.f ? 1.f : -1.f;
-        const float gn0 = ga[11], gn1 = ga[12], gn2 = ga[13];
-        float dtn[3];
-        dtn[0] = mult * (vm[0] * gn0 + vm[1] * gn1 + vm[2] * gn2);
-        dtn[1] = mult * (vm[4] * gn0 + vm[5] * gn1 + vm[6] * gn2);
-        dtn[2] = mult * (vm[8] * gn0 + vm[9] * gn1 + vm[10] * gn2);
-#pragma unroll
-        for (int k = 0; k < 3; k++) {
-            dR[k][0] += dM[0][k] * sx;
-            dR[k][1] += dM[1][k] * sy;
-            dR[k][2] += dtn[k];
-            gs[0] += dM[0][k] * R[k][0];
-            gs[1] += dM[1][k] * R[k][1];
-            gm[k] += dM[2][k];
-        }
-        gop += ga[14];
-        gcol[0] += ga[15]; gcol[1] += ga[16]; gcol[2] += ga[17];
+    for (int k = 0; k < 3; k++) {
+        dR[k][0] = dM[0][k] * sx;
+        dR[k][1] = dM[1][k] * sy;
+        dR[k][2] = dtn[k];
+        gs[0] += dM[0][k] * R[k][0];
+        gs[1] += dM[1][k] * R[k][1];
+        gm[k] = dM[2][k];
     }
+    const float gop = r3.x, gcol[3] = {r3.y, r3.z, r3.w};
     float n2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
     float s = rsqrtf(n2);
     float w = q[0] * s, x = q[1] * s, y = q[2] * s, z = q[3] * s;
@@ -298,7 +238,7 @@ preprocess_bwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ gauss
         const float dot = w * gw + x * gxq + y * gyq + z * gzq;
         gw = (gw - w * dot) * s; gxq = (gxq - x * dot) * s; gyq = (gyq - y * dot) * s; gzq = (gzq - z * dot) * s;
     }
-    float *o = grad_gauss13 + ((size_t)b * d.P + i) * 13;
+    float *o = g;                    // the inputs are all read above; the outputs take their place
     o[0] = gm[0]; o[1] = gm[1]; o[2] = gm[2];
     o[3] = gop;
     o[4] = d.scale_modifier * gs[0]; o[5] = d.scale_modifier * gs[1];
@@ -306,13 +246,30 @@ preprocess_bwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ gauss
     o[10] = gcol[0]; o[11] = gcol[1]; o[12] = gcol[2];
 }
 
-cudaError_t ga_launch_preprocess_bwd(const RasterDims &d, const RasterWs &w, const float *gauss13,
-                                     const float *viewmats, const float *projmats,
-                                     const int32_t *radii, const float *grad_acc,
+// The CTA's 256 surfels and their 13 output columns are staged in shared memory and moved as whole lines, as in K1:
+// a thread's own 52 bytes would make every load and store instruction touch 32 different lines.
+__global__ void __launch_bounds__(256)
+preprocess_bwd_kernel(RasterDims d, const float *__restrict__ gauss13, const float *__restrict__ grad_rows,
+                      float *__restrict__ grad_gauss13)
+{
+    __shared__ float s_g[256 * 13];
+    const int b = blockIdx.y;
+    const int i0 = blockIdx.x * 256;
+    const int n = min(256, d.P - i0);
+    const size_t base = ((size_t)b * d.P + i0) * 13;
+    for (int t = threadIdx.x; t < n * 13; t += 256) s_g[t] = gauss13[base + t];
+    __syncthreads();
+    if ((int)threadIdx.x < n)
+        preprocess_bwd_one(d, s_g + threadIdx.x * 13,
+                           reinterpret_cast<const float4 *>(grad_rows + ((size_t)b * d.P + i0 + threadIdx.x) * GA_ROW_F));
+    __syncthreads();
+    for (int t = threadIdx.x; t < n * 13; t += 256) grad_gauss13[base + t] = s_g[t];
+}
+
+cudaError_t ga_launch_preprocess_bwd(const RasterDims &d, const float *gauss13, const float *grad_rows,
                                      float *grad_gauss13, cudaStream_t s)
 {
     dim3 grid((d.P + 255) / 256, d.batch);
-    preprocess_bwd_kernel<<<grid, 256, 0, s>>>(d, w, gauss13, viewmats, projmats, radii, grad_acc,
-                                               grad_gauss13);
+    preprocess_bwd_kernel<<<grid, 256, 0, s>>>(d, gauss13, grad_rows, grad_gauss13);
     return cudaGetLastError();
 }

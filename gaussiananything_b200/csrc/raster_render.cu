@@ -14,7 +14,7 @@
 //    evaluating every (pixel, surfel) pair.
 //  * the backward walks each tile back to front, keeps the per-(pixel, surfel)
 //    records in shared memory, accumulates each surfel's gradient in registers
-//    and issues one global atomic per (tile, surfel, component).
+//    and adds it to the surfel's gradient row with vector reductions.
 #include "raster_common.cuh"
 #include "device_once.cuh"
 
@@ -89,7 +89,7 @@ __device__ __forceinline__ TileBox clip_box(const float4 bb, int ox, int oy, int
 // which is upstream's cross(k, l) re-associated around the tile origin (all
 // terms stay O(tile size), so no precision is lost) and costs 6 FMAs per pixel.
 //  rec[0] = C.x C.y C.z A.x | rec[1] = A.y A.z B.x B.y | rec[2] = B.z Tw.x Tw.y Tw.z
-//  rec[3] = xy.x-o.x xy.y-o.y opacity - | rec[4] = n.x n.y n.z r | rec[5] = g b - -
+//  rec[3] = xy.x-o.x xy.y-o.y opacity - | rec[4] = n.x n.y n.z r | rec[5] = g b sign -
 //
 // The tile's instances are staged in chunks of 256 list positions.  Each slot also gets its cull box clipped to the
 // tile's pixels inside the image (origin, width, a reciprocal for the division by the width) and its pair count
@@ -504,8 +504,10 @@ cudaError_t ga_launch_render_fwd(const RasterDims &d, const RasterWs &w, const f
 //     warp get instances of similar length, are walked by BWD_TPI lanes each; they re-derive the ray-splat geometry
 //     of every record with eval_pair() (upstream's cross(k, l) at the pixel; the forward's phase 1 evaluates the
 //     tile-origin form instead, so the bits can differ in the last place), accumulate the 18 gradient components in
-//     registers, reduce-scatter them over the lanes and add them to grad_acc: one global atomic per (tile, instance,
-//     non-zero component).
+//     registers, map them through the view's chain rule to the 16 floats of the surfel's gradient row (grad_row()),
+//     reduce-scatter those over the lanes and add them to the row: one 16-byte vector reduction per (tile, instance,
+//     four components).  The views of a batch item share the rows ([batch][P][16]), so the backward zeroes and K5
+//     reads 6.4 MB on C2 instead of the 43 MB of one 18-float row per view and surfel.
 // The records never leave the SM.  Tiles whose lists overflowed (and callers with list_k == 0) take the recompute
 // path of the same launch.
 // ---------------------------------------------------------------------------
@@ -532,79 +534,77 @@ struct BwdSmem {
     uint16_t perm[CHUNK];
     int wsum[8];
     int maxc, m;
+    // the CTA's view: A[k][c] at 3k+c, the 3x3 that maps dL/dT to dL/dM (see bwd_tile), then the view rotation
+    // R[k][j] = viewmat[4k+j] at 9+3k+j
+    float view[18];
 };
 
-// reduce-scatter of 18 components over TPI (2/4/8/16) consecutive lanes by recursive halving: after level l a lane
-// is responsible for half of the components it held before; the fully reduced leftovers are added to dst.
-template <int TPI>
-__device__ __forceinline__ void reduce_scatter18(const float (&g)[GA_GRAD_F], int lane, float *__restrict__ dst)
+// One view's chain rule, applied to the GA_GRAD_F components g that phase B summed over one instance's records: the
+// mean-2D term folded into dL/dT, then dL/dM = A dL/dT and the normal's dL/dR column 2 = sign R^T dL/dnormal, into
+// the surfel's gradient row o (GA_ROW_F, layout in raster_common.cuh).  The map is linear in g and depends only on
+// the view and on the record, so the sum of the transformed partials over tiles and views is the transform of the
+// per-view sums.  Tu = a.xyz, Tv = (a.w, b.x, b.y), Tw = (b.z, b.w, c.x); vc = the view's A and R (BwdSmem::view).
+__device__ __forceinline__ void grad_row(float (&g)[GA_GRAD_F], const float4 a, const float4 b, const float4 c,
+                                         float sign, const float *vc, float (&o)[GA_ROW_F])
 {
-    int off = 0, size = 9;
-    float a9[10];
-    {
-        const bool u = lane & (TPI >> 1);
+    const float Tu[3] = {a.x, a.y, a.z}, Tv[3] = {a.w, b.x, b.y}, Tw[3] = {b.z, b.w, c.x};
+    const float gmx = g[9], gmy = g[10];
+    if (gmx != 0.f || gmy != 0.f) {
+        // mean2D = (Tu . t Tw, Tv . t Tw) / (Tw . t Tw) with t = (9, 9, -1), K1's cutoff^2 weights
+        const float t[3] = {9.f, 9.f, -1.f};
+        float dd = 0.f;
 #pragma unroll
-        for (int i = 0; i < 9; i++) {
-            const float keep = u ? g[9 + i] : g[i], send = u ? g[i] : g[9 + i];
-            a9[i] = keep + __shfl_xor_sync(0xffffffffu, send, TPI >> 1);
+        for (int r = 0; r < 3; r++) dd += t[r] * Tw[r] * Tw[r];
+        const float idd = fast_rcp(dd);
+        float dL_dd = 0.f;
+#pragma unroll
+        for (int r = 0; r < 3; r++) {
+            const float f = t[r] * idd, u = gmx * Tu[r] + gmy * Tv[r];
+            g[r] += gmx * f * Tw[r];
+            g[3 + r] += gmy * f * Tw[r];
+            g[6 + r] += f * u;
+            dL_dd += u * Tw[r] * f;
         }
-        a9[9] = 0.f;
-        off += u ? 9 : 0;
+        dL_dd *= -idd;
+#pragma unroll
+        for (int r = 0; r < 3; r++) g[6 + r] += 2.0f * dL_dd * t[r] * Tw[r];
     }
-    if constexpr (TPI == 2) {
 #pragma unroll
-        for (int i = 0; i < 9; i++)
-            if (a9[i] != 0.f) atomicAdd(dst + off + i, a9[i]);
-        return;
-    } else {
-        float b5[6];
-        {
-            const bool u = lane & (TPI >> 2);
+    for (int r = 0; r < 3; r++)
 #pragma unroll
-            for (int i = 0; i < 5; i++) {
-                const float keep = u ? a9[5 + i] : a9[i], send = u ? a9[i] : a9[5 + i];
-                b5[i] = keep + __shfl_xor_sync(0xffffffffu, send, TPI >> 2);
-            }
-            b5[5] = 0.f;
-            off += u ? 5 : 0; size = u ? 4 : 5;
+        for (int k = 0; k < 3; k++) o[3 * r + k] = vc[3 * k] * g[r] + vc[3 * k + 1] * g[3 + r] + vc[3 * k + 2] * g[6 + r];
+#pragma unroll
+    for (int k = 0; k < 3; k++) o[9 + k] = sign * (vc[9 + 3 * k] * g[11] + vc[10 + 3 * k] * g[12] + vc[11 + 3 * k] * g[13]);
+#pragma unroll
+    for (int f = 0; f < 4; f++) o[12 + f] = g[14 + f];
+}
+
+// reduce-scatter of a gradient row over TPI (2 or 4) consecutive lanes by recursive halving: at each level a lane
+// keeps half of the components it held, summed with its partner's; the GA_ROW_F / TPI fully reduced components are
+// added to dst (16-byte aligned) with 16-byte vector reductions, skipping groups of four zeros.  On C2 (H100 SXM,
+// 700 W) the vector reductions made render_bwd 37 us shorter than one scalar atomic per non-zero component: the
+// transform mixes the components, so a row has few zeros left to skip (profiles/raster_grad_rows_h100.md).
+template <int TPI>
+__device__ __forceinline__ void reduce_scatter_row(float (&g)[GA_ROW_F], int lane, float *__restrict__ dst)
+{
+    static_assert((TPI == 2 || TPI == 4) && GA_ROW_F % (4 * TPI) == 0, "TPI: 2 or 4 lanes, whole float4 per lane");
+    int off = 0;
+#pragma unroll
+    for (int s = TPI >> 1; s >= 1; s >>= 1) {
+        const int h = GA_ROW_F * s / TPI;
+        const bool u = lane & s;
+#pragma unroll
+        for (int i = 0; i < h; i++) {
+            const float keep = u ? g[h + i] : g[i], send = u ? g[i] : g[h + i];
+            g[i] = keep + __shfl_xor_sync(0xffffffffu, send, s);
         }
-        if constexpr (TPI == 4) {
-#pragma unroll
-            for (int i = 0; i < 5; i++)
-                if (i < size && b5[i] != 0.f) atomicAdd(dst + off + i, b5[i]);
-            return;
-        } else {
-            float c3[4];
-            {
-                const bool u = lane & (TPI >> 3);
-#pragma unroll
-                for (int i = 0; i < 3; i++) {
-                    const float keep = u ? b5[3 + i] : b5[i], send = u ? b5[i] : b5[3 + i];
-                    c3[i] = keep + __shfl_xor_sync(0xffffffffu, send, TPI >> 3);
-                }
-                c3[3] = 0.f;
-                off += u ? 3 : 0; size = u ? size - 3 : 3;
-            }
-            if constexpr (TPI == 8) {
-#pragma unroll
-                for (int i = 0; i < 3; i++)
-                    if (i < size && c3[i] != 0.f) atomicAdd(dst + off + i, c3[i]);
-                return;
-            } else {
-                const bool u = lane & (TPI >> 4);
-                float d2[2];
-#pragma unroll
-                for (int i = 0; i < 2; i++) {
-                    const float keep = u ? c3[2 + i] : c3[i], send = u ? c3[i] : c3[2 + i];
-                    d2[i] = keep + __shfl_xor_sync(0xffffffffu, send, TPI >> 4);
-                }
-                off += u ? 2 : 0; size = u ? max(size - 2, 0) : min(size, 2);
-#pragma unroll
-                for (int i = 0; i < 2; i++)
-                    if (i < size && d2[i] != 0.f) atomicAdd(dst + off + i, d2[i]);
-            }
-        }
+        off += u ? h : 0;
     }
+#pragma unroll
+    for (int i = 0; i < GA_ROW_F / TPI; i += 4)
+        if (g[i] != 0.f || g[i + 1] != 0.f || g[i + 2] != 0.f || g[i + 3] != 0.f)
+            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + off + i), "f"(g[i]), "f"(g[i + 1]),
+                         "f"(g[i + 2]), "f"(g[i + 3]) : "memory");
 }
 
 __device__ __forceinline__ int clipped_box_area(const float4 bb, int ox, int oy)
@@ -618,8 +618,9 @@ __device__ __forceinline__ int clipped_box_area(const float4 bb, int ox, int oy)
 // surfels that do not reach alpha >= 1/255 at the pixel.  LISTS = false culls and re-evaluates every staged surfel.
 template <bool LISTS>
 __device__ __forceinline__ void bwd_tile(const RasterDims &d, const RasterWs &ws, BwdSmem &sm, const float *__restrict__ bg,
+                                         const float *__restrict__ viewmats, const float *__restrict__ projmats,
                                          const float *__restrict__ dL_dcolor, const float *__restrict__ dL_dallmap,
-                                         float *__restrict__ grad_acc)
+                                         float *__restrict__ grad_rows)
 {
     const int view = blockIdx.z;
     const int tile = blockIdx.y * d.gx + blockIdx.x;
@@ -638,7 +639,7 @@ __device__ __forceinline__ void bwd_tile(const RasterDims &d, const RasterWs &ws
     const float *fT = ws.final_T + (size_t)view * 3 * HW;
     const int32_t *nc = ws.n_contrib + (size_t)view * 2 * HW;
     const float *rec_base = ws.rec + (size_t)view * d.P * GA_REC_F;
-    float *acc_base = grad_acc + (size_t)view * d.P * GA_GRAD_F;
+    float *row_base = grad_rows + (size_t)(view / d.views) * d.P * GA_ROW_F;
 
     const float T_final = inside ? fT[pix] : 0.f;
     float T = T_final;
@@ -678,6 +679,19 @@ __device__ __forceinline__ void bwd_tile(const RasterDims &d, const RasterWs &ws
 
     // nothing behind the deepest contributor of the tile can receive gradient
     if (threadIdx.x == 0) sm.maxc = 0;
+    if (threadIdx.x < 9) {
+        // K1 builds T_c[r] = sum_k M[r][k] A[k][c] + const (c = u, v, w; M's rows are sx R[:,0], sy R[:,1] and the
+        // position), so dL/dM[r][k] = sum_c A[k][c] dL/dT_c[r].  Each product rounded on its own, as K1 rounds them.
+        const float *pm = projmats + (size_t)view * 16;
+        const int k = threadIdx.x / 3, c = threadIdx.x % 3;
+        const float hw = 0.5f * d.W, hh = 0.5f * d.H, cw = 0.5f * (d.W - 1), ch = 0.5f * (d.H - 1);
+        sm.view[threadIdx.x] = c == 0 ? __fadd_rn(__fmul_rn(pm[4 * k], hw), __fmul_rn(pm[4 * k + 3], cw))
+                             : c == 1 ? __fadd_rn(__fmul_rn(pm[4 * k + 1], hh), __fmul_rn(pm[4 * k + 3], ch))
+                                      : pm[4 * k + 3];
+    } else if (threadIdx.x < 18) {
+        const int k = (threadIdx.x - 9) / 3, j = (threadIdx.x - 9) % 3;
+        sm.view[threadIdx.x] = viewmats[(size_t)view * 16 + 4 * k + j];
+    }
     __syncthreads();
     {
         int mc = last_contributor;
@@ -833,10 +847,13 @@ __device__ __forceinline__ void bwd_tile(const RasterDims &d, const RasterWs &ws
                 const int slot = b0 + (int)threadIdx.x / BWD_TPI;
                 const int jj = slot < m ? (int)sm.perm[slot] : 0;
                 const int n = slot < m ? sm.cnt[jj] : 0;
-                float g[GA_GRAD_F];
+                float o[GA_ROW_F];
 #pragma unroll
-                for (int f = 0; f < GA_GRAD_F; f++) g[f] = 0.f;
+                for (int f = 0; f < GA_ROW_F; f++) o[f] = 0.f;
                 if (n > 0) {
+                    float g[GA_GRAD_F];
+#pragma unroll
+                    for (int f = 0; f < GA_GRAD_F; f++) g[f] = 0.f;
                     const float4 a = sm.rec[0][jj], b = sm.rec[1][jj], c = sm.rec[2][jj];
                     const float opa = c.w;
                     const uint4 *lst = sm.recs + (sm.off[jj] - base);
@@ -873,10 +890,11 @@ __device__ __forceinline__ void bwd_tile(const RasterDims &d, const RasterWs &ws
                         g[15] += w * ua.x; g[16] += w * ua.y; g[17] += w * ua.z;
                         g[11] += w * ua.w; g[12] += w * ub.x; g[13] += w * ub.y;
                     }
+                    grad_row(g, a, b, c, sm.rec[5][jj].z, sm.view, o);
                 }
                 // all lanes of the warp take part in the shuffles; lanes without records carry zeros (adds skipped)
                 if (__any_sync(0xffffffffu, n > 0))
-                    reduce_scatter18<BWD_TPI>(g, lane, acc_base + (size_t)(n > 0 ? sm.id[jj] : 0) * GA_GRAD_F);
+                    reduce_scatter_row<BWD_TPI>(o, lane, row_base + (size_t)(n > 0 ? sm.id[jj] : 0) * GA_ROW_F);
             }
             t0 = t1;
             if (t0 < cnt) base = sm.off[t0];
@@ -886,20 +904,22 @@ __device__ __forceinline__ void bwd_tile(const RasterDims &d, const RasterWs &ws
 }
 
 __global__ void __launch_bounds__(256, 2)
-render_bwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg, const float *__restrict__ dL_dcolor,
-                  const float *__restrict__ dL_dallmap, float *__restrict__ grad_acc)
+render_bwd_kernel(RasterDims d, RasterWs ws, const float *__restrict__ bg, const float *__restrict__ viewmats,
+                  const float *__restrict__ projmats, const float *__restrict__ dL_dcolor,
+                  const float *__restrict__ dL_dallmap, float *__restrict__ grad_rows)
 {
     extern __shared__ __align__(16) uint8_t bwd_smem_raw[];
     BwdSmem &sm = *reinterpret_cast<BwdSmem *>(bwd_smem_raw);
     if (ws.status[1]) return;
     if (d.list_k > 0 && ws.tile_flag[(size_t)blockIdx.z * d.T + blockIdx.y * d.gx + blockIdx.x] == 0)
-        bwd_tile<true>(d, ws, sm, bg, dL_dcolor, dL_dallmap, grad_acc);
+        bwd_tile<true>(d, ws, sm, bg, viewmats, projmats, dL_dcolor, dL_dallmap, grad_rows);
     else
-        bwd_tile<false>(d, ws, sm, bg, dL_dcolor, dL_dallmap, grad_acc);
+        bwd_tile<false>(d, ws, sm, bg, viewmats, projmats, dL_dcolor, dL_dallmap, grad_rows);
 }
 
 cudaError_t ga_launch_render_bwd(const RasterDims &d, const RasterWs &w, const float *bg,
-                                 const float *dL_dcolor, const float *dL_dallmap, float *grad_acc, cudaStream_t s)
+                                 const float *viewmats, const float *projmats,
+                                 const float *dL_dcolor, const float *dL_dallmap, float *grad_rows, cudaStream_t s)
 {
     static GaPerDevice attr_set;
     if (ga_first_use_on_device(attr_set)) {
@@ -908,6 +928,6 @@ cudaError_t ga_launch_render_bwd(const RasterDims &d, const RasterWs &w, const f
         if (e != cudaSuccess) return e;
     }
     dim3 grid(d.gx, d.gy, d.NV);
-    render_bwd_kernel<<<grid, 256, sizeof(BwdSmem), s>>>(d, w, bg, dL_dcolor, dL_dallmap, grad_acc);
+    render_bwd_kernel<<<grid, 256, sizeof(BwdSmem), s>>>(d, w, bg, viewmats, projmats, dL_dcolor, dL_dallmap, grad_rows);
     return cudaGetLastError();
 }

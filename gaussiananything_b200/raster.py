@@ -137,9 +137,9 @@ _scratch_pool = {}
 
 
 def _take_scratch(dev, nbytes):
-    """The backward's scratch (the gradient accumulators, 43 MB at 100k surfels x 6 views) is only live inside one
-    backward call, so it is kept per (device, stream, size) instead of going through the caching allocator every
-    step: large blocks allocated and freed alternately make the allocator split / re-grow its segments, i.e. an
+    """The backward's scratch (43 MB at 100k surfels x 6 views; its first 6.4 MB hold the gradient rows) is only live
+    inside one backward call, so it is kept per (device, stream, size) instead of going through the caching allocator
+    every step: large blocks allocated and freed alternately make the allocator split / re-grow its segments, i.e. an
     occasional synchronising cudaMalloc in the middle of a training step."""
     key = (dev.index, torch.cuda.current_stream(dev).cuda_stream, nbytes)
     pool = _scratch_pool.setdefault(key, [])

@@ -31,7 +31,8 @@ extern "C" {
 #define GA_ERR_SIZE     (-3)    /* image larger than 4080 px or P*views overflow */
 
 #define GA_RASTER_REC_FLOATS 24   /* packed per-(view,surfel) record, 96 bytes */
-#define GA_RASTER_GRAD_FLOATS 18  /* per-(view,surfel) gradient accumulator */
+#define GA_RASTER_GRAD_FLOATS 18  /* per (view, surfel): sizes the backward's scratch, see ga_raster_backward_scratch_bytes */
+#define GA_RASTER_ROW_FLOATS 16   /* per (batch item, surfel): the backward's gradient row, summed over the views */
 
 /* Byte offsets of the sections inside the forward workspace.  The forward
  * pass fills them; the backward pass reads them (the workspace is the
@@ -39,7 +40,7 @@ extern "C" {
 typedef struct GaRasterLayout {
     size_t total_bytes;
     size_t status;      /* int32[16]: [0]=instances D, [1]=overflow flag, [2]=tiles above 4096 instances (sorted in global memory), [3]=tiles above 512 */
-    size_t rec;         /* float[NV*P][24]  Tu3 Tv3 Tw3 | xy2 opacity | normal3 | r | bbox x0 x1 y0 y1 | g b - - */
+    size_t rec;         /* float[NV*P][24]  Tu3 Tv3 Tw3 | xy2 opacity | normal3 | r | bbox x0 x1 y0 y1 | g b sign - */
     size_t depth;       /* float[NV*P]      view-space z (0 when culled) */
     size_t rect;        /* uint32[NV*P]     x0 | y0<<8 | x1<<16 | y1<<24 (tile units) */
     size_t tile_count;  /* uint32[NV*T*9]   scratch: per-tile counters, then fill cursors (8 replicas per tile); then the list of tiles above 512 instances */
@@ -92,15 +93,18 @@ int ga_raster_forward_ex(const float *gauss13, int batch, int P, int views,
                          void *workspace, size_t workspace_bytes, int64_t max_instances, int list_k,
                          int32_t *status_host, void *status_event, void *stream);
 
-/* Bytes of scratch the backward wants: the gradient accumulators [NV*P][18].  A larger buffer is accepted; the
- * rest of it is not used. */
+/* Bytes of scratch the backward wants: NV*P*GA_RASTER_GRAD_FLOATS floats.  Only the leading
+ * batch*P*GA_RASTER_ROW_FLOATS floats are used (zeroed, then summed into); a larger buffer is accepted and the rest
+ * of it is not touched. */
 size_t ga_raster_backward_scratch_bytes(int batch, int P, int views);
 
 /*
  * Backward.  dL_dcolor [NV][3][H][W], dL_dallmap [NV][7][H][W]; grad_gauss13
  * [batch][P][13] is OVERWRITTEN with the gradient summed over the views of
  * each batch item (same column order as gauss13).  workspace and list_k must
- * be the ones the matching ga_raster_forward_ex filled and used.
+ * be the ones the matching ga_raster_forward_ex filled and used.  scratch must
+ * be 16-byte aligned.  radii is the forward's out_radii; it must not be NULL,
+ * but the gradient does not depend on it.
  */
 int ga_raster_backward_ex(const float *gauss13, int batch, int P, int views,
                           const float *viewmats, const float *projmats, const float *bg,
