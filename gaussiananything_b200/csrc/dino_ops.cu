@@ -9,6 +9,7 @@
 // Math follows /root/reference/sgm/modules/encoders/modules.py:862-875 and the DINOv2 token preparation; the checker
 // is oracle/dino_oracle.py.  The front end runs in fp32 whatever the caller's image dtype.
 #include "../../include/ga_b200.h"
+#include "row_common.cuh"
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -218,6 +219,8 @@ extern "C" int ga_dino_tokens(const float *patch_out, const float *cls_token, co
     if (!patch_out || !cls_token || !pos_embed || !x || batch <= 0 || n_patch <= 0 || n_reg < 0 || D <= 0 || D % 4)
         return GA_ERR_BADARG;
     if (n_reg > 0 && !reg_tokens) return GA_ERR_BADARG;
+    using ga_row::mis16;
+    if (mis16(patch_out) || mis16(cls_token) || mis16(reg_tokens) || mis16(pos_embed) || mis16(x)) return GA_ERR_BADARG;
     const int D4 = D / 4;
     const long long total = (long long)batch * (1 + n_reg + n_patch) * D4;
     tokens_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(

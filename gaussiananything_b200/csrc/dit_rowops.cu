@@ -361,7 +361,8 @@ extern "C" int ga_rmsnorm_modulate(const float *x, const float *w, const float *
                                    void *stream)
 {
     if (!x || !w || !out_bf16 || R <= 0 || D <= 0 || D % 4 || rows_per_batch <= 0) return GA_ERR_BADARG;
-    if ((shift == nullptr) != (scale == nullptr)) return GA_ERR_BADARG;
+    if ((shift == nullptr) != (scale == nullptr) || (shift && mod_ld % 4)) return GA_ERR_BADARG;
+    if (mis16(x) || mis16(w) || mis16(shift) || mis16(scale) || mis8(out_bf16)) return GA_ERR_BADARG;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((R + 7) / 8); cfg.blockDim = dim3(256); cfg.stream = (cudaStream_t)stream;
     cudaLaunchAttribute attr[1];
@@ -378,6 +379,8 @@ extern "C" int ga_linear_small(const float *x, const float *W, const float *bias
                                int act_in, int act_out, int accumulate, void *stream)
 {
     if (!x || !W || !y || rows <= 0 || rows > 16 || N <= 0 || K <= 0) return GA_ERR_BADARG;
+    if ((act_in != 0 && act_in != 1) || (act_out != 0 && act_out != 1)) return GA_ERR_BADARG;
+    if ((K & 127) == 0 && K <= 1024 && (mis16(x) || mis16(W))) return GA_ERR_BADARG;         // the prefetch path
     linear_small_kernel<<<(N + 7) / 8, 256, 0, (cudaStream_t)stream>>>(x, W, bias, y, rows, N, K, act_in, act_out,
                                                                        accumulate);
     return last_err();
@@ -393,7 +396,8 @@ extern "C" int ga_timestep_sinusoid(const float *t, float *out, int rows, int di
 extern "C" int ga_layernorm_rows(const float *x, const float *w, const float *b, float *y, int R, int D, float eps,
                                  void *stream)
 {
-    if (!x || !y || R <= 0 || D <= 0) return GA_ERR_BADARG;
+    if (!x || !y || R <= 0 || D <= 0 || (b && !w)) return GA_ERR_BADARG;
+    if (D % 4 == 0 && D <= kMaxD && (mis16(x) || mis16(w) || mis16(b) || mis16(y))) return GA_ERR_BADARG;
     layernorm_rows_kernel<<<(R + 7) / 8, 256, 0, (cudaStream_t)stream>>>(x, w, b, y, R, D, eps);
     return last_err();
 }
@@ -411,7 +415,7 @@ extern "C" int ga_add_tables(const float *tables, const float *t0, float *mod, i
 extern "C" int ga_embed_fc1(const float *xin, int Cx, const float *xin2, int C2, const float *W1, const float *b1,
                             void *h_bf16, int R, int D, void *stream)
 {
-    if (!xin || !W1 || !b1 || !h_bf16 || R <= 0 || D <= 0 || Cx <= 0 || (C2 > 0 && !xin2)) return GA_ERR_BADARG;
+    if (!xin || !W1 || !b1 || !h_bf16 || R <= 0 || D <= 0 || Cx <= 0 || C2 < 0 || (C2 > 0 && !xin2)) return GA_ERR_BADARG;
     const size_t total = (size_t)R * D;
     embed_fc1_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
         xin, Cx, xin2, C2, W1, b1, reinterpret_cast<__nv_bfloat16 *>(h_bf16), R, D);
@@ -428,7 +432,9 @@ extern "C" int ga_xyz_posenc(const float *xyz, void *out_bf16, int R, void *stre
 extern "C" int ga_final_layer(const float *x, const float *mod, const float *W, const float *bias, float *y, int R,
                               int D, int Cout, int rows_per_batch, float eps, void *stream)
 {
-    if (!x || !mod || !W || !bias || !y || R <= 0 || D <= 0 || Cout <= 0 || Cout > 16) return GA_ERR_BADARG;
+    if (!x || !mod || !W || !bias || !y || R <= 0 || D <= 0 || Cout <= 0 || Cout > 16 || rows_per_batch <= 0)
+        return GA_ERR_BADARG;
+    if (D % 4 == 0 && D <= kMaxD && (mis16(x) || mis16(mod) || mis16(W))) return GA_ERR_BADARG;
     final_layer_kernel<<<(R + 7) / 8, 256, 0, (cudaStream_t)stream>>>(x, mod, W, bias, y, R, D, Cout, rows_per_batch,
                                                                       eps);
     return last_err();

@@ -243,6 +243,7 @@ __global__ void heads32_kernel(const __nv_bfloat16 *__restrict__ qkv, const floa
 // logvar = 20 tanh(logvar / 20), std = exp(logvar / 2), latent = mean + std * eps.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int kHeadThreads = 256;
+constexpr int kHeadRed = kHeadThreads / 32;        // block_sum's static shared floats
 
 __device__ __forceinline__ float block_sum(float v, float *red)
 {
@@ -276,7 +277,7 @@ __global__ void __launch_bounds__(kHeadThreads) readout_head_kernel(const GaVaeE
 {
     extern __shared__ float sh[];
     float *xn = sh, *hv = sh + D, *m = hv + hid, *q1 = m + 2 * zc, *q2 = q1 + 2 * zc;
-    __shared__ float red[kHeadThreads / 32];
+    __shared__ float red[kHeadRed];
     const size_t r = blockIdx.x;
     const float *xr = x + r * D;
     float s = 0.f;
@@ -400,10 +401,11 @@ extern "C" int ga_vae_enc_input(const float *img, int n, int C, int H, int W, in
                                 int step, int off, float *token_xyz, void *stream)
 {
     if (!img || !x_bf16 || n <= 0 || C <= 0 || H <= 0 || W <= 0 || c_pad < C || c_pad % 8) return GA_ERR_BADARG;
+    if (reinterpret_cast<uintptr_t>(x_bf16) & 3) return GA_ERR_BADARG;                  // __nv_bfloat162 stores
+    if (token_xyz && (xyz_c < 0 || xyz_c + 3 > C || step <= 0 || off < 0 || off >= H || off >= W)) return GA_ERR_BADARG;
     cudaStream_t s = (cudaStream_t)stream;
     pack_input_kernel<<<1024, 256, 0, s>>>(img, n, C, H, W, c_pad, reinterpret_cast<__nv_bfloat16 *>(x_bf16));
     if (token_xyz) {
-        if (xyz_c < 0 || xyz_c + 3 > C || step <= 0 || off < 0 || off >= H || off >= W) return GA_ERR_BADARG;
         const int Ht = (H - off + step - 1) / step, Wt = (W - off + step - 1) / step;
         token_xyz_kernel<<<256, 256, 0, s>>>(img, n, C, H, W, xyz_c, step, off, Ht, Wt, token_xyz);
     }
@@ -427,8 +429,9 @@ extern "C" int ga_vae_enc_head(const GaVaeEncHead *p, const float *x, const floa
 {
     if (!p || !x || !h_out || !mean || !logvar || R <= 0 || D <= 0 || hid <= 0 || zc <= 0) return GA_ERR_BADARG;
     if (!p->ln_w || !p->ln_b || !p->fc1_w || !p->fc2_w || !p->q1_w || !p->q2_w) return GA_ERR_BADARG;
+    // the launch fails unless static + dynamic shared memory fit the default 48 KiB per block
     const size_t smem = (size_t)(D + hid + 6 * zc) * sizeof(float);
-    if (smem > 48 * 1024) return GA_ERR_SIZE;
+    if (smem + kHeadRed * sizeof(float) > 48 * 1024) return GA_ERR_SIZE;
     readout_head_kernel<<<R, kHeadThreads, smem, (cudaStream_t)stream>>>(*p, x, noise, D, hid, zc, h_out, mean, logvar, stdv,
                                                                          latent);
     return (int)cudaGetLastError();

@@ -474,6 +474,7 @@ extern "C" int ga_layernorm_modulate(const float *x, const float *w, const float
 {
     if (!x || !out_bf16 || R <= 0 || !row_ok(D) || (bias && !w) || ((shift == nullptr) != (scale == nullptr))) return GA_ERR_BADARG;
     if (shift && (rows_per_batch <= 0 || (mod_ld & 3))) return GA_ERR_BADARG;
+    if (mis16(x) || mis16(w) || mis16(bias) || mis16(shift) || mis16(scale) || mis8(out_bf16)) return GA_ERR_BADARG;
     layernorm_modulate_kernel<<<(R + 7) / 8, 256, 0, (cudaStream_t)stream>>>(
         x, w, bias, shift, scale, mod_ld, rows_per_batch > 0 ? rows_per_batch : 1, reinterpret_cast<__nv_bfloat16 *>(out_bf16), R,
         D, eps);
@@ -484,6 +485,7 @@ extern "C" int ga_thin_linear(const float *x, const float *ln_w, const float *ln
                               const float *bias, float *y, int R, int D, int C, float eps, void *stream)
 {
     if (!x || !W || !y || R <= 0 || !row_ok(D) || C <= 0 || C > 16 || (ln_b && !ln_w)) return GA_ERR_BADARG;
+    if (mis16(x) || mis16(ln_w) || mis16(ln_b) || mis16(W)) return GA_ERR_BADARG;
     thin_linear_kernel<<<(R + 8 * THIN_ROWS - 1) / (8 * THIN_ROWS), 256, 0, (cudaStream_t)stream>>>(x, ln_w, ln_b, apply_silu, W, bias, y, R, D, C, eps);
     return last_err();
 }
@@ -521,6 +523,7 @@ extern "C" int ga_micro_seq_build(const float *parents, int prev_f, const float 
 {
     if (!parents || !queries || !seq || S <= 0 || f <= 0 || prev_f < 0 || !row_ok(D)) return GA_ERR_BADARG;
     if (prev_f > 0 && S % prev_f) return GA_ERR_BADARG;
+    if (mis16(parents) || mis16(queries) || mis16(seq)) return GA_ERR_BADARG;
     const long long total = S * (1 + f) * (D >> 2);
     micro_seq_build_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(parents, prev_f, queries, seq, S,
                                                                                             f, D);

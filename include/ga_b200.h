@@ -217,23 +217,30 @@ int ga_attention_validate(const void *Q, const void *K, const void *Vt, const vo
                           int Nq, int Nk, int pitch_q, int pitch_k, int causal);
 
 /* out_bf16[r,:] = RMSNorm(x[r,:]; eps) * w [* (1 + scale[b,:]) + shift[b,:]], b = r / rows_per_batch;
- * shift/scale both NULL or both set, rows mod_ld apart. */
+ * shift/scale both NULL or both set, rows mod_ld apart (mod_ld % 4 == 0).  D % 4 == 0; x, w, shift, scale 16-byte
+ * and out_bf16 8-byte aligned (GA_ERR_BADARG otherwise). */
 int ga_rmsnorm_modulate(const float *x, const float *w, const float *shift, const float *scale,
                         int mod_ld, int rows_per_batch, void *out_bf16, int R, int D, float eps, void *stream);
 
-/* y[b,n] (+)= act_out(bias[n] + sum_k act_in(x[b,k]) W[n,k]);  rows <= 16; act: 0 none, 1 SiLU. */
+/* y[b,n] (+)= act_out(bias[n] + sum_k act_in(x[b,k]) W[n,k]);  rows <= 16; act: 0 none, 1 SiLU (other codes
+ * GA_ERR_BADARG).  SiLU is applied to the sum, then y's old value added.  When K % 128 == 0 and K <= 1024, x and W
+ * must be 16-byte aligned. */
 int ga_linear_small(const float *x, const float *W, const float *bias, float *y, int rows, int N, int K,
                     int act_in, int act_out, int accumulate, void *stream);
+/* out[r] = [cos(t[r] f_i) | sin(t[r] f_i)], f_i = exp(-ln(1e4) i / (dim / 2)), i < dim / 2; dim even, <= 2048 */
 int ga_timestep_sinusoid(const float *t, float *out, int rows, int dim, void *stream);
+/* y[r] = LayerNorm(x[r]; eps) [* w [+ b]], fp32; b needs w.  When D % 4 == 0 and D <= 1024, x, w, b and y must be
+ * 16-byte aligned. */
 int ga_layernorm_rows(const float *x, const float *w, const float *b, float *y, int R, int D, float eps, void *stream);
 /* mod[l,b,e] = tables[l,e] + t0[b, e % t0_ld], e in [0, JD) */
 int ga_add_tables(const float *tables, const float *t0, float *mod, int L, int rows, int JD, int t0_ld, void *stream);
-/* h = gelu_tanh(W1 [xin2 | xin] + b1) -> bf16 [R, D] (token embedder, first layer) */
+/* h = gelu_tanh(W1 [xin2 | xin] + b1) -> bf16 [R, D] (token embedder, first layer); Cx > 0, C2 >= 0 */
 int ga_embed_fc1(const float *xin, int Cx, const float *xin2, int C2, const float *W1, const float *b1,
                  void *h_bf16, int R, int D, void *stream);
 /* NeRF positional encoding of xyz (63 features, padded to 64) -> bf16 [R, 64] */
 int ga_xyz_posenc(const float *xyz, void *out_bf16, int R, void *stream);
-/* y[r,c] = bias[c] + sum_d (LayerNorm(x[r])[d] (1 + scale[b,d]) + shift[b,d]) W[c,d]; mod [B,2,D]; Cout <= 16 */
+/* y[r,c] = bias[c] + sum_d (LayerNorm(x[r])[d] (1 + scale[b,d]) + shift[b,d]) W[c,d]; mod [B,2,D]; Cout <= 16;
+ * b = r / rows_per_batch, rows_per_batch > 0.  When D % 4 == 0 and D <= 1024, x, mod and W must be 16-byte aligned. */
 int ga_final_layer(const float *x, const float *mod, const float *W, const float *bias, float *y, int R,
                    int D, int Cout, int rows_per_batch, float eps, void *stream);
 /* eps [2*half] = (cond | uncond) -> h = u + s (c - u) written to both halves of out */
@@ -245,10 +252,12 @@ int ga_f32_to_bf16(const float *x, void *y, int64_t n, void *stream);
  * Replaces the elementwise / small-matrix torch ops of /root/reference/vit/vit_triplane.py:287-345,991-1064,1289-1313,
  * 1388-1440, /root/reference/dit/dit_decoder.py:15-42 and /root/reference/nsr/srt/layers.py:82-90,146-186. */
 /* out_bf16[r] = LayerNorm(x[r]) [* w + bias] [* (1 + scale[b]) + shift[b]], b = r / rows_per_batch (1 = per token);
- * D % 4 == 0, D <= 1024 */
+ * D % 4 == 0, D <= 1024; bias needs w; mod_ld % 4 == 0.  x, w, bias, shift, scale 16-byte and out_bf16 8-byte
+ * aligned. */
 int ga_layernorm_modulate(const float *x, const float *w, const float *bias, const float *shift, const float *scale,
                           int mod_ld, int rows_per_batch, void *out_bf16, int R, int D, float eps, void *stream);
-/* y[r, c] = bias[c] + sum_d f(x[r])[d] W[c, d], f = optional LayerNorm (ln_w, ln_b) then optional SiLU; C <= 16 */
+/* y[r, c] = bias[c] + sum_d f(x[r])[d] W[c, d], f = optional LayerNorm (ln_w, ln_b) then optional SiLU; C <= 16;
+ * D % 4 == 0, D <= 1024; x, ln_w, ln_b, W 16-byte aligned */
 int ga_thin_linear(const float *x, const float *ln_w, const float *ln_b, int apply_silu, const float *W,
                    const float *bias, float *y, int R, int D, int C, float eps, void *stream);
 /* attention over S sequences of L <= 16 tokens: qkv bf16 [S*L, 3*H*64] ("(K H D)" columns), q/k RMS-normalised per
@@ -256,7 +265,8 @@ int ga_thin_linear(const float *x, const float *ln_w, const float *ln_b, int app
 int ga_micro_attention_bf16(const void *qkv, const float *qn_w, const float *kn_w, void *out, int S, int L, int H,
                             float eps, void *stream);
 /* seq [S, 1+f, D] fp32: row 0 = the parent token (prev_f == 0: parents[s]; else child s % prev_f of sequence
- * s / prev_f of the previous stage's [S/prev_f, 1+prev_f, D] buffer), rows 1..f = queries [f, D] */
+ * s / prev_f of the previous stage's [S/prev_f, 1+prev_f, D] buffer), rows 1..f = queries [f, D]; D % 4 == 0,
+ * D <= 1024; parents, queries, seq 16-byte aligned */
 int ga_micro_seq_build(const float *parents, int prev_f, const float *queries, float *seq, int64_t S, int f, int D,
                        void *stream);
 /* child r of parent r / f: res row = r, or (res_in_sequences) row (r/f)(1+f) + 1 + r%f of the [R/f, 1+f] sequence
@@ -290,7 +300,8 @@ size_t ga_dino_frontend_scratch_bytes(int batch, int H, int W, int out_size);
 int ga_dino_frontend(const float *img, int batch, int H, int W, int out_size, int patch, void *patches_bf16,
                      int k_pitch, void *scratch, size_t scratch_bytes, void *stream);
 /* x fp32 [batch, 1 + n_reg + n_patch, D] = cls_token + pos_embed[0] | reg_tokens [n_reg, D] (no pos_embed) |
- * patch_out [batch * n_patch, D] + pos_embed[1 ..] ; pos_embed [1 + n_patch, D], D % 4 == 0 */
+ * patch_out [batch * n_patch, D] + pos_embed[1 ..] ; pos_embed [1 + n_patch, D], D % 4 == 0; every pointer 16-byte
+ * aligned */
 int ga_dino_tokens(const float *patch_out, const float *cls_token, const float *reg_tokens, int n_reg,
                    const float *pos_embed, float *x, int batch, int n_patch, int D, void *stream);
 
@@ -401,7 +412,8 @@ int ga_group_norm_nhwc(const float *x, const float *gamma, const float *beta, in
 int ga_fps(const float *pcd, int batch, int N, int K, const int32_t *start_idx, int32_t *idx_out,
            float *xyz_out, void *stream);
 /* img fp32 NCHW [n, C, H, W] -> x_bf16 NHWC [n, H, W, c_pad] (channels from C on zero; c_pad % 8 == 0), and, when
- * token_xyz is not NULL, token_xyz fp32 ["(n ty tx)", 3] = img[:, xyz_c:xyz_c+3, off::step, off::step]. */
+ * token_xyz is not NULL, token_xyz fp32 ["(n ty tx)", 3] = img[:, xyz_c:xyz_c+3, off::step, off::step].  x_bf16
+ * 4-byte aligned.  Every argument, token_xyz's included, is checked before anything is written. */
 int ga_vae_enc_input(const float *img, int n, int C, int H, int W, int c_pad, void *x_bf16, int xyz_c,
                      int step, int off, float *token_xyz, void *stream);
 /* Head split for head_dim 32: qkv bf16 [R, 3 * heads * 32] ("(K H D)" columns, bias included) -> q, k per-head
@@ -420,7 +432,8 @@ typedef struct GaVaeEncHead {
 } GaVaeEncHead;
 /* Per token r of x fp32 [R, D]: h = fc2(gelu_tanh(fc1(LayerNorm(x)))) -> h_out [R, 2 zc]; moments =
  * q2(gelu_tanh(q1(h))); mean = moments[:zc], logvar = 20 tanh(moments[zc:] / 20), std = exp(logvar / 2) (stdv may
- * be NULL), latent = mean + std * noise (noise fp32 [R, zc]; NULL gives latent = mean; latent may be NULL). */
+ * be NULL), latent = mean + std * noise (noise fp32 [R, zc]; NULL gives latent = mean; latent may be NULL).
+ * GA_ERR_SIZE when (D + hid + 6 zc) * 4 bytes of shared memory, plus the kernel's 32 static bytes, exceed 48 KiB. */
 int ga_vae_enc_head(const GaVaeEncHead *p, const float *x, const float *noise, int R, int D, int hid, int zc,
                     float *h_out, float *mean, float *logvar, float *stdv, float *latent, void *stream);
 
