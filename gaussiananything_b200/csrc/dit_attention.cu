@@ -17,14 +17,12 @@
 //   warp 8    : TMA producer (Q once, K and V double buffered).
 #include "../../include/ga_b200.h"
 #include "device_once.cuh"
+#include "gemm_sm90.cuh"
 #include "row_common.cuh"
 #include "sm90_ptx.cuh"
 
 using namespace ga_row;
 using namespace sm90;
-
-int ga_make_tmap_bf16(CUtensorMap *map, const void *ptr, uint64_t rows, uint64_t cols, uint64_t ld_elems,
-                      uint32_t box_rows);
 
 namespace {
 

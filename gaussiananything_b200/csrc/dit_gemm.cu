@@ -5,33 +5,15 @@
 // /root/reference/vit/vision_transformer.py:215-303 and
 // /root/reference/ldm/modules/attention.py:484-561.
 //
-// Persistent kernel, one CTA per SM looping over 128 x BN output tiles, three warpgroups:
-//   warpgroup 0   : TMA producer (one elected thread; cp.async.bulk.tensor, 128B-swizzled K-major tiles)
-//   warpgroups 1-2: consumers, 64 rows each: wgmma m64nBNk16 from shared memory into registers, then the
-//                   epilogue straight from the accumulator registers
-// smem ring of kStages {A 128x64, W BNx64} bf16 tiles with full/empty mbarriers.  The producer keeps filling the
-// ring for the next tile while the consumers run the epilogue of this one.
+// The main loop is gemm_sm90.cuh's persistent kernel with both operands K-major; this file holds its epilogues.
 #include "../../include/ga_b200.h"
-#include "device_once.cuh"
+#include "gemm_sm90.cuh"
 #include "row_common.cuh"
-#include "sm90_ptx.cuh"
 
 using namespace ga_row;
-using namespace sm90;
+using namespace gemm_sm90;
 
 namespace {
-
-constexpr int BM = 128, BK = 64;
-constexpr int kConsumerWarps = 8;
-constexpr int kThreads = 128 + 32 * kConsumerWarps;      // producer warpgroup + 2 consumer warpgroups
-
-template <int BN> struct GemmCfg {
-    static constexpr int kABytes = BM * BK * 2;
-    static constexpr int kBBytes = BN * BK * 2;
-    static constexpr int kStages = (200 * 1024) / (kABytes + kBBytes) > 8 ? 8 : (200 * 1024) / (kABytes + kBBytes);
-    static constexpr int kRing = kStages * (kABytes + kBBytes);
-    static constexpr int kSmem = kRing + 1024 + kConsumerWarps * 2048;       // + epilogue staging
-};
 
 // exact-erf GELU to ~3e-7 (Abramowitz-Stegun 7.1.28: erf x = 1 - (1 + a1 x + .. + a6 x^6)^-16), 1 MUFU + ~16 FP32
 // ops per element; the library erff() costs about twice that and would make the GELU epilogue slower than the MMAs.
@@ -59,7 +41,6 @@ __device__ __forceinline__ float gelu_erf(float v)
 //   phase A (fragment layout)          : registers -> staging, 32 fp32 columns at a time
 //   phase B (8 lanes = one 128 B row)  : staging -> bias / GELU / gate / residual -> coalesced global stores
 // The epilogue mode is a template parameter, so the unrolled loops carry no run-time switch.
-constexpr int kStageBytes = 2048;          // per consumer warp
 constexpr int kWarpRows = 16;              // accumulator rows per warp
 
 // Epilogue of ga_linear_fc1_gelu_bf16 (include/ga_b200.h Part 13), outside the GA_EPI_* range so that
@@ -345,81 +326,16 @@ __device__ __forceinline__ void epilogue_tile(const GaGemmEpilogue &ep, uint32_t
     }
 }
 
-// Persistent: grid = min(#tiles, #SMs); producer and consumers walk the same tile sequence.
-template <int BN, int MODE>
-__global__ void __launch_bounds__(kThreads, 1)
-gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
-                    const GaGemmEpilogue ep, const int M, const int N, const int K)
-{
-    using Cfg = GemmCfg<BN>;
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t full_bar[Cfg::kStages], empty_bar[Cfg::kStages];
-    uint8_t *smem = align1024(smem_raw);
-    uint8_t *smem_a = smem, *smem_b = smem + Cfg::kStages * Cfg::kABytes;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int wg = threadIdx.x >> 7;
-    const int nk = (K + BK - 1) / BK;
-    const int num_m = (M + BM - 1) / BM, num_n = (N + BN - 1) / BN;
-    const int tiles = num_m * num_n;
-
-    if (threadIdx.x == 0) {
-        prefetch_tmap(&tma_a);
-        prefetch_tmap(&tma_b);
-        for (int s = 0; s < Cfg::kStages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps); }
-        fence_barrier_init();
+// The epilogue type of gemm_sm90_kernel: the staged epilogue above.
+template <int BN, int MODE> struct TnEpilogue {
+    static constexpr bool kStaging = true;
+    GaGemmEpilogue ep;
+    __device__ __forceinline__ void operator()(const float (&acc)[BN / 2], uint32_t stg, int lane, int row0, int n0,
+                                               int, int M, int N) const
+    {
+        epilogue_tile<BN, MODE>(ep, stg, acc, lane, row0, n0, M, N);
     }
-    __syncthreads();
-    pdl_wait();                     // inputs (A, the residual stream, the gate table) come from earlier kernels
-    pdl_launch_dependents();        // let the next kernel run its own prologue under our main loop
-
-    if (wg == 0) {
-        setmaxnreg_dec<40>();
-        if (warp == 0 && elect_one()) {
-            int it = 0;
-            for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-                const int m0 = (tile % num_m) * BM, n0 = (tile / num_m) * BN;
-                for (int kb = 0; kb < nk; kb++, it++) {
-                    const int s = it % Cfg::kStages;
-                    mbar_wait(&empty_bar[s], ((it / Cfg::kStages) & 1) ^ 1);     // every consumer warp released it
-                    mbar_expect_tx(&full_bar[s], Cfg::kABytes + Cfg::kBBytes);
-                    tma_load_2d(smem_a + s * Cfg::kABytes, &tma_a, &full_bar[s], kb * BK, m0);
-                    tma_load_2d(smem_b + s * Cfg::kBBytes, &tma_b, &full_bar[s], kb * BK, n0);
-                }
-            }
-        }
-    } else {
-        setmaxnreg_inc<232>();
-        const int cw = wg - 1;                      // which 64-row half of the tile
-        const int wi = warp & 3;                    // 16-row slice of that half
-        const uint32_t stg = smem_u32(smem + Cfg::kRing + (cw * 4 + wi) * kStageBytes);
-        float acc[BN / 2];
-        int it = 0;
-        for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-            const int m0 = (tile % num_m) * BM, n0 = (tile / num_m) * BN;
-            for (int kb = 0; kb < nk; kb++, it++) {
-                const int s = it % Cfg::kStages;
-                mbar_wait(&full_bar[s], (it / Cfg::kStages) & 1);
-                const uint64_t ad = wgmma_desc_k_sw128(smem_u32(smem_a + s * Cfg::kABytes + cw * 64 * 128));
-                const uint64_t bd = wgmma_desc_k_sw128(smem_u32(smem_b + s * Cfg::kBBytes));
-                fence_regs(acc);
-                wgmma_fence();
-#pragma unroll
-                for (int k = 0; k < BK / 16; k++)
-                    wgmma_ss<BN>(acc, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), (uint32_t)((kb | k) != 0));
-                wgmma_commit();
-                fence_regs(acc);
-                wgmma_wait<1>();                    // the previous stage's MMAs have retired: release its slot
-                fence_regs(acc);
-                if (kb > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % Cfg::kStages]);
-            }
-            wgmma_wait<0>();
-            fence_regs(acc);
-            if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % Cfg::kStages]);
-            epilogue_tile<BN, MODE>(ep, stg, acc, lane, m0 + cw * 64 + wi * kWarpRows, n0, M, N);
-        }
-    }
-}
+};
 
 // ---- host side -------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
@@ -458,25 +374,6 @@ int ga_make_tmap_bf16(CUtensorMap *map, const void *ptr, uint64_t rows, uint64_t
     return r == CUDA_SUCCESS ? 0 : 1000 + (int)r;
 }
 
-static int sm_count() { return ga_sm_count(); }
-
-template <int BN, int MODE>
-static int launch_gemm_mode(const CUtensorMap &ta, const CUtensorMap &tb, const GaGemmEpilogue &ep, int M, int N, int K,
-                            cudaStream_t s)
-{
-    using Cfg = GemmCfg<BN>;
-    static GaPerDevice attr_set;
-    if (ga_first_use_on_device(attr_set)) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_bf16_tn_kernel<BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             Cfg::kSmem);
-        if (e != cudaSuccess) return (int)e;
-    }
-    const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
-    const int grid = tiles < sm_count() ? tiles : sm_count();
-    return (int)ga_launch_pdl(gemm_bf16_tn_kernel<BN, MODE>, dim3(grid), dim3(kThreads), (size_t)Cfg::kSmem, s, ta, tb, ep,
-                              M, N, K);
-}
-
 template <int BN>
 static int launch_gemm(const void *A, int lda, const void *W, int ldw, const GaGemmEpilogue &ep, int M, int N, int K,
                        cudaStream_t s)
@@ -486,18 +383,29 @@ static int launch_gemm(const void *A, int lda, const void *W, int ldw, const GaG
     if (rc) return rc;
     rc = ga_make_tmap_bf16(&tb, W, (uint64_t)N, (uint64_t)K, (uint64_t)ldw, (uint32_t)BN);
     if (rc) return rc;
+    auto run = [&](auto epi) { return gemm_sm90_launch<BN, kMajorK, kMajorK, false>(ta, tb, epi, M, N, K, 1, s); };
     switch (ep.mode) {
-    case GA_EPI_BF16: return launch_gemm_mode<BN, GA_EPI_BF16>(ta, tb, ep, M, N, K, s);
-    case GA_EPI_GELU_BF16: return launch_gemm_mode<BN, GA_EPI_GELU_BF16>(ta, tb, ep, M, N, K, s);
-    case GA_EPI_F32: return launch_gemm_mode<BN, GA_EPI_F32>(ta, tb, ep, M, N, K, s);
-    case GA_EPI_RESID_GATE_F32: return launch_gemm_mode<BN, GA_EPI_RESID_GATE_F32>(ta, tb, ep, M, N, K, s);
-    case GA_EPI_GEGLU_BF16: return launch_gemm_mode<BN, GA_EPI_GEGLU_BF16>(ta, tb, ep, M, N, K, s);
+    case GA_EPI_BF16: return run(TnEpilogue<BN, GA_EPI_BF16>{ep});
+    case GA_EPI_GELU_BF16: return run(TnEpilogue<BN, GA_EPI_GELU_BF16>{ep});
+    case GA_EPI_F32: return run(TnEpilogue<BN, GA_EPI_F32>{ep});
+    case GA_EPI_RESID_GATE_F32: return run(TnEpilogue<BN, GA_EPI_RESID_GATE_F32>{ep});
+    case GA_EPI_GEGLU_BF16: return run(TnEpilogue<BN, GA_EPI_GEGLU_BF16>{ep});
     case GA_EPI_HEADS:
-        if (BN == 128 || BN == 256)
-            return launch_gemm_mode<((BN == 128 || BN == 256) ? BN : 128), GA_EPI_HEADS>(ta, tb, ep, M, N, K, s);
-        return GA_ERR_BADARG;
+        if constexpr (BN == 128 || BN == 256) return run(TnEpilogue<BN, GA_EPI_HEADS>{ep});
+        else return GA_ERR_BADARG;
+    case kEpiGeluKeepPre: return run(TnEpilogue<BN, kEpiGeluKeepPre>{ep});
     default: return GA_ERR_BADARG;
     }
+}
+
+// block_n = tile width {64, 128, 192, 256}
+static int gemm_tn(const void *A, int lda, const void *W, int ldw, const GaGemmEpilogue &ep, int M, int N, int K,
+                   int block_n, cudaStream_t s)
+{
+    if (block_n == 64) return launch_gemm<64>(A, lda, W, ldw, ep, M, N, K, s);
+    if (block_n == 128) return launch_gemm<128>(A, lda, W, ldw, ep, M, N, K, s);
+    if (block_n == 192) return launch_gemm<192>(A, lda, W, ldw, ep, M, N, K, s);
+    return launch_gemm<256>(A, lda, W, ldw, ep, M, N, K, s);
 }
 
 static bool misaligned(const void *p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) != 0; }
@@ -544,27 +452,10 @@ extern "C" int ga_gemm_bf16_tn(const void *A, int lda, const void *W, int ldw, i
 {
     const int rc = ga_gemm_validate(A, lda, W, ldw, M, N, K, epi, block_n);
     if (rc) return rc;
-    // block_n = tile width {64, 128, 192, 256}
-    const int bn = block_n;
-    cudaStream_t s = (cudaStream_t)stream;
-    if (bn == 64) return launch_gemm<64>(A, lda, W, ldw, *epi, M, N, K, s);
-    if (bn == 128) return launch_gemm<128>(A, lda, W, ldw, *epi, M, N, K, s);
-    if (bn == 192) return launch_gemm<192>(A, lda, W, ldw, *epi, M, N, K, s);
-    return launch_gemm<256>(A, lda, W, ldw, *epi, M, N, K, s);
+    return gemm_tn(A, lda, W, ldw, *epi, M, N, K, block_n, (cudaStream_t)stream);
 }
 
 // fc1 of a FusedMLP for training (Part 13): the GEMM above with the kEpiGeluKeepPre epilogue.
-template <int BN>
-static int launch_fc1(const void *x, const void *w1, const GaGemmEpilogue &ep, int M, int N, int K, cudaStream_t s)
-{
-    CUtensorMap ta, tb;
-    int rc = ga_make_tmap_bf16(&ta, x, (uint64_t)M, (uint64_t)K, (uint64_t)K, BM);
-    if (rc) return rc;
-    rc = ga_make_tmap_bf16(&tb, w1, (uint64_t)N, (uint64_t)K, (uint64_t)K, (uint32_t)BN);
-    if (rc) return rc;
-    return launch_gemm_mode<BN, kEpiGeluKeepPre>(ta, tb, ep, M, N, K, s);
-}
-
 extern "C" int ga_linear_fc1_gelu_bf16(const void *x, const void *w1, const float *b1, void *h, void *z, int M, int N,
                                        int K, int block_n, void *stream)
 {
@@ -576,9 +467,5 @@ extern "C" int ga_linear_fc1_gelu_bf16(const void *x, const void *w1, const floa
     ep.out = h;
     ep.ld_out = N;
     ep.q = z;
-    cudaStream_t s = (cudaStream_t)stream;
-    if (block_n == 64) return launch_fc1<64>(x, w1, ep, M, N, K, s);
-    if (block_n == 128) return launch_fc1<128>(x, w1, ep, M, N, K, s);
-    if (block_n == 192) return launch_fc1<192>(x, w1, ep, M, N, K, s);
-    return launch_fc1<256>(x, w1, ep, M, N, K, s);
+    return gemm_tn(x, K, w1, K, ep, M, N, K, block_n, (cudaStream_t)stream);
 }

@@ -5,52 +5,34 @@
 //   bias   db[N]     = column sums of G
 // bf16 operands, fp32 accumulation in registers, no atomics.
 //
-// The GEMMs are the persistent kernel of dit_gemm.cu with different operand majors: one CTA per SM loops over
-// 128 x 128 output tiles; warpgroup 0 is the TMA producer (one elected thread), warpgroups 1-2 each own 64 rows and
-// run wgmma m64n128k16 from a ring of shared-memory stages guarded by full/empty mbarriers.  The operands that are
-// contiguous along an output dimension ("MN-major": W in dgrad, both G and x in wgrad) are fed with wgmma's
-// transposed operand mode on the 128-byte-swizzled TMA box as it lands: a box {64 along M or N, 64 along K} is
-// exactly the MN-major swizzle atom wgmma reads (wgmma_desc_mn_sw128), so these operands go from global memory to
-// the tensor cores with no shared-memory pass and the same pipeline as the forward.  attention_grad.cu builds
-// transposed copies instead because it stages with cp.async through arbitrary strides and uses the same tiles as
-// K-major operands of other products in the kernel; neither applies here.
+// The GEMMs run the main loop of gemm_sm90.cuh at 128 x 128 tiles with this file's register-direct epilogue.  The
+// operands that are contiguous along an output dimension ("MN-major": W in dgrad, both G and x in wgrad) are fed with
+// wgmma's transposed operand mode on the TMA boxes as they land, so they reach the tensor cores with no shared-memory
+// pass and the same pipeline as the forward.  attention_grad.cu builds transposed copies instead because it stages
+// with cp.async through arbitrary strides and uses the same tiles as K-major operands of other products in the
+// kernel; neither applies here.
 //
 // wgrad splits its contraction (the M rows) into S consecutive ranges of 64-row blocks so that small weights still
 // fill the GPU (the SRT's 256 x 1024 weight has 16 output tiles); S depends on the shapes alone, so the bits do not
 // depend on the card.  Each range writes an fp32 partial; a second kernel adds them in split order.
 #include "../../include/ga_b200.h"
-#include "device_once.cuh"
+#include "gemm_sm90.cuh"
 #include "row_common.cuh"
-#include "sm90_ptx.cuh"
 
 using namespace ga_row;
-using namespace sm90;
-
-int ga_make_tmap_bf16(CUtensorMap *map, const void *ptr, uint64_t rows, uint64_t cols, uint64_t ld_elems,
-                      uint32_t box_rows);
+using namespace gemm_sm90;
 
 namespace {
 
-constexpr int BM = 128, BN = 128, BK = 64;
-constexpr int kThreads = 128 + 256;                 // producer warpgroup + 2 consumer warpgroups
-constexpr int kConsumerWarps = 8;
-constexpr int kABytes = BM * BK * 2, kBBytes = BN * BK * 2;
-constexpr int kHalf = 64 * BK * 2;                  // one 64-wide box: 8 KB
-constexpr int kStages = 6;
-constexpr int kSmem = kStages * (kABytes + kBBytes) + 1024;
-
-constexpr int kDgrad = 0, kWgrad = 1;               // kernel kinds: A K-major or MN-major (B is MN-major in both)
+constexpr int BN = 128;                             // the one tile width of dgrad and wgrad
 constexpr int kEpiBf16 = 0, kEpiF32 = 1, kEpiGeluBwd = 2;
 
 constexpr int kColRows = 256;                       // bias gradient: rows per chunk
 constexpr int kColWarps = 8;
 
 struct GradArgs {
-    void *out;                      // [Mo, No] (+ split * split_stride for wgrad partials)
-    const __nv_bfloat16 *z;         // kEpiGeluBwd: fc1's pre-activation, bf16 [Mo, No]
-    int Mo, No;                     // output rows and columns
-    int nkb;                        // 64-deep blocks of the contraction
-    int splits;
+    void *out;                      // [M, N] (+ split * split_stride for wgrad partials)
+    const __nv_bfloat16 *z;         // kEpiGeluBwd: fc1's pre-activation, bf16 [M, N]
     long long split_stride;         // elements between partials
 };
 
@@ -62,26 +44,12 @@ __device__ __forceinline__ float gelu_grad(float z)
     return fmaf(z, pdf, cdf);
 }
 
-struct TileCoord { int m0, n0, kb0, kb1; long long split; };
-
-__device__ __forceinline__ TileCoord tile_coord(const GradArgs &a, int tile, int num_m, int per_split)
-{
-    TileCoord t;
-    const int split = tile / per_split, r = tile - split * per_split;
-    t.m0 = (r % num_m) * BM;
-    t.n0 = (r / num_m) * BN;
-    t.kb0 = (int)((long long)split * a.nkb / a.splits);
-    t.kb1 = (int)((long long)(split + 1) * a.nkb / a.splits);
-    t.split = split;
-    return t;
-}
-
 // Accumulator of wgmma m64n128 (warp w of the warpgroup, lane l): acc[4 j + e] is row 16 w + l / 4 + 8 (e >> 1),
-// column 8 j + 2 (l % 4) + (e & 1).  Stored straight from registers as column pairs (No % 8 == 0, so a pair is
+// column 8 j + 2 (l % 4) + (e & 1).  Stored straight from registers as column pairs (N % 8 == 0, so a pair is
 // either wholly inside or wholly outside).
 template <int EPI>
 __device__ __forceinline__ void epilogue(const GradArgs &a, const float (&acc)[64], int row0, int n0, long long split,
-                                         int lane)
+                                         int lane, int M, int N)
 {
     const int r = lane >> 2, c = 2 * (lane & 3);
     // Z is read up front, all in flight at once: interleaved with the stores below the compiler must assume they
@@ -94,8 +62,8 @@ __device__ __forceinline__ void epilogue(const GradArgs &a, const float (&acc)[6
 #pragma unroll
             for (int j = 0; j < BN / 8; j++) {
                 const int col = n0 + 8 * j + c;
-                zr[hf][j] = (row < a.Mo && col < a.No)
-                                ? __ldg(reinterpret_cast<const unsigned int *>(a.z + (size_t)row * a.No + col))
+                zr[hf][j] = (row < M && col < N)
+                                ? __ldg(reinterpret_cast<const unsigned int *>(a.z + (size_t)row * N + col))
                                 : 0u;
             }
         }
@@ -103,12 +71,12 @@ __device__ __forceinline__ void epilogue(const GradArgs &a, const float (&acc)[6
 #pragma unroll
     for (int hf = 0; hf < 2; hf++) {
         const int row = row0 + r + 8 * hf;
-        if (row >= a.Mo) continue;
+        if (row >= M) continue;
 #pragma unroll
         for (int j = 0; j < BN / 8; j++) {
             const int col = n0 + 8 * j + c;
-            if (col >= a.No) continue;
-            const size_t idx = (size_t)row * a.No + col;
+            if (col >= N) continue;
+            const size_t idx = (size_t)row * N + col;
             const float v0 = acc[4 * j + 2 * hf], v1 = acc[4 * j + 2 * hf + 1];
             if constexpr (EPI == kEpiBf16) {
                 *reinterpret_cast<uint32_t *>(reinterpret_cast<__nv_bfloat16 *>(a.out) + idx) = pack_bf16(v0, v1);
@@ -124,89 +92,15 @@ __device__ __forceinline__ void epilogue(const GradArgs &a, const float (&acc)[6
     }
 }
 
-// Persistent: grid = min(#tiles, #SMs); producer and consumers walk the same tile sequence.  Which CTA takes a tile
-// does not change its result.
-template <int KIND, int EPI>
-__global__ void __launch_bounds__(kThreads, 1)
-linear_grad_gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
-                        const GradArgs a)
-{
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t full_bar[kStages], empty_bar[kStages];
-    uint8_t *smem = align1024(smem_raw);
-    uint8_t *smem_a = smem, *smem_b = smem + kStages * kABytes;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int wg = threadIdx.x >> 7;
-    const int num_m = (a.Mo + BM - 1) / BM, num_n = (a.No + BN - 1) / BN;
-    const int per_split = num_m * num_n, tiles = per_split * a.splits;
-
-    if (threadIdx.x == 0) {
-        prefetch_tmap(&tma_a);
-        prefetch_tmap(&tma_b);
-        for (int s = 0; s < kStages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps); }
-        fence_barrier_init();
+// The epilogue type of gemm_sm90_kernel: epilogue<EPI> straight from the registers, no staging.
+template <int EPI> struct GradEpilogue : GradArgs {
+    static constexpr bool kStaging = false;
+    __device__ __forceinline__ void operator()(const float (&acc)[64], uint32_t, int lane, int row0, int n0, int split,
+                                               int M, int N) const
+    {
+        epilogue<EPI>(*this, acc, row0, n0, split, lane, M, N);
     }
-    __syncthreads();
-    pdl_wait();
-    pdl_launch_dependents();
-
-    if (wg == 0) {
-        setmaxnreg_dec<40>();
-        if (warp == 0 && elect_one()) {
-            int it = 0;
-            for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-                const TileCoord t = tile_coord(a, tile, num_m, per_split);
-                for (int kb = t.kb0; kb < t.kb1; kb++, it++) {
-                    const int s = it % kStages;
-                    mbar_wait(&empty_bar[s], ((it / kStages) & 1) ^ 1);
-                    mbar_expect_tx(&full_bar[s], kABytes + kBBytes);
-                    uint8_t *sa = smem_a + s * kABytes, *sb = smem_b + s * kBBytes;
-                    if (KIND == kDgrad) {
-                        tma_load_2d(sa, &tma_a, &full_bar[s], kb * BK, t.m0);            // G [M, N]: 128 rows
-                    } else {
-                        tma_load_2d(sa, &tma_a, &full_bar[s], t.m0, kb * BK);            // G [M, N]: columns m0..
-                        tma_load_2d(sa + kHalf, &tma_a, &full_bar[s], t.m0 + 64, kb * BK);
-                    }
-                    tma_load_2d(sb, &tma_b, &full_bar[s], t.n0, kb * BK);
-                    tma_load_2d(sb + kHalf, &tma_b, &full_bar[s], t.n0 + 64, kb * BK);
-                }
-            }
-        }
-    } else {
-        setmaxnreg_inc<232>();
-        const int cw = wg - 1;                      // which 64-row half of the tile
-        const int wi = warp & 3;                    // 16-row slice of that half
-        float acc[64];
-        int it = 0;
-        for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-            const TileCoord t = tile_coord(a, tile, num_m, per_split);
-            for (int kb = t.kb0; kb < t.kb1; kb++, it++) {
-                const int s = it % kStages;
-                mbar_wait(&full_bar[s], (it / kStages) & 1);
-                const uint32_t sa = smem_u32(smem_a + s * kABytes + cw * kHalf);
-                const uint64_t ad = KIND == kDgrad ? wgmma_desc_k_sw128(sa) : wgmma_desc_mn_sw128(sa, kHalf);
-                const uint64_t bd = wgmma_desc_mn_sw128(smem_u32(smem_b + s * kBBytes), kHalf);
-                constexpr uint64_t a_step = KIND == kDgrad ? 2 : 128;      // 16 columns (32 B) or 16 rows (2 KB)
-                fence_regs(acc);
-                wgmma_fence();
-#pragma unroll
-                for (int k = 0; k < BK / 16; k++)
-                    wgmma_m64n128k16_ss_t<KIND == kDgrad ? 0 : 1, 1>(acc, ad + a_step * k, bd + 128 * k,
-                                                                     (uint32_t)((kb != t.kb0) | k));
-                wgmma_commit();
-                fence_regs(acc);
-                wgmma_wait<1>();                    // the previous stage's MMAs have retired: release its slot
-                fence_regs(acc);
-                if (kb > t.kb0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % kStages]);
-            }
-            wgmma_wait<0>();
-            fence_regs(acc);
-            if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % kStages]);
-            epilogue<EPI>(a, acc, t.m0 + cw * 64 + wi * 16, t.n0, t.split, lane);
-        }
-    }
-}
+};
 
 // Column sums of g bf16 [M, N], one block per (64 columns, chunk of kColRows rows): warp w adds rows w, w + 8, ...
 // of the chunk in order, lane l columns 2 l, 2 l + 1; the warp sums are added in warp order into out[chunk, :].
@@ -248,22 +142,6 @@ int wgrad_splits(int M, int N, int K)
 }
 
 int col_chunks(int M) { return (M + kColRows - 1) / kColRows; }
-
-template <int KIND, int EPI>
-int launch_grad_gemm(const CUtensorMap &ta, const CUtensorMap &tb, const GradArgs &a, cudaStream_t s)
-{
-    static GaPerDevice attr_set;
-    if (ga_first_use_on_device(attr_set)) {
-        cudaError_t e = cudaFuncSetAttribute(linear_grad_gemm_kernel<KIND, EPI>,
-                                             cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-        if (e != cudaSuccess) return (int)e;
-    }
-    const long long tiles = (long long)((a.Mo + BM - 1) / BM) * ((a.No + BN - 1) / BN) * a.splits;
-    const int sms = ga_sm_count();
-    const int grid = tiles < sms ? (int)tiles : sms;
-    return (int)ga_launch_pdl(linear_grad_gemm_kernel<KIND, EPI>, dim3(grid), dim3(kThreads), (size_t)kSmem, s, ta, tb,
-                              a);
-}
 
 }  // namespace
 
@@ -329,11 +207,12 @@ extern "C" int ga_linear_dgrad_bf16(const void *g, const void *w, const void *z,
     if (rc) return rc;
     rc = ga_make_tmap_bf16(&tb, w, (uint64_t)N, (uint64_t)K, (uint64_t)K, BK);        // MN-major: 64 rows along N
     if (rc) return rc;
-    GradArgs a = {out, reinterpret_cast<const __nv_bfloat16 *>(z), M, K, (N + BK - 1) / BK, 1, 0};
+    const GradArgs a = {out, reinterpret_cast<const __nv_bfloat16 *>(z), 0};
     cudaStream_t s = (cudaStream_t)stream;
-    if (z) return launch_grad_gemm<kDgrad, kEpiGeluBwd>(ta, tb, a, s);
-    if (out_f32) return launch_grad_gemm<kDgrad, kEpiF32>(ta, tb, a, s);
-    return launch_grad_gemm<kDgrad, kEpiBf16>(ta, tb, a, s);
+    auto run = [&](auto epi) { return gemm_sm90_launch<BN, kMajorK, kMajorMN, false>(ta, tb, epi, M, K, N, 1, s); };
+    if (z) return run(GradEpilogue<kEpiGeluBwd>{a});
+    if (out_f32) return run(GradEpilogue<kEpiF32>{a});
+    return run(GradEpilogue<kEpiBf16>{a});
 }
 
 extern "C" int ga_linear_wgrad_bf16(const void *g, const void *x, float *dw, int M, int N, int K, void *workspace,
@@ -347,9 +226,9 @@ extern "C" int ga_linear_wgrad_bf16(const void *g, const void *x, float *dw, int
     rc = ga_make_tmap_bf16(&tb, x, (uint64_t)M, (uint64_t)K, (uint64_t)K, BK);
     if (rc) return rc;
     const int S = wgrad_splits(M, N, K);
-    GradArgs a = {S > 1 ? workspace : dw, nullptr, N, K, (M + BK - 1) / BK, S, (long long)N * K};
+    const GradEpilogue<kEpiF32> epi = {{S > 1 ? workspace : dw, nullptr, (long long)N * K}};
     cudaStream_t s = (cudaStream_t)stream;
-    rc = launch_grad_gemm<kWgrad, kEpiF32>(ta, tb, a, s);
+    rc = gemm_sm90_launch<BN, kMajorMN, kMajorMN, true>(ta, tb, epi, N, K, M, S, s);
     if (rc || S == 1) return rc;
     return (int)ga_launch_partial_sum(reinterpret_cast<const float *>(workspace), dw, 1, S, (long long)N * K, s);
 }

@@ -865,7 +865,7 @@ int ga_attention_bwd_bf16(const void *q, const void *k, const void *v, const voi
 int ga_linear_grad_validate(int op, const void *a, const void *b, const void *aux, const void *out, int out_f32, int M,
                             int N, int K, int block_n, const void *workspace, size_t workspace_bytes);
 /* fc1 of the MLP for training: v = x W1^T + b1 (b1 fp32 [N] or NULL), H = bf16(gelu_erf(v)), Z = bf16(v), both bf16
- * [M, N] (row pitch N).  x bf16 [M, K], W1 bf16 [N, K].  The ga_gemm_bf16_tn kernel at tile width block_n, with an
+ * [M, N] (row pitch N).  x bf16 [M, K], W1 bf16 [N, K].  ga_gemm_bf16_tn's GEMM at tile width block_n, with an
  * epilogue that writes both outputs from one accumulator; gelu_erf is GA_EPI_GELU_BF16's. */
 int ga_linear_fc1_gelu_bf16(const void *x, const void *w1, const float *b1, void *h, void *z, int M, int N, int K,
                             int block_n, void *stream);
