@@ -339,8 +339,6 @@ layernorm_rows_bwd_kernel(const float *__restrict__ x, const float *__restrict__
     if (db) reinterpret_cast<float4 *>(db)[q] = ab;
 }
 
-bool mis4(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 3) != 0; }
-
 }  // namespace
 
 extern "C" int ga_dit_final_layer_bwd_validate(const float *x, const float *mod, const float *W, const float *dy,

@@ -97,6 +97,7 @@ __device__ __forceinline__ void cta_colsum(float4 (*red)[kMaxD / 4], const float
 // ---- host
 static inline bool mis16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
 static inline bool mis8(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 7) != 0; }
+static inline bool mis4(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 3) != 0; }
 
 }  // namespace ga_row
 

@@ -11,12 +11,15 @@ using namespace ga_row;
 namespace {
 
 // ---------------------------------------------------------------------------------------------------------------
-// GroupNorm(32) over NHWC fp32, deterministic split reduction.  Pass 1: one CTA per (pixel chunk, image) writes the
-// chunk's per-group fp32 sum and sum of squares.  Pass 2: every CTA folds its image's partials in fp64 into mean and
-// 1/sqrt(var + eps), then normalises its chunk, applies the affine and optional SiLU and writes bf16 or fp32.
+// GroupNorm(32) over NHWC fp32, deterministic split reduction.  Pass 1: one CTA per (pixel chunk, image) sums each
+// channel's values shifted by the chunk's first pixel (the pivot), so a group whose |mean| is large against its std
+// loses nothing to cancellation, and writes the chunk's per-group Chan terms (mean, M2 = sum of squared deviations)
+// formed in fp64.  Pass 2: every CTA merges its image's terms in fp64 into mean and 1/sqrt(var + eps), then
+// normalises its chunk, applies the affine and optional SiLU and writes bf16 or fp32.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int kGnThreads = 256;
 constexpr int kGroups = 32;
+constexpr int kGnMergeLanes = kGnThreads / kGroups;     // pass 2: lanes that merge one group's chunk terms
 
 __host__ __device__ inline int gn_chunk_px(int HW) { return HW >= 65536 ? 1024 : (HW >= 4096 ? 256 : 64); }
 
@@ -25,16 +28,21 @@ __global__ void __launch_bounds__(kGnThreads) gn_stats_kernel(const float *__res
 {
     __shared__ float2 red[kGnThreads * 4];
     __shared__ float2 ch_sum[1024];
+    __shared__ float piv[1024];
     const int img = blockIdx.y, ck = blockIdx.x;
     const int quads = C / 4, slots = kGnThreads / quads;
     const int q = threadIdx.x % quads, s = threadIdx.x / quads;
     const int p0 = ck * chunk_px, p1 = min(HW, p0 + chunk_px);
+    const float *xi = x + (size_t)img * HW * C;
     float sm[4] = {0.f, 0.f, 0.f, 0.f}, sq[4] = {0.f, 0.f, 0.f, 0.f};
     if (s < slots) {
+        const float4 pv = __ldg(reinterpret_cast<const float4 *>(xi + (size_t)p0 * C) + q);
+        if (s == 0) { piv[4 * q] = pv.x; piv[4 * q + 1] = pv.y; piv[4 * q + 2] = pv.z; piv[4 * q + 3] = pv.w; }
         for (int p = p0 + s; p < p1; p += slots) {
-            const float4 v = __ldg(reinterpret_cast<const float4 *>(x + ((size_t)img * HW + p) * C) + q);
-            sm[0] += v.x; sm[1] += v.y; sm[2] += v.z; sm[3] += v.w;
-            sq[0] += v.x * v.x; sq[1] += v.y * v.y; sq[2] += v.z * v.z; sq[3] += v.w * v.w;
+            const float4 v = __ldg(reinterpret_cast<const float4 *>(xi + (size_t)p * C) + q);
+            const float d[4] = {v.x - pv.x, v.y - pv.y, v.z - pv.z, v.w - pv.w};
+#pragma unroll
+            for (int e = 0; e < 4; e++) { sm[e] += d[e]; sq[e] += d[e] * d[e]; }
         }
     }
 #pragma unroll
@@ -50,10 +58,19 @@ __global__ void __launch_bounds__(kGnThreads) gn_stats_kernel(const float *__res
     }
     __syncthreads();
     if (threadIdx.x < kGroups) {
-        const int cpg = C / kGroups;
-        float a = 0.f, b = 0.f;
-        for (int c = threadIdx.x * cpg; c < (threadIdx.x + 1) * cpg; c++) { a += ch_sum[c].x; b += ch_sum[c].y; }
-        part[((size_t)img * nchunk + ck) * kGroups + threadIdx.x] = make_float2(a, b);
+        // channel c: mean_c = pivot_c + sum d / n, M2_c = sum d^2 - (sum d)^2 / n; the group's equal-count merge:
+        // mean = average of mean_c, M2 = sum M2_c + n sum (mean_c - mean)^2
+        const int cpg = C / kGroups, c0 = threadIdx.x * cpg;
+        const double n = (double)(p1 - p0), rn = 1.0 / n;
+        double mean = 0.0;
+        for (int c = c0; c < c0 + cpg; c++) mean += (double)piv[c] + (double)ch_sum[c].x * rn;
+        mean /= cpg;
+        double m2 = 0.0;
+        for (int c = c0; c < c0 + cpg; c++) {
+            const double a = ch_sum[c].x, dm = (double)piv[c] + a * rn - mean;
+            m2 += fmax((double)ch_sum[c].y - a * a * rn, 0.0) + n * dm * dm;
+        }
+        part[((size_t)img * nchunk + ck) * kGroups + threadIdx.x] = make_float2((float)mean, (float)m2);
     }
 }
 
@@ -64,17 +81,26 @@ __global__ void __launch_bounds__(kGnThreads) gn_apply_kernel(const float *__res
 {
     __shared__ float2 stat[kGroups];          // mean, rstd
     const int img = blockIdx.y, ck = blockIdx.x;
-    if (threadIdx.x < kGroups) {
-        double a = 0.0, b = 0.0;
-        for (int i = 0; i < nchunk; i++) {
-            const float2 v = part[((size_t)img * nchunk + i) * kGroups + threadIdx.x];
-            a += v.x; b += v.y;
+    {
+        // Chan's merge of the chunks' (mean, M2), chunk i holding n_i pixels of the group's cpg channels: lane j of
+        // the group's kGnMergeLanes takes chunks j, j + kGnMergeLanes, ...; the lanes' sums meet by xor shuffles
+        const int g = threadIdx.x / kGnMergeLanes, j = threadIdx.x % kGnMergeLanes;
+        const float2 *pg = part + (size_t)img * nchunk * kGroups + g;
+        double a = 0.0;
+        for (int i = j; i < nchunk; i += kGnMergeLanes) a += (double)min(chunk_px, HW - i * chunk_px) * pg[(size_t)i * kGroups].x;
+#pragma unroll
+        for (int o = 1; o < kGnMergeLanes; o <<= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+        const double mean = a / HW;
+        double b = 0.0;
+        for (int i = j; i < nchunk; i += kGnMergeLanes) {
+            const float2 v = pg[(size_t)i * kGroups];
+            const double d = v.x - mean;
+            b += v.y + (double)min(chunk_px, HW - i * chunk_px) * (C / kGroups) * d * d;
         }
-        const double n = (double)HW * (C / kGroups);
-        const double mean = a / n;
-        double var = b / n - mean * mean;
-        if (var < 0.0) var = 0.0;
-        stat[threadIdx.x] = make_float2((float)mean, (float)(1.0 / sqrt(var + (double)eps)));
+#pragma unroll
+        for (int o = 1; o < kGnMergeLanes; o <<= 1) b += __shfl_xor_sync(0xffffffffu, b, o);
+        const double var = b / ((double)HW * (C / kGroups));
+        if (j == 0) stat[g] = make_float2((float)mean, (float)(1.0 / sqrt(var + (double)eps)));
     }
     __syncthreads();
     const int quads = C / 4, cpg = C / kGroups;
@@ -319,6 +345,8 @@ static int conv_args(ConvArgs &a, const void *x, int n, int H, int W, int Cin, c
     if (!out_f32 && !out_bf16) return GA_ERR_BADARG;
     const int Ho = ga_conv3x3_out_size(H, stride), Wo = ga_conv3x3_out_size(W, stride);
     if (Ho <= 0 || Wo <= 0) return GA_ERR_BADARG;
+    // the epilogue reads residual and writes out_f32 as float2, out_bf16 as __nv_bfloat162
+    if (mis8(residual) || mis8(out_f32) || mis4(out_bf16)) return GA_ERR_BADARG;
     // stride 1: pad 1 on every side; stride 2: pad (0, 1, 0, 1), i.e. none on the top / left
     const int pad = stride == 1 ? 1 : 0;
     return conv_args_common(a, 3, x, n, H, W, Cin, Ho, Wo, w_packed, k_pitch, bias, Cout, stride, pad, pad, residual,
@@ -377,8 +405,9 @@ extern "C" int ga_group_norm_nhwc(const float *x, const float *gamma, const floa
                                   int silu, void *out, int out_bf16, void *scratch, size_t scratch_bytes, void *stream)
 {
     if (!x || !gamma || !beta || !out || !scratch || n <= 0 || HW <= 0) return GA_ERR_BADARG;
-    if (C % kGroups || C % 4 || C > 1024 || (C / kGroups) * kGroups != C) return GA_ERR_BADARG;
+    if (C <= 0 || C % kGroups || C % 4 || C > 1024) return GA_ERR_BADARG;
     if (C / 4 > kGnThreads) return GA_ERR_BADARG;
+    if (mis16(x) || (out_bf16 ? mis8(out) : mis16(out))) return GA_ERR_BADARG;      // float4 loads, float4 / uint2 stores
     if (scratch_bytes < ga_group_norm_scratch_bytes(n, HW)) return GA_ERR_WORKSPACE;
     const int cp = gn_chunk_px(HW), nchunk = (HW + cp - 1) / cp;
     cudaStream_t s = (cudaStream_t)stream;

@@ -494,6 +494,8 @@ extern "C" int ga_micro_attention_bf16(const void *qkv, const float *qn_w, const
                                        int H, float eps, void *stream)
 {
     if (!qkv || !qn_w || !kn_w || !out || S <= 0 || L <= 0 || L > kMicroL || H <= 0) return GA_ERR_BADARG;
+    // __nv_bfloat162 loads and stores; the small kernel reads the norm weights as float2
+    if (mis4(qkv) || mis4(out) || mis8(qn_w) || mis8(kn_w)) return GA_ERR_BADARG;
     static GaPerDevice attr_set;
     if (ga_first_use_on_device(attr_set)) {
         cudaError_t e = cudaFuncSetAttribute(micro_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,

@@ -261,7 +261,8 @@ int ga_layernorm_modulate(const float *x, const float *w, const float *bias, con
 int ga_thin_linear(const float *x, const float *ln_w, const float *ln_b, int apply_silu, const float *W,
                    const float *bias, float *y, int R, int D, int C, float eps, void *stream);
 /* attention over S sequences of L <= 16 tokens: qkv bf16 [S*L, 3*H*64] ("(K H D)" columns), q/k RMS-normalised per
- * head with weights qn_w / kn_w [64], softmax(q k^T / 8) v -> out bf16 [S*L, H*64] */
+ * head with weights qn_w / kn_w [64], softmax(q k^T / 8) v -> out bf16 [S*L, H*64].  qkv and out 4-byte, qn_w and
+ * kn_w 8-byte aligned. */
 int ga_micro_attention_bf16(const void *qkv, const float *qn_w, const float *kn_w, void *out, int S, int L, int H,
                             float eps, void *stream);
 /* seq [S, 1+f, D] fp32: row 0 = the parent token (prev_f == 0: parents[s]; else child s % prev_f of sequence
@@ -394,15 +395,18 @@ int ga_conv3x3_out_size(int H, int stride);
  * Cin % 8 == 0; w_packed bf16 [Cout, k_pitch], column (ky * 3 + kx) * Cin + c, zero beyond 9 * Cin, k_pitch >=
  * 9 * Cin rounded up to 64; Cout % 64 == 0.  stride 1: pad 1 on every side; stride 2: pad (0, 1, 0, 1) (the SD
  * Downsample).  out[m, :] = bias + conv (+ residual[m, :], fp32), m = (image, oy, ox) over [n, Ho, Wo]; written to
- * out_f32 and / or out_bf16 (either may be NULL, not both). */
+ * out_f32 and / or out_bf16 (either may be NULL, not both).  x and w_packed 16-byte, residual and out_f32 8-byte
+ * (float2), out_bf16 4-byte (__nv_bfloat162) aligned. */
 int ga_conv3x3_bf16(const void *x, int n, int H, int W, int Cin, const void *w_packed, int k_pitch,
                     const float *bias, int Cout, int stride, const float *residual, float *out_f32,
                     void *out_bf16, void *stream);
 /* Bytes of scratch ga_group_norm_nhwc needs for n images of HW pixels.  Host-only. */
 size_t ga_group_norm_scratch_bytes(int n, int HW);
-/* GroupNorm(32 groups) over x fp32 NHWC [n, HW, C] (statistics per image and group, fp32 partial sums folded in
- * fp64), * gamma + beta, then SiLU if silu != 0; out bf16 (out_bf16 != 0) or fp32, same layout.  C % 32 == 0,
- * C <= 1024.  Deterministic. */
+/* GroupNorm(32 groups) over x fp32 NHWC [n, HW, C] (statistics per image and group: per pixel chunk, fp32 sums of
+ * the values less the chunk's first pixel, formed into the chunk's (mean, M2) in fp64 and merged in fp64, so a
+ * group's |mean| / std costs no precision), * gamma + beta, then SiLU if silu != 0; out bf16 (out_bf16 != 0) or
+ * fp32, same layout.  0 < C <= 1024, C % 32 == 0.  x 16-byte aligned; out 16-byte (fp32) or 8-byte (bf16) aligned.
+ * Deterministic. */
 int ga_group_norm_nhwc(const float *x, const float *gamma, const float *beta, int n, int HW, int C, float eps,
                        int silu, void *out, int out_bf16, void *scratch, size_t scratch_bytes, void *stream);
 /* Farthest-point sampling, one CTA per sample: pcd fp32 [batch, N, 3], N <= 16384, K <= min(N, 1024).  Point 0 is
@@ -517,7 +521,8 @@ int ga_recon_metrics(const float *image, const float *depth, const float *alpha,
  * ---------------------------------------------------------------------------
  */
 /* ga_conv3x3_bf16 at stride 1 with no residual and a ReLU epilogue: out_bf16[m, :] = bf16(max(bias + conv, 0)),
- * fp32 up to the final rounding.  Same arguments and checks as ga_conv3x3_bf16 (bias may be NULL). */
+ * fp32 up to the final rounding.  Same arguments and checks as ga_conv3x3_bf16 (bias may be NULL; out_bf16 4-byte
+ * aligned). */
 int ga_conv3x3_relu_bf16(const void *x, int n, int H, int W, int Cin, const void *w_packed, int k_pitch,
                          const float *bias, int Cout, void *out_bf16, void *stream);
 /* The two images of n pairs, in0 and in1 fp32 NCHW [n, 3, H, W] each -> out bf16 NHWC [2n, H, W, 8] (16-byte
